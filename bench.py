@@ -3,7 +3,7 @@
 bench.py -- BASELINE.json's metric on BASELINE.json's configs.
 
     metric  : rows/sec of DT[:, sum(f.v), by(f.k)]  (groupby-sum) ...
-    config  : C2 = 1e9 rows, int32 key with 1e6 distinct values, float64 value, 1 x B200
+    config  : C2 = 1e9 rows, int32 key with 1e6 distinct values, float64 value, 1 x H100
               (N > 1: every rank owns its own 1e9-row partition -> weak scaling; the per-group
                partials are merged with an NCCL all-reduce of the dense per-key tables)
               ... "; sort HBM GB/s vs peak": C3 (1e9-row float64 sort -> RowIndex) and C4 (2-key
@@ -17,11 +17,14 @@ One "step" = one pass of the hot path over one batch:
     e2e      the public Frame API on pinned HOST columns: H2D of k and v, the query,
              D2H of the result frame, all inside the timed region
     roofline dominant kernel (radix scatter pass): algorithmic bytes / CUDA-event time
-    cpu_baseline   the reference itself (oracle/_ref, an unmodified build of /root/reference staged by
+    cpu_baseline   the reference itself (oracle/_ref, an unmodified build of the reference staged by
              oracle/build_ref.sh) or, where that is absent, the CPU oracle port, on a bounded sample,
              timed on this box's host cores
 
 `--impl reference` times the CPU implementation alone and prints the same line.
+`--dump-outputs DIR` writes what the last timed step computed (a fixed sample of the RowIndex, the
+Groupby offsets and the group sums) as DIR/<name>.npy; the inputs are seeded, so two builds can be
+compared output for output.
 """
 import argparse
 import json
@@ -46,7 +49,7 @@ def config_of(args, world):
     """The same dict in both arms (the driver compares them)."""
     return {"workload": WORKLOAD, "rows_per_gpu": args.rows, "groups": args.groups,
             "outputs": "RowIndex int32[n] + Groupby offsets int32[ng+1] + float64 sums[ng]",
-            "l2": "inputs (12 GB/GPU) exceed L2 (126 MB); no flush needed",
+            "l2": "inputs (12 GB/GPU) exceed L2 (50 MB); no flush needed",
             "parallelism": f"row-partitioned x{world}, NCCL all-reduce of the dense per-key partial tables" if world > 1 else "single GPU"}
 
 
@@ -65,7 +68,12 @@ def parse():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the C3 / C4 sub-records")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float64; a fixed sample of the RowIndex)")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    return args
 
 
 # ---------------------------------------------------------------------------
@@ -144,7 +152,7 @@ def cpu_groupby_sum(k, v, sort_new=False):
     if have_reference():
         if REF_DIR not in sys.path:
             sys.path.insert(0, REF_DIR)
-        import datatable as rdt                         # the reference, built unmodified from /root/reference
+        import datatable as rdt                         # the reference, built unmodified by oracle/build_ref.sh
         rdt.options.sort.new = bool(sort_new)
         try:
             DT = rdt.Frame(k=k, v=v)
@@ -228,7 +236,7 @@ def run_reference(args, rank, world):
         "cpu_baseline": {"value": value, "unit": UNIT, "cores": cores, "kind": kind,
                          "sample": f"{rows} rows of the C2 workload per step (uniform keys in [0,{args.groups})); {why}",
                          "rows_per_step": rows, "probes": probes,
-                         "implementation": ("h2oai/datatable built unmodified from /root/reference (oracle/build_ref.sh), "
+                         "implementation": ("h2oai/datatable built unmodified (oracle/build_ref.sh), "
                                             "default options (legacy SortContext path, nthreads = all cores)") if kind == "reference"
                                            else "oracle/dt_oracle.c (pthreads port of the reference's algorithm)"},
         "e2e": {"value": value, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
@@ -238,7 +246,7 @@ def run_reference(args, rank, world):
 
 
 # ---------------------------------------------------------------------------
-# the B200 arm
+# the GPU arm
 # ---------------------------------------------------------------------------
 def cuda_ms(torch, fn, reps):
     ts, r = [], None
@@ -247,6 +255,9 @@ def cuda_ms(torch, fn, reps):
         a.record(); r = fn(); b.record(); torch.cuda.synchronize()
         ts.append(a.elapsed_time(b))
     return sum(ts) / len(ts), r
+
+
+C4_MAX_ROWS = 250_000_000
 
 
 def other_configs(torch, engine, _lib, n, peak):
@@ -277,7 +288,11 @@ def other_configs(torch, engine, _lib, n, peak):
                  "key_bits": st["key_bits"], "radix_passes": st["radix_passes"], "check_sorted_nan_first": ok}
     del x
     torch.cuda.empty_cache()
-    # ---- C4: (int64, int32) keys, mean/min/max/count over 3 float64 columns
+    engine.set_option("trim_scratch", 1)                     # C3's sort scratch
+    # ---- C4: (int64, int32) keys, mean/min/max/count over 3 float64 columns.  Its inputs take 40 B/row and the
+    # bucketed reducers stage another 26 B/row: at most C4_MAX_ROWS rows, so that C4 fits 80 GB of HBM next to
+    # what the earlier legs leave cached.
+    n = min(n, C4_MAX_ROWS)
     k1 = torch.randint(0, 1000, (n,), generator=g, device="cuda", dtype=torch.int64) << 33
     k2 = torch.randint(0, 1000, (n,), generator=g, device="cuda", dtype=torch.int32)
     vs = [torch.randn(n, generator=g, device="cuda", dtype=torch.float64) for _ in range(3)]
@@ -350,8 +365,25 @@ def c5_record(torch, dist, engine, _lib, ddist, rank, world, steps=3):
             "groups_total": int(float(tsum[5])),
             "alltoall": {"bytes_sent_per_rank": bytes_max, "ms": x_ms,
                          "GBps_per_direction": bytes_max / (x_ms / 1e3) / 1e9 if x_ms > 0 else None,
-                         "nvlink5_peak_GBps_per_direction": 900.0},
+                         "nvlink4_peak_GBps_per_direction": 450.0},
             "check_sums_add_up": bool(ok), "steps": steps}
+
+
+DUMP_MAX_ELEMS = 1 << 20      # per array: with its sample positions at most 6 x 8 MB in all
+
+
+def dump_outputs(torch, out_dir, arrays):
+    """Writes every array as out_dir/<name>.npy in float64 (exact for the int32 RowIndex and offsets).  An array of
+    more than DUMP_MAX_ELEMS elements is replaced by a fixed sample (seeded by its length alone, so two builds
+    pick the same positions), and the positions go to out_dir/<name>_index.npy."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, x in arrays.items():
+        x = x.reshape(-1)
+        if x.numel() > DUMP_MAX_ELEMS:
+            pos = np.unique(np.random.default_rng(x.numel()).integers(0, x.numel(), DUMP_MAX_ELEMS))
+            np.save(os.path.join(out_dir, f"{name}_index.npy"), pos.astype(np.float64))
+            x = x[torch.from_numpy(pos).to(x.device)]
+        np.save(os.path.join(out_dir, f"{name}.npy"), x.to(torch.float64).cpu().numpy())
 
 
 def bind_to_gpu_numa_node(torch, local_rank):
@@ -406,9 +438,10 @@ def run_b200(args, rank, local_rank, world):
 
     local_ev = []             # N > 1: CUDA events around every rank's own group()+reduce (the part before the merge)
 
-    def step():
+    def step(keep=False):
         # group(): RowIndex int32[n] + Groupby offsets int32[ng+1], both left in HBM behind the handle,
-        # and the SUM reducer, evaluated inside the same engine call
+        # and the SUM reducer, evaluated inside the same engine call.  keep: return the open handle (closed by
+        # the caller once the outputs are dumped)
         if world > 1 and profiling[0]:
             le0 = torch.cuda.Event(enable_timing=True); le0.record()
         gb = engine.Groupby([k], [0], _lib.NA_FIRST, reducers=[(_lib.OP_SUM, v)])
@@ -423,8 +456,10 @@ def run_b200(args, rank, local_rank, world):
             launches[0] += 2
             gkeys, sums = ddist.merge_partials_dense(gkeys, sums, _lib.OP_SUM, key_range=(0, G - 1))   # dictionary-coded keys
             launches[0] += ddist.LAST_MERGE_LAUNCHES
-        gb.close()
-        return None, None, ng, sums
+        if not keep:
+            gb.close()
+            gb = None
+        return gb, None, ng, sums
 
     def barrier():
         if world > 1:
@@ -445,11 +480,17 @@ def run_b200(args, rank, local_rank, world):
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     barrier()
     ev0.record()
-    for _ in range(args.steps):
-        out = step()
+    for i in range(args.steps):
+        out = step(keep=bool(args.dump_outputs) and i == args.steps - 1)
     ev1.record()
     barrier()
     ms_total = ev0.elapsed_time(ev1)
+    # With --dump-outputs the last step's handle is closed here, after ev1: its close (an asynchronous free of the
+    # RowIndex and offsets) is left out of the timed region, the only difference to a run without the flag.
+    if out[0] is not None:
+        if rank == 0:
+            dump_outputs(torch, args.dump_outputs, {"order": out[0].order(), "offsets": out[0].offsets(), "sums": out[3]})
+        out[0].close()
     clocks = sampler.stop() if rank == 0 else None
     engine.set_option("profile", 0)
     profiling[0] = False
@@ -490,7 +531,7 @@ def run_b200(args, rank, local_rank, world):
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
     fam = {}
     for name, ms in main_prof:
         fam.setdefault(name, []).append(ms)
@@ -682,12 +723,14 @@ def run_b200(args, rank, local_rank, world):
             line["other_configs"] = {"C5": c5, "C2_strong": strong}
 
     # ---- the drop-in number: the PATCHED reference's own query with the engine options off / on -----
-    patched = os.path.join(ROOT, "integration", "_ref_patched")
+    patched = os.path.join(ROOT, "oracle", "_ref", "patched")
     if rank == 0 and world == 1 and not args.no_extra and os.path.exists(os.path.join(patched, "datatable", "__init__.py")):
         torch.cuda.empty_cache()
         engine.set_option("trim_scratch", 1)
         try:
-            env = dict(os.environ, PYTHONPATH=patched)
+            lib = os.path.join(ROOT, "datatable_b200", "lib")           # the patched extension links libdtb200.so
+            env = dict(os.environ, PYTHONPATH=patched,
+                       LD_LIBRARY_PATH=os.pathsep.join(p for p in (lib, os.environ.get("LD_LIBRARY_PATH")) if p))
             r = subprocess.run([sys.executable, os.path.join(ROOT, "integration", "bench_hook.py")], env=env,
                                capture_output=True, text=True, timeout=600)
             js = [ln for ln in r.stdout.splitlines() if ln.startswith("{")]

@@ -1,8 +1,8 @@
 """
-datatable_b200 -- B200-native groupby/sort engine behind h2oai/datatable's
+datatable_b200 -- H100-native groupby/sort engine behind h2oai/datatable's
 DT[i, j, by(), sort()] hot path.  See DESIGN.md / INTEGRATION.md.
 
-Importing this package loads libdtb200.so (sm_100a CUDA); it raises if the
+Importing this package loads libdtb200.so (sm_90a CUDA); it raises if the
 library has not been built.  There is no CPU fallback.
 """
 from . import _lib

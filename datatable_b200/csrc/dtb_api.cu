@@ -69,7 +69,7 @@ void prof_end(cudaStream_t s) {
 }
 
 // Lazy: the calls only record events; the first query (dtb_profile_count / _reset) waits for them.  (A sync at the
-// end of every profiled call kept the host from running ahead and cost ~0.4 ms per C2 step in bench.py's timed region.)
+// end of every profiled call kept the host from running ahead and lengthened bench.py's timed steps.)
 static void prof_collect() {
   for (auto& r : t_prof_open) {
     float ms = 0.f;
@@ -117,8 +117,8 @@ static int ensure_context() {
     set_error(std::string("no usable CUDA device: ") + cudaGetErrorString(e));
     return DTB_ECUDA;
   }
-  if (prop.major != 10) {
-    set_error("dtb200 is built for sm_100a (B200) only; device is sm_" + std::to_string(prop.major) +
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("dtb200 is built for sm_90a (H100) only; device is sm_" + std::to_string(prop.major) +
               std::to_string(prop.minor));
     return DTB_ECUDA;
   }
@@ -1002,6 +1002,14 @@ int dtb_set_option(const char* name, int64_t value) {
       if (cur != t_arena.device) cudaSetDevice(t_arena.device);
       t_arena.trim();
       if (cur != t_arena.device) cudaSetDevice(cur);
+    }
+    // handles' RowIndex / offsets / results come from the device's stream-ordered pool, which keeps what they
+    // freed (release threshold = max): give that back too, so that one large call can use the whole HBM
+    int dev = 0;
+    cudaMemPool_t pool;
+    if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
+      DTB_CUDA_CHECK(cudaDeviceSynchronize());
+      DTB_CUDA_CHECK(cudaMemPoolTrimTo(pool, 0));
     }
     return DTB_OK;
   }

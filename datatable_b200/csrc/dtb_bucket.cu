@@ -5,7 +5,7 @@
 // pass per reducer per column (column/latent.cc:103-135 materialising sumprod.h / mean.h / minmax.h /
 // count.h one after the other: 12 passes for BASELINE config C4) -- and this engine's own first
 // version, which streamed the rows once per reducer and folded them with L2 atomics (1-2 per row and
-// reducer: 15e9 atomics at ~190 G/s = the 100 ms of C4's 122 ms in round 1).
+// reducer: 15e9 atomics for C4 at 1e9 rows).
 //
 // When the normalised group key x spans 2^12 .. 2^20 values and no key is hot:
 //   count    : rows per bucket, bucket = x >> 11 (<= 512 buckets of 2048 consecutive keys)      [once per call]
@@ -31,19 +31,19 @@ constexpr int BK_KEYS = 1 << BK_BITS;
 constexpr int BK_MAXB = 512;                      // buckets: group key domain <= 2^20
 constexpr int BK_THREADS = 512;                   // = BK_MAXB: thread t owns bucket t in the tile scan
 constexpr int BK_IPT = 8;                         // (16 rows x 256 threads ran at 24 % occupancy: 48 registers of row
-constexpr int BK_TILE = BK_THREADS * BK_IPT;      //  state per thread; profiles/r2_c4_launches_1e9.txt) 4096 rows per tile
+constexpr int BK_TILE = BK_THREADS * BK_IPT;      //  state per thread) 4096 rows per tile
 constexpr int64_t BK_CHUNK = 262144;              // rows per aggregate CTA
 
 static inline int bk_grid(int64_t n, int threads) {
   const int64_t want = (n + threads - 1) / threads;
-  return (int)(want > NUM_SMS_B200 * 16 ? NUM_SMS_B200 * 16 : (want < 1 ? 1 : want));
+  return (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : (want < 1 ? 1 : want));
 }
 
 // ---- rows per (slab, bucket) -> start[slab][bucket] ------------------------------------------------
 // A slab is a contiguous range of tiles.  Every slab gets its own output range inside every bucket
 // (buckets stay contiguous: slab 0's rows, then slab 1's, ...), so that the scatter tiles of one slab
 // reserve their runs from a cursor only they share: with ONE cursor per bucket the 244 k tiles of a 1e9-row
-// column issued 244 k same-address L2 atomics-with-return per bucket (7.4 ms per column, LSU half idle).
+// column issued 244 k same-address L2 atomics-with-return per bucket (the LSUs sat half idle).
 __global__ void __launch_bounds__(512)
 bucket_count_kernel(const u32* __restrict__ xkeys, int gshift, int64_t n, int64_t slab_rows, u32* __restrict__ hist /*[nslabs][BK_MAXB]*/)
 {
@@ -84,7 +84,7 @@ bucket_scan_kernel(u32* __restrict__ hist /*in: counts, out: starts*/, int nslab
 
 int64_t bucket_slab_rows(int64_t n) {
   // ~4 slabs per SM, whole tiles per slab
-  int64_t r = (n + NUM_SMS_B200 * 4 - 1) / (NUM_SMS_B200 * 4);
+  int64_t r = (n + NUM_SMS * 4 - 1) / (NUM_SMS * 4);
   r = (r + BK_TILE - 1) / BK_TILE * BK_TILE;
   return r < BK_TILE ? BK_TILE : r;
 }
@@ -107,7 +107,7 @@ int launch_bucket_starts(const u32* xkeys, int gshift, int64_t n, int nb, u32* h
 // All the value columns of a sweep share one rank: the rows' tile slots are computed once (shared-memory
 // counters, one reservation per (tile, bucket)), xlow is written once, and every column is then staged
 // through the same shared-memory buffer and written out in bucket runs.  (One launch per column repeated the
-// rank for every column: 7.5 ms per float64 column at 1e9 rows, profiles/r2_c4_launches_1e9.txt.)
+// rank for every column.)
 struct BucketCols {
   int ncols;
   int esz[BK_MAXCOLS];
@@ -149,7 +149,7 @@ __device__ __forceinline__ void bucket_write_column(void* v_out, const unsigned 
 
 // The next column's values are loaded into registers before the staged column is written out, and the
 // columns alternate between two staging buffers: one barrier per column (2 CTAs and 2 x 80 KB per SM;
-// 3 CTAs of 40 registers without the prefetch: 15.4 instead of 14.7 ms for C4's three columns).
+// 3 CTAs of 40 registers without the prefetch measured slower).
 template <int TH, int IP>
 __global__ void __launch_bounds__(TH, 2048 / TH > 2 ? 2 : 2048 / TH)
 bucket_scatter_kernel(const u32* __restrict__ xkeys, int gshift, int64_t n, int64_t slab_rows,
@@ -235,16 +235,16 @@ bucket_scatter_kernel(const u32* __restrict__ xkeys, int gshift, int64_t n, int6
 // rows are counting-sorted by their 11-bit key in shared memory (one native 32-bit shared-memory atomic per
 // row hands out the rank, one scattered store places the value); thread t then owns keys 4t..4t+3, whose rows
 // are now contiguous, and folds them into REGISTER accumulators: every requested word (int sum, float sum,
-// count, min, max, NA count) at once, no 64-bit shared-memory atomics (they are CAS loops on sm_100:
+// count, min, max, NA count) at once, no 64-bit shared-memory atomics (they compile to CAS loops:
 // ATOMS.CAST.SPIN -- the first version of this kernel spent 1.85 LSU wavefronts per row in them), and the
 // valid-row count falls out of the walk.  The registers are flushed once per (chunk, bucket).
 struct BucketAcc { u64* w[BK_NWORDS]; };        // global accumulator tables, indexed by group key x (NULL = not requested)
 
 constexpr int BK_KPT = BK_KEYS / BK_THREADS;                  // 4 keys per thread
 
-constexpr int BK_AIPT = 16;                                   // rows per thread and tile (8: 7.3 ms per float64 column
-constexpr int BK_ATILE = BK_THREADS * BK_AIPT;                //  at 1e9 rows against 6.0 ms; re-reading the keys in the
-                                                              //  place phase to save registers: 8.1 ms)
+constexpr int BK_AIPT = 16;                                   // rows per thread and tile (8 rows, and re-reading
+constexpr int BK_ATILE = BK_THREADS * BK_AIPT;                //  the keys in the place phase to save registers,
+                                                              //  both measured slower)
 template <typename T>
 __global__ void __launch_bounds__(BK_THREADS, 2)
 bucket_aggregate_kernel(const unsigned short* __restrict__ xlow, const typename RawKey<T>::load_t* __restrict__ v,
@@ -398,7 +398,7 @@ int launch_bucketed_reduce(const u32* xkeys, int gshift, int dbits, int ncols, c
   const unsigned tiles = (unsigned)((n + BK_TILE - 1) / BK_TILE);
   const int stage_bytes = maxb * BK_TILE;
   const size_t sm_scatter = (size_t)4 * BK_TILE + (size_t)stage_bytes * (ncols > 1 ? 2 : 1);
-  // 1024 threads x 4 rows: 32 registers, two CTAs = every warp slot of the SM (512 x 8 at 64 registers: 14.6 instead of 14.1 ms)
+  // 1024 threads x 4 rows: 32 registers, two CTAs = every warp slot of the SM (512 x 8 at 64 registers measured slower)
   DTB_CUDA_CHECK(cudaFuncSetAttribute(bucket_scatter_kernel<1024, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 20 * BK_TILE));
   prof_begin("bucket_scatter", s);
   bucket_scatter_kernel<1024, 4><<<tiles, 1024, sm_scatter, s>>>(xkeys, gshift, n, slab_rows, cursor, xlow, cols, stage_bytes);

@@ -1,4 +1,4 @@
-// dtb_common.cuh -- device-side helpers shared by all kernels (sm_100a only).
+// dtb_common.cuh -- device-side helpers shared by all kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,7 +7,7 @@
 
 namespace dtb {
 
-constexpr int NUM_SMS_B200 = 148;
+constexpr int NUM_SMS = 132;                  // H100 SXM
 
 // radix pass geometry (dtb_radix.cu; the fused statistics kernel of dtb_stats.cu counts by the same tiles)
 constexpr int PASS_THREADS = 256;
@@ -95,7 +95,7 @@ __device__ __forceinline__ u64 norm_load_dynamic(const KeyNorm& k, int64_t i) {
 // ---- key sources for the radix kernels ---------------------------------------
 // load_raw / norm are split so that a kernel can issue all the loads of a tile before it touches any of
 // them (with load() alone ptxas reused one register for the raw element and serialised the 16 loads of
-// the scatter pass behind one another: +2.3 ms per 1e9 int32 rows).
+// the scatter pass behind one another).
 template <typename KeyT>
 struct PackedSrc {
   typedef KeyT raw_t;

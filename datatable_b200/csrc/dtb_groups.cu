@@ -145,7 +145,7 @@ int launch_mark_heads(const void* sorted_keys, int key_bytes, int group_shift, i
 {
   if (n == 0) return DTB_OK;
   int64_t want = (n + 255) / 256;
-  int grid = (int)(want > NUM_SMS_B200 * 16 ? NUM_SMS_B200 * 16 : want);
+  int grid = (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : want);
   if (key_bytes == 4) mark_heads_kernel<u32><<<grid, 256, 0, s>>>((const u32*)sorted_keys, group_shift, n, flags);
   else                mark_heads_kernel<u64><<<grid, 256, 0, s>>>((const u64*)sorted_keys, group_shift, n, flags);
   count_launch();
@@ -329,7 +329,7 @@ int launch_dense_scatter(const void* keys, int key_bytes, const void* vals, int6
                          void* table, uint32_t* present, cudaStream_t s)
 {
   if (n == 0) return DTB_OK;
-  const int grid = (int)((n + 255) / 256 > NUM_SMS_B200 * 8 ? NUM_SMS_B200 * 8 : (n + 255) / 256);
+  const int grid = (int)((n + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (n + 255) / 256);
   if (key_bytes == 4) dense_scatter_kernel<int32_t><<<grid, 256, 0, s>>>((const int32_t*)keys, (const u64*)vals, n, kmin, size, (u64*)table, present);
   else                dense_scatter_kernel<int64_t><<<grid, 256, 0, s>>>((const int64_t*)keys, (const u64*)vals, n, kmin, size, (u64*)table, present);
   count_launch();
@@ -341,7 +341,7 @@ int launch_dense_emit(const uint32_t* gidx, const void* table, int64_t ng, int64
                       void* out_keys, void* out_vals, cudaStream_t s)
 {
   if (ng == 0) return DTB_OK;
-  const int grid = (int)((ng + 255) / 256 > NUM_SMS_B200 * 8 ? NUM_SMS_B200 * 8 : (ng + 255) / 256);
+  const int grid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
   if (key_bytes == 4) dense_emit_kernel<int32_t><<<grid, 256, 0, s>>>(gidx, (const u64*)table, ng, kmin, (int32_t*)out_keys, (u64*)out_vals);
   else                dense_emit_kernel<int64_t><<<grid, 256, 0, s>>>(gidx, (const u64*)table, ng, kmin, (int64_t*)out_keys, (u64*)out_vals);
   count_launch();

@@ -22,7 +22,7 @@ namespace dtb {
 
 static inline int grid_for(int64_t n, int threads = 256) {
   const int64_t want = (n + threads - 1) / threads;
-  return (int)(want > NUM_SMS_B200 * 16 ? NUM_SMS_B200 * 16 : (want < 1 ? 1 : want));
+  return (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : (want < 1 ? 1 : want));
 }
 
 // raw element -> (valid, double) / (valid, order-preserving u64 image) ------------------------

@@ -15,7 +15,7 @@
 //
 // No look-back, no status words, no spinning: a first version used single-sweep tiles with
 // a decoupled look-back; with ~600 tiles in flight the look-back walk was 40 % of the stall
-// samples and 31 % of the instructions of the pass (profiles/r1_ncu_summary.md).  The price
+// samples and 31 % of the instructions of the pass.  The price
 // is one extra read of the keys per pass (K of 2(K+4) bytes per row).
 //
 // Stability (ties keep ascending row index, sort.cc:27-33): chunks and tiles are in row
@@ -34,8 +34,7 @@ namespace dtb {
 // Composite key materialisation (multi-column keys)
 // ===========================================================================
 // Four rows per thread and column: the stype switch is taken once per four rows and the four loads of a
-// column are in flight together (one row per thread cost 104 instructions per row: 5.2 ms for C4's two key
-// columns at 1e9 rows, profiles/r2_c4_launches_1e9.txt).
+// column are in flight together (one row per thread cost 104 instructions per row).
 template <typename T>
 __device__ __forceinline__ void compose_col4(const KeyNorm& k, const int64_t (&row)[4], const bool (&in)[4], u64 (&x)[4]) {
   typedef typename RawKey<T>::load_t L;
@@ -84,7 +83,7 @@ int launch_compose_keys(const KeyPlan& kp, int64_t n, const int32_t* idx, void* 
 {
   if (n == 0) return DTB_OK;
   int64_t want = (n + 1023) / 1024;
-  int grid = (int)(want > NUM_SMS_B200 * 16 ? NUM_SMS_B200 * 16 : want);
+  int grid = (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : want);
   if (key_bytes == 4) compose_keys_kernel<u32><<<grid, 256, 0, s>>>(kp, n, idx, (u32*)keys_out);
   else                compose_keys_kernel<u64><<<grid, 256, 0, s>>>(kp, n, idx, (u64*)keys_out);
   count_launch();
@@ -96,9 +95,8 @@ int launch_compose_keys(const KeyPlan& kp, int64_t n, const int32_t* idx, void* 
 // Pass geometry
 // ===========================================================================
 // Digits are at most 8 bits (256 bins).  Wider digits were built and measured twice and removed: round 1, two
-// 10-bit ballot-ranked passes over 1024 bins: 24 ms against 19 ms for three 7/7/6-bit passes on 20-bit keys at
-// n = 1e9; round 2, 1024/2048 bins ranked with shared-memory atomics: 17 ms of scatter against 11 ms
-// (profiles/r2_exp_b_wide_digits.log) -- 16-byte output runs and 16-32 KB of per-warp tables cost more LSU
+// 10-bit ballot-ranked passes over 1024 bins, slower than three 7/7/6-bit passes on 20-bit keys; round 2,
+// 1024/2048 bins ranked with shared-memory atomics, slower scatter -- 16-byte output runs and 16-32 KB of per-warp tables cost more LSU
 // wavefronts than the pass they save.
 // PASS_THREADS / PASS_IPT / PASS_TILE (4096 rows) / CHUNK_TILES / CHUNK_ROWS (65536 rows per count CTA): dtb_common.cuh
 
@@ -195,7 +193,7 @@ __global__ void __launch_bounds__(256)
 chunk_scan_kernel(u32* __restrict__ counts, int64_t nchunks, int nbins, u32* __restrict__ total)
 {
   // one CTA per digit walks the chunks, 1024 per round: every thread owns four consecutive chunks (four strided
-  // loads in flight; one chunk per thread and round took 60 dependent rounds for 1e9 rows: 0.08 ms per pass)
+  // loads in flight; one chunk per thread and round took 60 dependent rounds for 1e9 rows)
   __shared__ u32 wsum[8];
   __shared__ u32 s_carry;
   const int d = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
@@ -380,9 +378,9 @@ __device__ __forceinline__ void scatter_tile(const PassArgs<KeyT, Src>& a, unsig
   // (peers = AND over the bits of "lanes whose bit equals mine"), NB = digit width of the pass: no
   // shared-memory traffic, and the cost does not depend on how the digits are distributed.
   // Measured against a shared-memory atomicOr on a per-warp mask table (one word per digit): C2 scatter
-  // passes 13.3 -> 11.9 ms, float64 sort -11 %; a hot digit made the atomicOr form serialise on one word.
-  // Never MATCH.ANY: on sm_100 it issues once per ~60 SM cycles and bound the whole kernel
-  // (scripts/ubench/match_bench.cu).
+  // passes and the float64 sort got faster; a hot digit made the atomicOr form serialise on one word.
+  // Never MATCH.ANY: it issues far more slowly than a ballot and would bound the whole kernel
+  // (scripts/ubench/match_bench.cu measures it).
   u32 rank2[IPT / 2];                                         // two 16-bit ranks per register
   unsigned short* myhist = whist + warp * NBINS;
   const unsigned lt = lanemask_lt();
@@ -473,7 +471,7 @@ __device__ __forceinline__ void scatter_tile(const PassArgs<KeyT, Src>& a, unsig
 
 // key of the sorted tile's slot q (32-bit keys are staged as (key, row id) pairs)
 // (Staging the first pass of keys below 2^20 as one word per row, key << 12 | tile position -- a 4-byte
-// scattered store instead of an 8-byte one -- was measured: +0.2 ms on EVERY pass for the extra uniform
+// scattered store instead of an 8-byte one -- was measured slower on EVERY pass for the extra uniform
 // branch and registers, no gain on the first.)
 template <typename KeyT>
 __device__ __forceinline__ KeyT staged_key(const KeyT* skey, int q) {
@@ -692,7 +690,7 @@ __global__ void widen_u32_kernel(const u32* __restrict__ in, int64_t n, int64_t*
 int launch_widen_u32(const uint32_t* in, int64_t n, int64_t* out, cudaStream_t s) {
   if (n == 0) return DTB_OK;
   int64_t want = (n + 255) / 256;
-  int grid = (int)(want > NUM_SMS_B200 * 16 ? NUM_SMS_B200 * 16 : want);
+  int grid = (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : want);
   widen_u32_kernel<<<grid, 256, 0, s>>>(in, n, out);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
@@ -707,7 +705,7 @@ __global__ void iota32_kernel(int32_t* out, int64_t n) {
 int launch_iota32(int32_t* out, int64_t n, cudaStream_t s) {
   if (n == 0) return DTB_OK;
   int64_t want = (n + 255) / 256;
-  int grid = (int)(want > NUM_SMS_B200 * 16 ? NUM_SMS_B200 * 16 : want);
+  int grid = (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : want);
   iota32_kernel<<<grid, 256, 0, s>>>(out, n);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());

@@ -196,7 +196,7 @@ __global__ void fill_u64_kernel(u64* p, int64_t n, u64 v) {
 
 void fill_u64(unsigned long long* p, int64_t n, unsigned long long v, cudaStream_t s) {
   if (n <= 0) return;
-  const int g = (int)((n + 255) / 256 > NUM_SMS_B200 * 8 ? NUM_SMS_B200 * 8 : (n + 255) / 256);
+  const int g = (int)((n + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (n + 255) / 256);
   fill_u64_kernel<<<g, 256, 0, s>>>(p, n, v);
   count_launch();
 }
@@ -330,7 +330,7 @@ int launch_reduce_impl(int op, const void* value, int stype, int64_t nv, const v
   const int out_st = reduce_out_stype(op, stype);
   if (!out_st) { set_error("Invalid column type in reducer"); return DTB_EINVAL; }
   if (ng == 0) return DTB_OK;
-  const int fgrid = (int)((ng + 255) / 256 > NUM_SMS_B200 * 8 ? NUM_SMS_B200 * 8 : (ng + 255) / 256);
+  const int fgrid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
   if (op >= DTB_OP_FIRST && op <= DTB_OP_NUNIQUE) {
     // within-group ordered reducers (dtb_next.cu): they walk the ARR32 RowIndex
     if (order_is64) { set_error("first/last/sd/median/nunique take an int32 RowIndex"); return DTB_ENOTIMPL; }
@@ -405,7 +405,7 @@ __global__ void offsets_check_kernel(const int32_t* __restrict__ offsets, int64_
 
 int launch_offsets_check(const int32_t* offsets, int64_t ng, int* d_bad, cudaStream_t s) {
   if (ng == 0) return DTB_OK;
-  const int fgrid = (int)((ng + 255) / 256 > NUM_SMS_B200 * 8 ? NUM_SMS_B200 * 8 : (ng + 255) / 256);
+  const int fgrid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
   offsets_check_kernel<<<fgrid, 256, 0, s>>>(offsets, ng, d_bad);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
@@ -414,7 +414,7 @@ int launch_offsets_check(const int32_t* offsets, int64_t ng, int* d_bad, cudaStr
 
 int launch_nrows(const int32_t* offsets, int64_t ng, void* out, cudaStream_t s) {
   if (ng == 0) return DTB_OK;
-  const int fgrid = (int)((ng + 255) / 256 > NUM_SMS_B200 * 8 ? NUM_SMS_B200 * 8 : (ng + 255) / 256);
+  const int fgrid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
   nrows_kernel<<<fgrid, 256, 0, s>>>(offsets, ng, (int64_t*)out);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
@@ -427,12 +427,12 @@ int launch_nrows(const int32_t* offsets, int64_t ng, void* out, cudaStream_t s) 
 // When the group key of a row can be computed from the key columns alone -- the normalised
 // composite key x = X(row) >> group_shift spans at most 2^22 values -- the reducers do not
 // need the RowIndex at all: rows are streamed in storage order (coalesced, no gather), and
-// each row folds its value into acc[x] with one L2 atomic.  The table (<= 32 MB) stays
-// resident in the 126 MB L2.  Rows of a warp that share x are combined first
+// each row folds its value into acc[x] with one L2 atomic.  One table (<= 32 MB) fits the
+// 50 MB L2 of an H100.  Rows of a warp that share x are combined first
 // (__match_any_sync) so that hot keys do not serialise on one address.  A finalize kernel
 // maps group g -> acc[gkeys[g]] and applies the reference's output stype / NA rules.
 //
-// Bound: L2 atomic throughput (measured 170 G atomics/s on B200), then HBM.
+// Bound: L2 atomic throughput, then HBM.
 // Algorithmic bytes per row: key column(s) + value column, read once.
 struct HotSpec {            // "may one key own a large share of the rows?"
   const u32* count;         // device: largest digit count of the first pass (NULL = use `value`)
@@ -458,7 +458,7 @@ direct_reduce_kernel(KSrc ksrc, int gshift, const typename RawKey<T>::load_t* __
       p_add<T, CAT>(part, v[i], true, flag);
     }
     // HOT: a key may own a large share of the rows (skewed digit histograms): fold equal keys of the
-    // warp before touching L2.  MATCH.ANY is slow on sm_100 (~60 SM cycles per warp), so the
+    // warp before touching L2.  MATCH.ANY is a slow, multi-cycle warp instruction, so the
     // common spread-out case skips it entirely.
     const unsigned peers = HOT ? __match_any_sync(0xffffffffu, x) : (1u << lane);
     if (HOT && __any_sync(0xffffffffu, peers != (1u << lane))) {  // warp-uniform: the body shuffles
@@ -550,7 +550,7 @@ __device__ __forceinline__ void slot_flush(u64 a0, u64 a1, int64_t g, u64* acc0,
 
 // Few distinct group keys (<= 2048): every CTA folds its rows into a shared-memory copy of the
 // accumulator table and flushes it once, so the L2 sees gridDim x groups atomics instead of one per row
-// (100 keys at 2e8 rows: 1.6e8 same-address L2 atomics took 30 ms; low-cardinality by() is the common case).
+// (100 keys at 2e8 rows = 1.6e8 same-address L2 atomics; low-cardinality by() is the common case).
 constexpr int SMALL_TABLE = 2048;
 
 template <typename T, int CAT, typename KSrc>
@@ -594,8 +594,7 @@ direct_reduce_small_kernel(KSrc ksrc, int gshift, const typename RawKey<T>::load
 }
 
 // Skewed group sizes (some key owns more than ~0.1 % of the rows): one L2 atomic per row would
-// serialise on the hot accumulators (same-address L2 atomics retire at one per 5-15 ns: a key with
-// half of 2e8 rows cost 16 ms).  `hot[x]` (built from the group sizes, see plan_direct) marks the
+// serialise on the hot accumulators (same-address L2 atomics retire one at a time).  `hot[x]` (built from the group sizes, see plan_direct) marks the
 // keys above the threshold; their rows are folded inside the warp (MATCH.ANY, only in warps that hold
 // a hot row) and then inside the CTA in a small open-addressed shared-memory table that is flushed
 // once per CTA; every other row takes the plain one-atomic path.
@@ -673,7 +672,7 @@ static int run_direct(const KSrc& ks, int gshift, const void* v, int64_t n, u64*
   typedef typename RawKey<T>::load_t L;
   int64_t want = (n + 511) / 512;
   if (t_dp.kind == DIRECT_SMALL) {
-    int grid = (int)(want > NUM_SMS_B200 * 4 ? NUM_SMS_B200 * 4 : want);
+    int grid = (int)(want > NUM_SMS * 4 ? NUM_SMS * 4 : want);
     direct_reduce_small_kernel<T, CAT, KSrc><<<grid, 512, 0, s>>>(ks, gshift, (const L*)v, n, (int)t_dp.nslots,
                                                                   (const uint16_t*)t_dp.map, acc0, acc1, flag);
     count_launch();
@@ -681,7 +680,7 @@ static int run_direct(const KSrc& ks, int gshift, const void* v, int64_t n, u64*
     return DTB_OK;
   }
   if (t_dp.kind == DIRECT_HOT) {
-    int grid = (int)(want > NUM_SMS_B200 * 4 ? NUM_SMS_B200 * 4 : want);
+    int grid = (int)(want > NUM_SMS * 4 ? NUM_SMS * 4 : want);
     direct_reduce_hot_kernel<T, CAT, KSrc><<<grid, 512, 0, s>>>(ks, gshift, (const L*)v, n, (const uint8_t*)t_dp.map,
                                                                 acc0, acc1, flag);
     count_launch();
@@ -690,7 +689,7 @@ static int run_direct(const KSrc& ks, int gshift, const void* v, int64_t n, u64*
   }
   HotSpec hs = {nullptr, 0, 0};
   if (t_dp.kind == DIRECT_DEVICE_HOT) { hs.count = t_dp.hot_count; hs.thresh = t_dp.hot_thresh; }
-  int grid = (int)(want > NUM_SMS_B200 * 16 ? NUM_SMS_B200 * 16 : want);
+  int grid = (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : want);
   direct_reduce_kernel<T, CAT, KSrc><<<grid, 512, 0, s>>>(ks, gshift, (const L*)v, n, acc0, acc1, flag, hs);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
@@ -769,7 +768,7 @@ int plan_direct(int64_t table, const uint32_t* gkeys, const int32_t* offsets, in
   if (gmax > hot_at) {
     const int64_t key_thresh = (n / 2048 > 1024) ? n / 2048 : 1024;  // at most 2048 keys can exceed it
     DTB_CUDA_CHECK(cudaMemsetAsync(map_scratch, 0, (size_t)table, s));
-    const int grid = (int)((ng + 255) / 256 > NUM_SMS_B200 * 8 ? NUM_SMS_B200 * 8 : (ng + 255) / 256);
+    const int grid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
     hot_map_kernel<<<grid, 256, 0, s>>>(gkeys, offsets, ng, (u32)key_thresh, (uint8_t*)map_scratch);
     count_launch();
     DTB_CUDA_CHECK(cudaGetLastError());
@@ -794,7 +793,7 @@ int launch_direct_accumulate(int op, const KeyPlan& kp, const DirectPlan& dp,
 int launch_direct_init(int op, const DirectPlan& dp, int64_t table, u64* acc0, u64* acc1, cudaStream_t s)
 {
   if (dp.kind == DIRECT_SMALL) table = dp.nslots;                // only the used accumulators are initialised
-  const int tgrid = (int)((table + 255) / 256 > NUM_SMS_B200 * 8 ? NUM_SMS_B200 * 8 : (table + 255) / 256);
+  const int tgrid = (int)((table + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (table + 255) / 256);
   fill_u64_kernel<<<tgrid, 256, 0, s>>>(acc0, table, (op == DTB_OP_MIN) ? ~0ull : 0ull);
   count_launch();
   if (op == DTB_OP_MEAN) { fill_u64_kernel<<<tgrid, 256, 0, s>>>(acc1, table, 0ull); count_launch(); }
@@ -843,7 +842,7 @@ int launch_direct_finalize(int op, int stype, const u64* acc0, const u64* acc1, 
   const int out_st = reduce_out_stype(op, stype);
   if (!out_st) { set_error("Invalid column type in reducer"); return DTB_EINVAL; }
   if (ng == 0) return DTB_OK;
-  const int fgrid = (int)((ng + 255) / 256 > NUM_SMS_B200 * 8 ? NUM_SMS_B200 * 8 : (ng + 255) / 256);
+  const int fgrid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
   finalize_direct_kernel<<<fgrid, 256, 0, s>>>(op, stype, out_st, acc0, acc1, gkeys, ng, out);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
@@ -874,7 +873,7 @@ int launch_group_keys(const void* sorted_keys, int key_bytes, const int32_t* off
                       int64_t ng, uint32_t* gkeys, cudaStream_t s)
 {
   if (ng == 0) return DTB_OK;
-  const int grid = (int)((ng + 255) / 256 > NUM_SMS_B200 * 8 ? NUM_SMS_B200 * 8 : (ng + 255) / 256);
+  const int grid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
   if (key_bytes == 4) group_keys_kernel<u32><<<grid, 256, 0, s>>>((const u32*)sorted_keys, offsets, gshift, ng, gkeys);
   else                group_keys_kernel<u64><<<grid, 256, 0, s>>>((const u64*)sorted_keys, offsets, gshift, ng, gkeys);
   count_launch();
@@ -909,7 +908,7 @@ static int run_gather(const void* src, int64_t nsrc, const void* order, int orde
 {
   if (n == 0) return DTB_OK;
   int64_t want = (n + 1023) / 1024;
-  int grid = (int)(want > NUM_SMS_B200 * 16 ? NUM_SMS_B200 * 16 : want);
+  int grid = (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : want);
   if (order_is64) gather_kernel<E, int64_t><<<grid, 256, 0, s>>>((const E*)src, nsrc, (const int64_t*)order, n, (E*)out, na);
   else            gather_kernel<E, int32_t><<<grid, 256, 0, s>>>((const E*)src, nsrc, (const int32_t*)order, n, (E*)out, na);
   count_launch();

@@ -2,7 +2,7 @@
 // streaming read.  Replaces NumericStats<T>::compute_minmax (stats.cc:601-634),
 // which feeds the integer key normalisation (sort.cc:729-740).
 //
-// HBM-bound: 1 read of the column, 16-byte vector loads, grid = 148 SMs x 8.
+// HBM-bound: 1 read of the column, 16-byte vector loads, grid = 132 SMs x 8.
 // Algorithmic bytes per row: sizeof(T).
 // Single-column keys take col_stats_hist_kernel: the same statistics plus the first radix pass's histogram
 // (per 4096-row tile, low 8 bits of u) from the same read -- the pass then needs no count kernel.
@@ -11,7 +11,7 @@
 namespace dtb {
 
 // Per-thread accumulator.  Columns of at most 32 bits accumulate in 32-bit registers (the 64-bit
-// form costs twice the ALU work and kept the kernel at 58 % issue utilisation / 3.8 TB/s).
+// form costs twice the ALU work and kept the kernel below the HBM rate).
 template <typename T, bool IS_FLOAT, bool NARROW = Raw32<T>::ok>
 struct StatAcc;
 
@@ -217,7 +217,7 @@ static int run_stats(const void* data, int64_t n, ColStats* d_stats, cudaStream_
   } else if (n > 0) {
     const int threads = 512;
     int64_t want = (n / (16 / (int)sizeof(T)) + threads - 1) / threads;
-    int grid = (int)(want < 1 ? 1 : (want > NUM_SMS_B200 * 8 ? NUM_SMS_B200 * 8 : want));
+    int grid = (int)(want < 1 ? 1 : (want > NUM_SMS * 8 ? NUM_SMS * 8 : want));
     col_stats_kernel<T, IS_FLOAT><<<grid, threads, 0, s>>>(
         reinterpret_cast<const typename RawKey<T>::load_t*>(data), n, d_stats);
     count_launch();

@@ -125,6 +125,9 @@ def group(cols, flags=None, na_pos=NA_FIRST):
     return order, offs[:ng.value + 1], ng.value
 
 
+GROUP64_OFFSETS_GUESS = 1 << 24
+
+
 def group64(cols, flags=None, na_pos=NA_FIRST):
     """group() with the ARR64 layout (dtb_group64): int64 RowIndex and int64 Groupby offsets; for frames of
     more than INT32_MAX rows (up to 2^32 on one GPU) or callers that want 64-bit indices."""
@@ -139,13 +142,20 @@ def group64(cols, flags=None, na_pos=NA_FIRST):
     order, optr = _alloc(n, INT64, device)
     ng = ctypes.c_int64(-1)
     no = ctypes.c_int64(0)
-    if do_groups:
-        # the number of groups is not known in advance: a first sizing pass is avoided by allocating n + 1
-        offs, fptr = _alloc(n + 1, INT64, device)
-    else:
-        offs, fptr = None, 0
-    check(lib.dtb_group64(ckeys, nk, cflags, na_pos, n, _stream(), ctypes.c_void_p(optr),
-                          ctypes.c_void_p(fptr), n + 1 if do_groups else 0, ctypes.byref(ng), ctypes.byref(no)))
+    # The number of groups is not known in advance.  n + 1 int64 offsets would cost as much HBM as the RowIndex
+    # (16 GB past 2^31 rows), so the first call gets room for GROUP64_OFFSETS_GUESS groups; with more groups it
+    # reports DTB_ENOSPACE and their count, and the call is repeated with exactly sized offsets: a frame with more
+    # than 2^24 groups is sorted twice, the price of not holding n + 1 offsets for every call.
+    cap = min(n, GROUP64_OFFSETS_GUESS) + 1 if do_groups else 0
+    offs, fptr = _alloc(cap, INT64, device) if do_groups else (None, 0)
+    rc = lib.dtb_group64(ckeys, nk, cflags, na_pos, n, _stream(), ctypes.c_void_p(optr),
+                         ctypes.c_void_p(fptr), cap, ctypes.byref(ng), ctypes.byref(no))
+    if rc == _lib.ENOSPACE and do_groups and ng.value + 1 > cap:
+        cap = ng.value + 1
+        offs, fptr = _alloc(cap, INT64, device)
+        rc = lib.dtb_group64(ckeys, nk, cflags, na_pos, n, _stream(), ctypes.c_void_p(optr),
+                             ctypes.c_void_p(fptr), cap, ctypes.byref(ng), ctypes.byref(no))
+    check(rc)
     order = order[:no.value]
     if ng.value < 0:
         return order, None, None

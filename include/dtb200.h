@@ -1,11 +1,11 @@
 /*
- * dtb200.h -- C-ABI of the B200-native groupby/sort engine that sits behind
+ * dtb200.h -- C-ABI of the H100-native groupby/sort engine that sits behind
  * h2oai/datatable's DT[i, j, by(), sort()] hot path.
  *
  * The reference has no FFI seam on this path (SURVEY.md 8b): the boundary is
  * its internal C++ function group() and the materialize() of its reducer /
  * view columns.  Every entry point below names the reference interface it
- * replaces (paths relative to /root/reference/src/core/).  INTEGRATION.md
+ * replaces (paths relative to the reference's src/core/).  INTEGRATION.md
  * shows the reference-side binding.
  *
  * Conventions
@@ -355,15 +355,16 @@ DTB_API int dtb_memcpy(void* dst, const void* src, int64_t nbytes, dtb_stream st
  *                  concurrently with the sort passes (default 0: same stream, measured equally fast)
  *   "stage_keys"   0 (default) = the first count and scatter kernels of a single raw key column normalise it on
  *                  the fly (no normalised-key array is written); 1 = the first count kernel materialises the
- *                  normalised keys and the first scatter reads those (round-1 behaviour; measured at 1e9 rows:
- *                  +0.5 ms and +8 GB of DRAM traffic for int32 keys, +0.9 ms for float64)
+ *                  normalised keys and the first scatter reads those (round-1 behaviour: one more
+ *                  write and read of the keys)
  *   "fuse_stats_hist" 1 (default) = single-column keys: the statistics kernel also counts the low 8 bits of every
  *                  tile and the first radix pass folds that into its digit counts instead of reading the column
  *                  again (DESIGN.md 4.1); 0 = separate statistics and count kernels
  *   "bucketed_reducers" 1 (default) = value columns that would cost two or more L2 atomics per row (mean, or
  *                  several reducers of one column) take the bucketed multi-reducer (dtb_bucket.cu); 0 = always
  *                  one streaming pass per reducer
- *   "trim_scratch" (set only) release the calling thread's cached HBM scratch slab
+ *   "trim_scratch" (set only) release the calling thread's cached HBM scratch slab and the memory the current
+ *                  device's stream-ordered pool keeps from freed handles
  */
 DTB_API int dtb_set_option(const char* name, int64_t value);
 DTB_API int dtb_get_option(const char* name, int64_t* value);

@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """Applies the in-extension hook of INTEGRATION.md (B) to a SCRATCH COPY of the reference.
 
-    cp -r /root/reference /tmp/dthook
+    cp -r <reference source tree> /tmp/dthook
     python integration/apply_hook.py /tmp/dthook            # edits src/core/sort.cc and ci/ext.py
     (cd /tmp/dthook && python ci/ext.py build)              # the reference's own backend, ~2 min
     PYTHONPATH=/tmp/dthook/src python integration/check_hook.py
@@ -23,7 +23,7 @@ What it adds:
   * src/core/expr/eval_context.cc -- a residency bracket (dtb_cache_begin/end) around EvalContext::evaluate():
     host columns staged by group() / the reducers / the gathers of one query are uploaded once.
   * ci/ext.py         -- include path of include/dtb200.h, link + rpath of datatable_b200/lib/libdtb200.so.
-/root/reference itself is never touched.
+The reference's own tree is never touched.
 """
 import os
 import sys
@@ -31,7 +31,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 INCLUDE_ANCHOR = '#include "utils/misc.h"\n'
-INCLUDE_ADD = '#include <dtb200.h>      // B200 engine C-ABI (drop-in for group()); -I<repo>/include, see ci/ext.py\n'
+INCLUDE_ADD = '#include <dtb200.h>      // dtb200 engine C-ABI (drop-in for group()); -I<repo>/include, see ci/ext.py\n'
 
 OPTION_ANCHOR = 'static bool sort_new = false;\n'
 OPTION_ADD = ('static bool sort_b200 = false;   // option sort.b200: route group() through libdtb200\n'
@@ -109,7 +109,7 @@ RED_INCLUDE_ANCHOR = '#include "expr/workframe.h"\n'
 RED_INCLUDE_ADD = '''#include <cstring>
 #include "datatable.h"
 #include "stype.h"
-#include <dtb200.h>      // B200 engine C-ABI (reducers)
+#include <dtb200.h>      // dtb200 engine C-ABI (reducers)
 bool dtb200_reducers_enabled();   // sort.cc, option sort.b200_reducers
 '''
 
@@ -178,7 +178,7 @@ VIEW_H_ADD = '    void materialize(Column& out, bool to_memory) override;   // d
 
 VIEW_CC_INCLUDE_ANCHOR = '#include "column/view.h"\n'
 VIEW_CC_INCLUDE_ADD = '''#include "stype.h"
-#include <dtb200.h>      // B200 engine C-ABI (RowIndex gather)
+#include <dtb200.h>      // dtb200 engine C-ABI (RowIndex gather)
 bool dtb200_enabled();   // sort.cc, option sort.b200
 '''
 
@@ -214,14 +214,14 @@ void ArrayView_ColumnImpl<T>::materialize(Column& out, bool to_memory) {
 
 # ---- residency bracket: src/core/expr/eval_context.cc ---------------------------------------------------
 EVAL_INCLUDE_ANCHOR = '#include "expr/eval_context.h"\n'
-EVAL_INCLUDE_ADD = '''#include <dtb200.h>      // B200 engine C-ABI (residency bracket)
+EVAL_INCLUDE_ADD = '''#include <dtb200.h>      // dtb200 engine C-ABI (residency bracket)
 namespace { struct Dtb200CacheScope { Dtb200CacheScope() { dtb_cache_begin(); } ~Dtb200CacheScope() { dtb_cache_end(); } }; }
 '''
 EVAL_ANCHOR = 'py::oobj EvalContext::evaluate() {\n'
 EVAL_ADD = '  Dtb200CacheScope dtb200_cache_scope;   // host columns staged by the engine stay in HBM for this query\n'
 
 EXT_ANCHOR = '            ext.compiler.add_linker_flag("-lstdc++")\n'
-EXT_ADD = '''            # dtb200: B200 engine C-ABI
+EXT_ADD = '''            # dtb200: dtb200 engine C-ABI
             ext.compiler.add_compiler_flag("-I{inc}")
             ext.compiler.add_linker_flag("-L{lib}", "-ldtb200", "-Wl,-rpath,{lib}")
 '''
@@ -242,9 +242,10 @@ def insert(text, anchor, add, before, what):
 def main():
     if len(sys.argv) != 2:
         sys.exit(__doc__)
-    tree = os.path.abspath(sys.argv[1])
-    if tree.startswith("/root/reference"):
-        sys.exit("apply_hook: refusing to modify /root/reference; work on a scratch copy")
+    tree = os.path.realpath(sys.argv[1])
+    src = os.path.realpath(os.environ.get("DATATABLE_REFERENCE_SRC") or os.path.join(os.path.dirname(ROOT), "reference"))
+    if tree == src or tree.startswith(src + os.sep):
+        sys.exit(f"apply_hook: refusing to modify the reference's source tree {src}; work on a scratch copy")
     sort_cc = os.path.join(tree, "src", "core", "sort.cc")
     s = open(sort_cc).read()
     s = insert(s, INCLUDE_ANCHOR, INCLUDE_ADD, before=False, what="include")

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Times the PATCHED reference (integration/_ref_patched on PYTHONPATH): its own
+"""Times the PATCHED reference (oracle/_ref/patched on PYTHONPATH): its own
 DT[:, dt.sum(f.v), by(f.k)] on host Frames with the engine options off (stock CPU path) and on
 (group() -> dtb_group, sum -> dtb_reduce, residency bracket).  This is the drop-in end-to-end number:
 the user's code and the reference's Frame objects are unchanged, only `dt.options.sort.b200*` flip.

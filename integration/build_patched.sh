@@ -1,15 +1,18 @@
 #!/bin/sh
 # Builds the reference WITH the dtb200 hook from a scratch copy and stages the result (stripped) under
-# integration/_ref_patched/ (git-ignored).  Dev container only: needs /root/reference.
+# oracle/_ref/patched/ (git-ignored; travels with oracle/_ref).  Needs the reference's source tree:
+# $DATATABLE_REFERENCE_SRC, by default `reference` next to this repository.
 set -e
 HERE=$(cd "$(dirname "$0")" && pwd)
-SCRATCH=${1:-/tmp/dthook}
-rm -rf "$SCRATCH" && cp -r /root/reference "$SCRATCH"
+REF=${DATATABLE_REFERENCE_SRC:-$HERE/../../reference}
+OUT="$HERE/../oracle/_ref/patched"
+SCRATCH=${1:-${TMPDIR:-/tmp}/dthook}
+rm -rf "$SCRATCH" && cp -r "$REF" "$SCRATCH"
 python "$HERE/apply_hook.py" "$SCRATCH"
 (cd "$SCRATCH" && python ci/ext.py build > "$SCRATCH/build.log" 2>&1) || { tail -20 "$SCRATCH/build.log"; exit 1; }
-rm -rf "$HERE/_ref_patched" && mkdir -p "$HERE/_ref_patched"
-cp -r "$SCRATCH/src/datatable" "$HERE/_ref_patched/"
-find "$HERE/_ref_patched" -name __pycache__ -type d -prune -exec rm -rf {} +
-strip -g "$HERE"/_ref_patched/datatable/lib/_datatable*.so
-PYTHONPATH="$HERE/_ref_patched" python "$HERE/check_hook.py"
-PYTHONPATH="$HERE/_ref_patched" python "$HERE/check_hook_views.py"
+rm -rf "$OUT" && mkdir -p "$OUT"
+cp -r "$SCRATCH/src/datatable" "$OUT/"
+find "$OUT" -name __pycache__ -type d -prune -exec rm -rf {} +
+strip -g "$OUT"/datatable/lib/_datatable*.so
+PYTHONPATH="$OUT" python "$HERE/check_hook.py"
+PYTHONPATH="$OUT" python "$HERE/check_hook_views.py"

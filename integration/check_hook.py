@@ -3,7 +3,7 @@
 
 * option sort.b200 exists and defaults to False; with it off, results are the stock CPU results;
 * with it on, group() goes through libdtb200's dtb_group:
-    - on a box with a B200: the results must equal the stock CPU results (bit-exact RowIndex / offsets,
+    - on a box with a GPU: the results must equal the stock CPU results (bit-exact RowIndex / offsets,
       sums within 1e-6 relative);
     - on a box without a usable GPU (this build container): the engine's own error must surface as a
       datatable exception -- there is no CPU fallback inside the library, and unsupported column types

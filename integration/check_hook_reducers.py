@@ -1,9 +1,9 @@
 #!/usr/bin/env python3
 """Checks the reducer hook of a patched reference build (option sort.b200_reducers; run with
-PYTHONPATH=<scratch>/src or integration/_ref_patched).
+PYTHONPATH=<scratch>/src or oracle/_ref/patched).
 
 With the option on, sum/mean/min/max/count/countna of plain numeric columns go through dtb_reduce.
-* B200: results must equal the stock CPU results (ints/min/max/counts bit-exact, float sums/means 1e-6);
+* GPU: results must equal the stock CPU results (ints/min/max/counts bit-exact, float sums/means 1e-6);
   with sort.b200 on as well the whole DT[:, reducers, by(k)] runs on the engine.
 * no usable GPU: the engine's error must surface; reducers outside the engine's scope (prod, sd) and
   computed arguments (f.v * 2) must keep working through the reference's own columns.

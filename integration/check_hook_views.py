@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Checks the ArrayView gather hook and the residency bracket of a patched reference build
-(run with PYTHONPATH=integration/_ref_patched).
+(run with PYTHONPATH=oracle/_ref/patched).
 
 * option sort.b200 on: DT[:, :, sort(f.k)] -- the reference's group() through dtb_group, then the
   materialisation of every ArrayView column through dtb_gather -- must equal the stock CPU result.

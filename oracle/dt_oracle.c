@@ -8,13 +8,13 @@
  *
  * Parity status: PINNED.  tests/test_oracle_golden.py checks every function
  * here against fixtures under tests/golden/ that were produced by importing
- * the reference itself (built from /root/reference, commit 3611640) with
+ * the reference itself (built from its source tree, commit 3611640) with
  * tests/golden/make_golden.py, which also restates the reference's own
  * known-answer vectors (tests/ijby/test-sort.py, tests/test-groups.py,
  * tests/test-reduce.py).
  *
  * Each function cites the reference file:line it restates
- * (paths relative to /root/reference/src/core/).
+ * (paths relative to the reference's src/core/).
  *
  * Plain C99 + pthreads.  Single-threaded by default (the parity tests); orc_set_threads(T)
  * lets bench.py's CPU legs use the host's cores the way the reference does (its radix sort

@@ -17,9 +17,9 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _SO = os.path.join(_HERE, "liborc.so")
 
-# stype codes: /root/reference/src/datatable/include/datatable.h:32-42
+# stype codes: the reference's src/datatable/include/datatable.h:32-42
 BOOL, INT8, INT16, INT32, INT64, FLOAT32, FLOAT64 = 1, 2, 3, 4, 5, 6, 7
-# sort flags / NA position: /root/reference/src/core/sort.h:36-48
+# sort flags / NA position: the reference's src/core/sort.h:36-48
 DESCENDING, SORT_ONLY = 2, 4
 NA_FIRST, NA_LAST, NA_REMOVE = 1, 2, 3
 SUM, MEAN, MIN, MAX, COUNT, COUNTNA, NROWS = 1, 2, 3, 4, 5, 6, 7

@@ -1,4 +1,4 @@
-"""Timings of the non-headline BASELINE configs (C3, C4) at full size on one B200, with
+"""Timings of the non-headline BASELINE configs (C3, C4) at full size on one H100, with
 size-independent correctness checks.  Not bench lines: reported in DESIGN.md."""
 import sys, time, json
 import torch

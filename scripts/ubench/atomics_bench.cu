@@ -26,17 +26,17 @@ int main(int argc, char** argv) {
   uint32_t K = argc > 2 ? atoi(argv[2]) : 1000000;
   uint32_t* k; double* v; double* sum; unsigned* cnt;
   cudaMalloc(&k, n * 4); cudaMalloc(&v, n * 8); cudaMalloc(&sum, (size_t)K * 8); cudaMalloc(&cnt, (size_t)K * 4);
-  gen<<<148 * 8, 256>>>(k, v, n, K);
+  gen<<<132 * 8, 256>>>(k, v, n, K);
   cudaMemset(sum, 0, (size_t)K * 8); cudaMemset(cnt, 0, (size_t)K * 4);
   cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
   const char* names[4] = {"read-only k,v", "f64 sum atomics", "u32 count atomics", "sum + count"};
   for (int mode = 0; mode < 4; mode++) {
     for (int rep = 0; rep < 3; rep++) {
       cudaEventRecord(a);
-      if (mode == 0) agg<0><<<148 * 16, 512>>>(k, v, n, sum, cnt);
-      if (mode == 1) agg<1><<<148 * 16, 512>>>(k, v, n, sum, cnt);
-      if (mode == 2) agg<2><<<148 * 16, 512>>>(k, v, n, sum, cnt);
-      if (mode == 3) agg<3><<<148 * 16, 512>>>(k, v, n, sum, cnt);
+      if (mode == 0) agg<0><<<132 * 16, 512>>>(k, v, n, sum, cnt);
+      if (mode == 1) agg<1><<<132 * 16, 512>>>(k, v, n, sum, cnt);
+      if (mode == 2) agg<2><<<132 * 16, 512>>>(k, v, n, sum, cnt);
+      if (mode == 3) agg<3><<<132 * 16, 512>>>(k, v, n, sum, cnt);
       cudaEventRecord(b); cudaEventSynchronize(b);
       float ms; cudaEventElapsedTime(&ms, a, b);
       if (rep == 2) printf("K=%u n=%zu %-20s %.3f ms  %.1f Grows/s\n", K, n, names[mode], ms, n / ms / 1e6);

@@ -45,7 +45,7 @@ __global__ void __launch_bounds__(256, 4) k(unsigned* out, int iters, int bits) 
 }
 
 int main() {
-  unsigned* out; cudaMalloc(&out, 148 * 4 * 256 * 4);
+  unsigned* out; cudaMalloc(&out, 132 * 4 * 256 * 4);
   cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
   const int iters = 20000;
   const char* names[3] = {"match.any", "ballot x bits", "smem atomicOr"};
@@ -53,15 +53,15 @@ int main() {
     for (int mode = 0; mode < 3; mode++) {
       for (int rep = 0; rep < 2; rep++) {
         cudaEventRecord(a);
-        if (mode == 0) k<0><<<148 * 4, 256>>>(out, iters, bits);
-        if (mode == 1) k<1><<<148 * 4, 256>>>(out, iters, bits);
-        if (mode == 2) k<2><<<148 * 4, 256>>>(out, iters, bits);
+        if (mode == 0) k<0><<<132 * 4, 256>>>(out, iters, bits);
+        if (mode == 1) k<1><<<132 * 4, 256>>>(out, iters, bits);
+        if (mode == 2) k<2><<<132 * 4, 256>>>(out, iters, bits);
         cudaEventRecord(b); cudaEventSynchronize(b);
         float ms; cudaEventElapsedTime(&ms, a, b);
         // warp-level operations per second over the chip, and SM cycles per warp-op at 1.965 GHz
-        double wops = 148.0 * 4 * 8 * iters;
+        double wops = 132.0 * 4 * 8 * iters;
         if (rep == 1) printf("bits=%d %-14s %.3f ms  %.1f G warp-ops/s  %.1f SM-cycles per warp-op (32 warps/SM resident)\n",
-                             bits, names[mode], ms, wops / ms / 1e6, ms * 1e-3 * 1.965e9 / (wops / 148));
+                             bits, names[mode], ms, wops / ms / 1e6, ms * 1e-3 * 1.98e9 / (wops / 132));
       }
     }
   printf("err=%s\n", cudaGetErrorString(cudaDeviceSynchronize()));

@@ -127,27 +127,27 @@ template <int NB> void run(unsigned* out, unsigned* bad) {
   cudaFuncSetAttribute(k<1, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   cudaFuncSetAttribute(k<2, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   cudaFuncSetAttribute(k<3, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-  check<NB><<<148, 256, 2 * smem>>>(bad, 400);
+  check<NB><<<132, 256, 2 * smem>>>(bad, 400);
   unsigned hbad = 0; cudaMemcpy(&hbad, bad, 4, cudaMemcpyDeviceToHost);
   for (int mode = 0; mode < 4; mode++) {
     float ms = 0;
     for (int rep = 0; rep < 2; rep++) {
       cudaEventRecord(a);
-      if (mode == 0) k<0, NB><<<148 * 4, 256, smem>>>(out, iters);
-      else if (mode == 1) k<1, NB><<<148 * 4, 256, smem>>>(out, iters);
-      else if (mode == 2) k<2, NB><<<148 * 4, 256, smem>>>(out, iters);
-      else           k<3, NB><<<148 * 4, 256, smem>>>(out, iters);
+      if (mode == 0) k<0, NB><<<132 * 4, 256, smem>>>(out, iters);
+      else if (mode == 1) k<1, NB><<<132 * 4, 256, smem>>>(out, iters);
+      else if (mode == 2) k<2, NB><<<132 * 4, 256, smem>>>(out, iters);
+      else           k<3, NB><<<132 * 4, 256, smem>>>(out, iters);
       cudaEventRecord(b); cudaEventSynchronize(b);
       cudaEventElapsedTime(&ms, a, b);
     }
-    const double wops = 148.0 * 4 * 8 * iters;
+    const double wops = 132.0 * 4 * 8 * iters;
     printf("bits=%2d %-7s %8.3f ms  %6.1f SM-cycles per 32-row round (32 warps/SM)  mismatches=%u\n", NB,
-           mode == 0 ? "ballot" : mode == 1 ? "atomic" : mode == 2 ? "redux" : "mixed", ms, ms * 1e-3 * 1.965e9 / (wops / 148), hbad);
+           mode == 0 ? "ballot" : mode == 1 ? "atomic" : mode == 2 ? "redux" : "mixed", ms, ms * 1e-3 * 1.98e9 / (wops / 132), hbad);
   }
 }
 
 int main() {
-  unsigned* out; cudaMalloc(&out, 148 * 4 * 256 * 4);
+  unsigned* out; cudaMalloc(&out, 132 * 4 * 256 * 4);
   unsigned* bad; cudaMalloc(&bad, 4);
   run<6>(out, bad); run<7>(out, bad); run<8>(out, bad);
   printf("err=%s\n", cudaGetErrorString(cudaDeviceSynchronize()));

@@ -1,3 +1,4 @@
+import glob
 import json
 import os
 import sys
@@ -11,7 +12,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -37,14 +38,18 @@ class Golden:
         g = os.path.join(ROOT, "tests", "golden")
         with open(os.path.join(g, "golden_v1.json")) as fh:
             self.meta = json.load(fh)
-        self.arr = np.load(os.path.join(g, "golden_v1.npz"))
+        # the arrays are stored in parts below 1 MB each (golden_v1_00.npz, ...; make_golden.save_parts)
+        self.arr = {}
+        for part in sorted(glob.glob(os.path.join(g, "golden_v1_*.npz"))):
+            with np.load(part) as z:
+                self.arr.update((k, z[k]) for k in z.files)
         self.cases = self.meta["cases"]
 
     def get(self, case, key):
         return self.arr[f"{case['name']}__{key}"]
 
     def has(self, case, key):
-        return f"{case['name']}__{key}" in self.arr.files
+        return f"{case['name']}__{key}" in self.arr
 
 
 _golden = None

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """
-Generates tests/golden/golden_v1.{npz,json} by running the *reference itself*.
+Generates tests/golden/golden_v1.json and golden_v1_NN.npz (parts below 1 MB) by running the *reference itself*.
 
 Usage (in the build container, where the reference was built from
-/root/reference with its own backend into a scratch copy):
+the reference's source tree with its own backend into a scratch copy):
 
     PYTHONPATH=/tmp/dtref/src python tests/golden/make_golden.py
 
@@ -19,6 +19,7 @@ The literal cases restate the reference's own known-answer tests
 (tests/ijby/test-sort.py, tests/test-groups.py, tests/test-reduce.py); the
 expected values are *recomputed by the reference here*, not typed in.
 """
+import io
 import json
 import os
 import sys
@@ -118,6 +119,25 @@ def add_case(name, keys, kst=None, reverse=None, na_position="first", nby=None,
 
 
 # ---------------------------------------------------------------------------
+def save_parts(arrays, prefix, max_bytes=900_000):
+    """Writes the arrays as prefix_00.npz, prefix_01.npz, ... (every case's arrays in one part), each part
+    compressed and below max_bytes, so that no stored file reaches 1 MB."""
+    cases = {}
+    for key, a in arrays.items():
+        cases.setdefault(key.split("__")[0], {})[key] = a
+    parts, cur = [], {}
+    for case in cases.values():
+        trial = dict(cur, **case)
+        buf = io.BytesIO(); np.savez_compressed(buf, **trial)
+        if cur and buf.tell() > max_bytes:
+            parts.append(cur); cur = dict(case)
+        else:
+            cur = trial
+    parts.append(cur)
+    for i, part in enumerate(parts):
+        np.savez_compressed(f"{prefix}_{i:02d}.npz", **part)
+
+
 # Literal cases restating the reference's own tests
 # ---------------------------------------------------------------------------
 I4 = np.int32
@@ -268,7 +288,7 @@ n = 20000
 add_case("c2_shape", [rng.integers(0, 1000, n).astype(np.int32)], nby=1, vals=[rng.random(n)],
          reducers=[("sum", 0)])
 
-np.savez_compressed(os.path.join(HERE, "golden_v1.npz"), **arrays)
+save_parts(arrays, os.path.join(HERE, "golden_v1"))
 with open(os.path.join(HERE, "golden_v1.json"), "w") as fh:
     json.dump({"reference": "h2oai/datatable @ 3611640 (1.2.0a), sort.new=False",
                "datatable_version": dt.__version__, "cases": manifest}, fh, indent=0)

@@ -4,8 +4,6 @@ import os
 import subprocess
 import sys
 
-import pytest
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -26,26 +24,33 @@ def test_reference_arm_prints_the_contract_line():
     assert j["steps"] == 1 and "workload" in j["config"]
 
 
-def test_hook_script_anchors_match_the_reference():
+def test_hook_script_anchors_match_the_reference(tmp_path):
     """integration/apply_hook.py inserts next to short anchor strings: each must occur exactly once in the
-    reference revision the goldens were generated from (skipped where /root/reference is absent), and
-    the script must refuse to touch /root/reference itself."""
+    reference revision the goldens were generated from (tests/golden/hook_anchors.json, recounted in the
+    reference tree itself where DATATABLE_REFERENCE_SRC names one), and the script must refuse to touch
+    the configured reference source tree or anything inside it."""
     sys.path.insert(0, os.path.join(ROOT, "integration"))
     try:
         import apply_hook as ah
     finally:
         sys.path.pop(0)
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "integration", "apply_hook.py"), "/root/reference"],
-                       capture_output=True, text=True)
-    assert r.returncode != 0 and "refusing" in (r.stdout + r.stderr)
-    ref = "/root/reference"
-    if not os.path.exists(os.path.join(ref, "src", "core", "sort.cc")):
-        pytest.skip("no reference tree here")
-    sort_cc = open(os.path.join(ref, "src", "core", "sort.cc")).read()
-    red_cc = open(os.path.join(ref, "src", "core", "expr", "fexpr_reduce_unary.cc")).read()
-    ext_py = open(os.path.join(ref, "ci", "ext.py")).read()
-    for text, anchors in ((sort_cc, (ah.INCLUDE_ANCHOR, ah.OPTION_ANCHOR, ah.REGISTER_ANCHOR, ah.HOOK_ANCHOR)),
-                          (red_cc, (ah.RED_INCLUDE_ANCHOR, ah.RED_HELPER_ANCHOR, ah.RED_LOOP_ANCHOR)),
-                          (ext_py, (ah.EXT_ANCHOR,))):
-        for a in anchors:
-            assert text.count(a) == 1, a
+    src = tmp_path / "reference"
+    (src / "src").mkdir(parents=True)
+    for tree in (src, src / "src"):
+        r = subprocess.run([sys.executable, os.path.join(ROOT, "integration", "apply_hook.py"), str(tree)],
+                           env=dict(os.environ, DATATABLE_REFERENCE_SRC=str(src)), capture_output=True, text=True)
+        assert r.returncode != 0 and "refusing" in (r.stdout + r.stderr)
+    with open(os.path.join(ROOT, "tests", "golden", "hook_anchors.json")) as fh:
+        recorded = json.load(fh)["anchors"]
+    sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
+    try:
+        import make_golden_anchors as mga
+    finally:
+        sys.path.pop(0)
+    assert set(recorded) == set(mga.ANCHORS)
+    for name, rec in recorded.items():
+        assert rec["anchor"] == getattr(ah, name), f"{name} changed since the anchors were counted in the reference"
+        assert rec["count"] == 1, name
+    ref = os.environ.get("DATATABLE_REFERENCE_SRC", "")
+    if os.path.isdir(ref):
+        assert all(rec["count"] == 1 for rec in mga.count_anchors(ref).values())

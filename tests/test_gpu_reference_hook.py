@@ -1,7 +1,7 @@
 """GPU: the REFERENCE itself, patched by integration/apply_hook.py so that its group() calls dtb_group
 (option sort.b200), must give the stock CPU results -- the drop-in boundary exercised from the
-reference's side.  Needs the patched build staged under integration/_ref_patched (git-ignored, built
-in the dev container from a scratch copy of the reference; see INTEGRATION.md B); skipped without it."""
+reference's side.  Needs the patched build staged under oracle/_ref/patched (git-ignored; build() makes it from a
+scratch copy of the reference's source tree where that is readable, see INTEGRATION.md B); skipped without it."""
 import os
 import subprocess
 import sys
@@ -11,13 +11,16 @@ import pytest
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PATCHED = os.path.join(ROOT, "integration", "_ref_patched")
+PATCHED = os.path.join(ROOT, "oracle", "_ref", "patched")
 
 
 def _run(script):
     if not os.path.exists(os.path.join(PATCHED, "datatable", "__init__.py")):
-        pytest.skip("no patched reference build under integration/_ref_patched")
-    env = dict(os.environ, PYTHONPATH=PATCHED)
+        pytest.skip("no patched reference build under oracle/_ref/patched: build() makes it only where the "
+                    "reference's source tree is readable (DATATABLE_REFERENCE_SRC, or `reference` next to the repository)")
+    lib = os.path.join(ROOT, "datatable_b200", "lib")                   # the patched extension links libdtb200.so
+    env = dict(os.environ, PYTHONPATH=PATCHED,
+               LD_LIBRARY_PATH=os.pathsep.join(p for p in (lib, os.environ.get("LD_LIBRARY_PATH")) if p))
     r = subprocess.run([sys.executable, os.path.join(ROOT, "integration", script)],
                        env=env, capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stdout + r.stderr
