@@ -27,11 +27,7 @@ void count_launch(int n) { t_stats.kernels_launched += n; }
 static int64_t opt_radix_bits = 0;     // 0 = default (8-bit digits); 4..8 = largest digit width
 static int64_t opt_verbose = 0;
 static int64_t opt_profile = 0;
-static thread_local int opt_trust_offsets = 0;  // internal: dtb_groupby_reduce passes the handle's own offsets to dtb_reduce
-static int64_t opt_fuse_hist = 1;      // 1 = single-column keys: statistics and the first pass's histogram from one read of the column
-static int64_t opt_stage_keys = 0;     // 1 = the first count kernel also materialises the normalised keys of a raw key column (round-1 behaviour)
 static int64_t opt_bucketed = 1;       // 1 = columns with >= 2 L2 atomics per row take the bucketed multi-reducer (dtb_bucket.cu)
-static int64_t opt_overlap = 0;        // 1 = run fused direct reducers on a side stream under the sort passes
 
 // ---------------------------------------------------------------------------
 // optional per-kernel timing with CUDA events on the launching stream
@@ -348,31 +344,17 @@ struct FusedReducers {
   std::vector<void*> out;       // owned device buffers, ngroups elements each
 };
 
-// Side stream on which the direct-address reducers run while the sort passes occupy `s`.
-struct SideStream {
-  cudaStream_t stream = nullptr;
-  cudaEvent_t fork = nullptr, join = nullptr;
-  int device = -1;
-  int ensure() {
-    int dev = 0;
-    DTB_CUDA_CHECK(cudaGetDevice(&dev));
-    if (stream && device != dev) {               // the thread moved to another device: new stream there
-      cudaSetDevice(device);
-      cudaStreamDestroy(stream); cudaEventDestroy(fork); cudaEventDestroy(join);
-      cudaSetDevice(dev);
-      stream = nullptr;
-    }
-    device = dev;
-    if (stream) return DTB_OK;
-    int lo = 0, hi = 0;
-    DTB_CUDA_CHECK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    DTB_CUDA_CHECK(cudaStreamCreateWithPriority(&stream, cudaStreamNonBlocking, hi));
-    DTB_CUDA_CHECK(cudaEventCreateWithFlags(&fork, cudaEventDisableTiming));
-    DTB_CUDA_CHECK(cudaEventCreateWithFlags(&join, cudaEventDisableTiming));
-    return DTB_OK;
+// L2 atomics per row that the reducers spec[i..n) of spec[i]'s value column cost on the one-atomic-per-row
+// path (mean = sum + count).  For the first reducer of a column: the whole column's cost.
+static int column_atomics(const dtb_reduce_spec* spec, int n, int i) {
+  int cost = 0;
+  for (int j = i; j < n; j++) {
+    const dtb_reduce_spec& sj = spec[j];
+    if (sj.op == DTB_OP_NROWS || sj.value.data != spec[i].value.data || sj.value.stype != spec[i].value.stype) continue;
+    cost += sj.op == DTB_OP_MEAN ? 2 : (sj.op >= DTB_OP_SUM && sj.op <= DTB_OP_COUNTNA ? 1 : 0);
   }
-};
-static thread_local SideStream t_side;
+  return cost;
+}
 
 struct GroupResult {
   DevBuf order;          // int32[n]
@@ -497,7 +479,7 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
   DevBuf d_stats; DTB_TRY(d_stats.alloc(sizeof(ColStats) * nkeys, s));
   // single key column: the statistics kernel also counts the low 8 bits of every tile, which becomes the first
   // pass's histogram once edge / inc are known (no count kernel, one read of the column less)
-  const bool fuse_hist = nkeys == 1 && opt_fuse_hist && !opt_stage_keys;
+  const bool fuse_hist = nkeys == 1;
   DevBuf rawhist, rawna;
   if (fuse_hist) {
     DTB_TRY(rawhist.alloc(stats_hist_bytes(n), s));
@@ -586,49 +568,38 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
   // ---- fused reducers: when the group key domain is small the reducers only need the key
   //      columns, not the RowIndex: they stream the rows in storage order once the groups are known
   //      (the streaming mode -- plain / shared-memory table / hot-key cache -- depends on the number of
-  //      groups and the size of the largest one, see plan_direct).  Option "overlap_reducers" runs
-  //      them on a side stream WHILE the sort passes run instead (hot keys guessed on the device). ----
+  //      groups and the size of the largest one, see plan_direct).  They run on `s` after the offsets
+  //      stage: measured on C2, running them on a second stream under the sort passes gained ~2 % for the
+  //      accumulation (both want the same SMs) and made every scatter launch ~40 % slower. ----
+  // Streaming by group key needs one round of at most 22 group-key bits, key columns that are still in
+  // device memory after the call, and every row in a group.
   bool staged_keys = false;
   for (int c = 0; c < nkeys; c++) staged_keys = staged_keys || (in[c].buf.p != nullptr);
-  const int dbits0 = (nrounds == 1) ? rounds[0].kp.total_bits - rounds[0].kp.group_shift : 99;
-  bool fused_direct = fr && fr->n > 0 && groups_k && nrounds == 1 && !staged_keys && dbits0 <= 22 &&
-                      na_pos != DTB_NA_REMOVE;
+  const int dbits = (nrounds == 1) ? rounds[0].kp.total_bits - rounds[0].kp.group_shift : 99;
+  const bool direct_ok = groups_k && nrounds == 1 && !staged_keys && dbits <= 22 && na_pos != DTB_NA_REMOVE;
+  bool fused_direct = direct_ok && fr && fr->n > 0;
   if (fused_direct)
     for (int i = 0; i < fr->n; i++)
       fused_direct = fused_direct && fr->spec[i].op <= DTB_OP_NROWS &&           // streaming modes exist for sum..nrows only
                      (fr->spec[i].op == DTB_OP_NROWS || is_device_ptr(fr->spec[i].value.data));
   // Small key domain + handle path: the last pass counts rows per group key instead of writing
   // the sorted keys, and the offsets come from a scan over that table.
-  const bool count_table = want_direct && groups_k && nrounds == 1 && !staged_keys && dbits0 <= 22 &&
-                           na_pos != DTB_NA_REMOVE;
+  const bool count_table = want_direct && direct_ok;
   int64_t ctable = 0;
   DevBuf gcount;
   if (count_table) {
-    ctable = (int64_t)1 << (dbits0 < 10 ? 10 : dbits0);
+    ctable = (int64_t)1 << (dbits < 10 ? 10 : dbits);
     DTB_TRY(gcount.alloc(sizeof(u32) * (size_t)ctable, s));
     DTB_CUDA_CHECK(cudaMemsetAsync(gcount.p, 0, sizeof(u32) * (size_t)ctable, s));
   }
   DevBuf facc;
   DevBuf bxk;                                          // bucketed reducers: the rows' composite keys, kept
   bool bucket_wanted = false;                          // some value column costs >= 2 L2 atomics per row
-  if (fused_direct && opt_bucketed && dbits0 >= BK_MIN_DBITS && dbits0 <= BK_MAX_DBITS)
-    for (int i = 0; i < fr->n && !bucket_wanted; i++) {
-      if (fr->spec[i].op == DTB_OP_NROWS) continue;
-      int cost = 0;
-      for (int j = 0; j < fr->n; j++)
-        if (fr->spec[j].op != DTB_OP_NROWS && fr->spec[j].value.data == fr->spec[i].value.data)
-          cost += fr->spec[j].op == DTB_OP_MEAN ? 2 : 1;
-      bucket_wanted = cost >= 2;
-    }
-  const int64_t ftable = fused_direct ? ((int64_t)1 << dbits0) : 0;
-  // Measured on C2: under the sort passes the accumulation gains ~2 % (both want the same SMs) and
-  // inflates every scatter launch by ~40 %, so by default it runs on `s` after the offsets stage;
-  // option "overlap_reducers" moves it to the side stream.
-  cudaStream_t rs = s;
-  if (fused_direct) {
-    if (opt_overlap) { DTB_TRY(t_side.ensure()); rs = t_side.stream; }
-    DTB_TRY(facc.alloc(sizeof(u64) * (size_t)ftable * 2 * (size_t)fr->n, s));
-  }
+  if (fused_direct && opt_bucketed && dbits >= BK_MIN_DBITS && dbits <= BK_MAX_DBITS)
+    for (int i = 0; i < fr->n && !bucket_wanted; i++)
+      bucket_wanted = fr->spec[i].op != DTB_OP_NROWS && column_atomics(fr->spec, fr->n, i) >= 2;
+  const int64_t ftable = fused_direct ? ((int64_t)1 << dbits) : 0;
+  if (fused_direct) DTB_TRY(facc.alloc(sizeof(u64) * (size_t)ftable * 2 * (size_t)fr->n, s));
   const int32_t* idx_cur = nullptr;        // rows in the order established by the previous rounds
   void* sorted_keys = nullptr;             // last round's sorted composite keys
   int last_key_bytes = 4;
@@ -669,12 +640,10 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
       DTB_TRY(launch_compose_keys(rk, n, idx_cur, keep_composite ? bxk.p : keyA.p, key_bytes, s)); src_kind = 0;
     }
 
-    // per-pass scratch: chunk x digit counts + digit totals/bases; largest digit count per pass
+    // per-pass scratch: chunk x digit counts + digit totals/bases
     DevBuf work; DTB_TRY(work.alloc(radix_pass_work_bytes(n), s));
-    DevBuf hmax; DTB_TRY(hmax.alloc(sizeof(u32) * MAX_PASSES, s));
 
     int32_t* round_out = last_round ? order : ((ri & 1) ? idxR1.as<int32_t>() : idxR0.as<int32_t>());
-    // raw single column: the first count kernel materialises the normalised keys into keyA
     void* kin = keep_composite ? bxk.p : keyA.p; void* kout = keyB.p;
     const int32_t* iin = idx_cur;
     for (int p = 0; p < pp.npasses; p++) {
@@ -682,7 +651,6 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
       PassIO io;
       io.src_kind = (p == 0) ? src_kind : 0;
       io.keys_in = kin;
-      io.keys_stage = (p == 0 && src_kind == 1 && opt_stage_keys) ? keyA.p : nullptr;
       io.narrow_out = (p == narrow_after) ? (rk.total_bits - 32) : 0;
       if (fuse_hist && ri == 0 && p == 0 && src_kind == 1 && pp.shift[0] == 0 && rk.k[0].cshift == 0 && rk.k[0].lshift == 0) {
         io.raw_hist = rawhist.as<unsigned short>(); io.raw_na = rawna.as<unsigned short>();
@@ -692,24 +660,8 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
       io.keys_out = (last && !want_sorted_keys) ? nullptr : kout;
       int32_t* iout = last ? round_out : ((p & 1) ? idxB.as<int32_t>() : idxA.as<int32_t>());
       io.idx_out = iout;
-      const bool fork_here = fused_direct && rs != s && ri == 0 && p == 0;
-      DTB_TRY(launch_radix_pass(io, rk, kb, n, pp.shift[p], pp.bits[p], work.as<u32>(),
-                                hmax.as<u32>() + p, s, fork_here ? t_side.fork : nullptr,
+      DTB_TRY(launch_radix_pass(io, rk, kb, n, pp.shift[p], pp.bits[p], work.as<u32>(), s,
                                 (count_table && last) ? gcount.as<u32>() : nullptr, rk.group_shift));
-      if (fork_here) {
-        // the digit totals of pass 0 exist (hmax): the reducers decide about hot keys on the device
-        DTB_CUDA_CHECK(cudaStreamWaitEvent(rs, t_side.fork, 0));
-        DirectPlan dp = {DIRECT_DEVICE_HOT, nullptr, ftable, hmax.as<u32>(), (u32)(0.02 * (double)n)};
-        for (int i = 0; i < fr->n; i++) {
-          if (fr->spec[i].op == DTB_OP_NROWS) continue;
-          ProfScope ps("reduce_direct_overlapped", rs);
-          DTB_TRY(launch_direct_accumulate(fr->spec[i].op, rk, dp, fr->spec[i].value.data,
-                                           fr->spec[i].value.stype, n, ftable,
-                                           facc.as<u64>() + (size_t)ftable * 2 * i,
-                                           facc.as<u64>() + (size_t)ftable * (2 * i + 1), rs));
-        }
-        DTB_CUDA_CHECK(cudaEventRecord(t_side.join, rs));
-      }
       if (last && want_sorted_keys) { sorted_keys = kout; last_key_bytes = key_bytes; }
       kin = kout;
       kout = (kout == keyA.p) ? keyB.p : keyA.p;
@@ -766,10 +718,7 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
     DTB_CUDA_CHECK(stream_wait(s));
     res.ngroups = (int64_t)h_ng[0];
     // group key of every group, for the direct-address reducers
-    bool staged = false;
-    for (int c = 0; c < nkeys; c++) staged = staged || (in[c].buf.p != nullptr);
-    const int dbits = (nrounds == 1) ? rounds[0].kp.total_bits - rounds[0].kp.group_shift : 99;
-    if ((want_direct || fused_direct) && nrounds == 1 && !staged && dbits <= 22 && na_pos != DTB_NA_REMOVE) {
+    if (direct_ok && (want_direct || fused_direct)) {
       if (!count_table) {
         DTB_TRY(res.gkeys.alloc_owned(sizeof(u32) * (size_t)(res.ngroups + 1), s));
         DTB_TRY(launch_group_keys(sorted_keys, last_key_bytes, offsets, rounds[0].kp.group_shift, res.ngroups,
@@ -787,10 +736,9 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
   if (fr && fr->n > 0 && do_groups) {
     const int64_t ng = res.ngroups;
     fr->out.assign(fr->n, nullptr);
-    if (fused_direct && rs != s) DTB_CUDA_CHECK(cudaStreamWaitEvent(s, t_side.join, 0));
-    DirectPlan dp = {DIRECT_PLAIN, nullptr, ftable, nullptr, 0};
+    DirectPlan dp = {DIRECT_PLAIN, nullptr, ftable};
     DevBuf dmap;
-    if (fused_direct && rs == s && ng > 0) {
+    if (fused_direct && ng > 0) {
       DTB_TRY(dmap.alloc(direct_map_bytes(ftable), s));
       DTB_TRY(plan_direct(ftable, res.gkeys.as<u32>(), offsets, ng, n, res.direct_gmax, dmap.p, s, dp));
     }
@@ -806,17 +754,12 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
     std::vector<int> bcol_of(fr->n, -1);
     std::list<DevBuf> bbufs;                                   // accumulator tables (live until the finalizes ran)
     DevBuf bstart, bscr;
-    if (fused_direct && rs == s && ng > 0 && dp.kind == DIRECT_PLAIN && opt_bucketed &&
-        dbits0 >= BK_MIN_DBITS && dbits0 <= BK_MAX_DBITS) {
-      auto natomics = [](int op) { return op == DTB_OP_MEAN ? 2 : (op >= DTB_OP_SUM && op <= DTB_OP_COUNTNA ? 1 : 0); };
+    if (fused_direct && ng > 0 && dp.kind == DIRECT_PLAIN && opt_bucketed &&
+        dbits >= BK_MIN_DBITS && dbits <= BK_MAX_DBITS) {
       for (int i = 0; i < fr->n; i++) {
         const dtb_reduce_spec& sp = fr->spec[i];
         if (sp.op == DTB_OP_NROWS || bcol_of[i] >= 0 || !reduce_out_stype_host(sp.op, sp.value.stype)) continue;
-        int cost = 0;
-        for (int j = i; j < fr->n; j++)
-          if (fr->spec[j].op != DTB_OP_NROWS && fr->spec[j].value.data == sp.value.data && fr->spec[j].value.stype == sp.value.stype)
-            cost += natomics(fr->spec[j].op);
-        if (cost < 2) continue;
+        if (column_atomics(fr->spec, fr->n, i) < 2) continue;
         BucketCol bc; bc.data = sp.value.data; bc.stype = sp.value.stype;
         for (int w = 0; w < BK_NWORDS; w++) bc.w[w] = nullptr;
         bool want[BK_NWORDS] = {false, false, false, false, false, false};
@@ -844,7 +787,7 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
         bcols.push_back(bc);
       }
       if (!bcols.empty()) {
-        const int nb = 1 << (dbits0 > 11 ? dbits0 - 11 : 0);
+        const int nb = 1 << (dbits > 11 ? dbits - 11 : 0);
         // sweeps of up to BK_MAXCOLS columns / 32 value bytes per row (the partitioned copies live in scratch)
         std::vector<std::pair<int, int>> sweeps;           // [first, last) into bcols
         size_t scr = 0;
@@ -873,7 +816,7 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
             vals[c] = bc.data; sts[c] = bc.stype;
             for (int w = 0; w < BK_NWORDS; w++) words[c][w] = bc.w[w];
           }
-          DTB_TRY(launch_bucketed_reduce(bxk.as<u32>(), rounds[0].kp.group_shift, dbits0, nc, vals, sts, n, slab_starts,
+          DTB_TRY(launch_bucketed_reduce(bxk.as<u32>(), rounds[0].kp.group_shift, dbits, nc, vals, sts, n, slab_starts,
                                          start, words, bscr.p, s));
         }
       }
@@ -904,7 +847,7 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
       } else if (fused_direct) {
         u64* a0 = facc.as<u64>() + (size_t)ftable * 2 * i;
         u64* a1 = facc.as<u64>() + (size_t)ftable * (2 * i + 1);
-        if (rs == s && ng > 0) {
+        if (ng > 0) {
           ProfScope ps("reduce_direct", s);
           DTB_TRY(launch_direct_accumulate(sp.op, rounds[0].kp, dp, sp.value.data, sp.value.stype, n, ftable, a0, a1, s));
         }
@@ -992,10 +935,7 @@ int dtb_set_option(const char* name, int64_t value) {
   }
   if (!strcmp(name, "verbose")) { opt_verbose = value; return DTB_OK; }
   if (!strcmp(name, "profile")) { opt_profile = value; return DTB_OK; }
-  if (!strcmp(name, "overlap_reducers")) { opt_overlap = value; return DTB_OK; }
   if (!strcmp(name, "bucketed_reducers")) { opt_bucketed = value ? 1 : 0; return DTB_OK; }
-  if (!strcmp(name, "stage_keys")) { opt_stage_keys = value ? 1 : 0; return DTB_OK; }
-  if (!strcmp(name, "fuse_stats_hist")) { opt_fuse_hist = value ? 1 : 0; return DTB_OK; }
   if (!strcmp(name, "trim_scratch")) {
     if (t_arena.depth == 0 && t_arena.device >= 0) {
       int cur = 0; cudaGetDevice(&cur);
@@ -1034,10 +974,7 @@ int dtb_get_option(const char* name, int64_t* value) {
   if (!strcmp(name, "radix_bits")) { *value = opt_radix_bits; return DTB_OK; }
   if (!strcmp(name, "verbose")) { *value = opt_verbose; return DTB_OK; }
   if (!strcmp(name, "profile")) { *value = opt_profile; return DTB_OK; }
-  if (!strcmp(name, "overlap_reducers")) { *value = opt_overlap; return DTB_OK; }
   if (!strcmp(name, "bucketed_reducers")) { *value = opt_bucketed; return DTB_OK; }
-  if (!strcmp(name, "stage_keys")) { *value = opt_stage_keys; return DTB_OK; }
-  if (!strcmp(name, "fuse_stats_hist")) { *value = opt_fuse_hist; return DTB_OK; }
   set_error(std::string("unknown option ") + name);
   return DTB_EINVAL;
 }
@@ -1154,8 +1091,9 @@ int dtb_groupby_destroy(dtb_groupby* g, dtb_stream stream) {
   return DTB_OK;
 }
 
-int dtb_reduce(int op, dtb_col value, int64_t nrows_value, const void* order, int order_is64,
-               const void* offsets, int64_t ngroups, dtb_stream stream, void* out)
+// check_offsets = false: the offsets come from group() (a handle's own), so they need no device check
+static int reduce_groups(int op, dtb_col value, int64_t nrows_value, const void* order, int order_is64,
+                         const void* offsets, int64_t ngroups, dtb_stream stream, void* out, bool check_offsets)
 {
   cudaStream_t s = (cudaStream_t)stream;
   ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
@@ -1179,7 +1117,7 @@ int dtb_reduce(int op, dtb_col value, int64_t nrows_value, const void* order, in
   if (is_device_ptr(offsets)) {
     DevBuf d_bad; DTB_TRY(d_bad.alloc(sizeof(int), s));
     DTB_CUDA_CHECK(cudaMemsetAsync(d_bad.p, 0, sizeof(int), s));
-    if (!opt_trust_offsets) DTB_TRY(launch_offsets_check((const int32_t*)offsets, ngroups, d_bad.as<int>(), s));
+    if (check_offsets) DTB_TRY(launch_offsets_check((const int32_t*)offsets, ngroups, d_bad.as<int>(), s));
     DTB_CUDA_CHECK(cudaMemcpyAsync(&n32, (const int32_t*)offsets + ngroups, sizeof(int32_t), cudaMemcpyDeviceToHost, s));
     DTB_CUDA_CHECK(cudaMemcpyAsync(&bad, d_bad.p, sizeof(int), cudaMemcpyDeviceToHost, s));
     DTB_CUDA_CHECK(cudaStreamSynchronize(s));
@@ -1218,6 +1156,12 @@ int dtb_reduce(int op, dtb_col value, int64_t nrows_value, const void* order, in
   return DTB_OK;
 }
 
+int dtb_reduce(int op, dtb_col value, int64_t nrows_value, const void* order, int order_is64,
+               const void* offsets, int64_t ngroups, dtb_stream stream, void* out)
+{
+  return reduce_groups(op, value, nrows_value, order, order_is64, offsets, ngroups, stream, out, true);
+}
+
 int dtb_groupby_reduce(dtb_groupby* g, int op, dtb_col value, int64_t nrows_value, dtb_stream stream, void* out)
 {
   cudaStream_t s = (cudaStream_t)stream;
@@ -1225,12 +1169,8 @@ int dtb_groupby_reduce(dtb_groupby* g, int op, dtb_col value, int64_t nrows_valu
   if (g->ngroups < 0) { set_error("the handle holds no Groupby (sort-only call)"); return DTB_EINVAL; }
   ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
   const bool device_value = (op == DTB_OP_NROWS) || is_device_ptr(value.data);
-  if (!g->direct || op == DTB_OP_NROWS || op >= DTB_OP_FIRST || !device_value || nrows_value != g->nrows) {
-    opt_trust_offsets = 1;                         // the handle's own offsets come from group()
-    const int rc = dtb_reduce(op, value, nrows_value, g->order, 0, g->offsets, g->ngroups, stream, out);
-    opt_trust_offsets = 0;
-    return rc;
-  }
+  if (!g->direct || op == DTB_OP_NROWS || op >= DTB_OP_FIRST || !device_value || nrows_value != g->nrows)
+    return reduce_groups(op, value, nrows_value, g->order, 0, g->offsets, g->ngroups, stream, out, false);
   t_stats = dtb_call_stats{0, 0, 0, 0, 0};
   const int out_st = reduce_out_stype_host(op, value.stype);
   if (!out_st) {

@@ -104,8 +104,6 @@ struct PassIO {
   const int32_t* idx_in;
   void*       keys_out;     // may be NULL on the last pass of a sort-only call
   int32_t*    idx_out;
-  void*       keys_stage;   // src_kind 1 only, optional: buffer that receives the normalised keys in the
-                            // count kernel; the scatter kernel of the pass then reads them from there
   // first pass over a raw column whose normalisation keeps the low bits (cshift == 0): per-tile histogram of
   // the low 8 bits of u from launch_col_stats_hist; the pass folds it (x = +-(u - edge) + inc, NA -> na_value)
   // into its digit counts and does not run its count kernel
@@ -114,15 +112,13 @@ struct PassIO {
   int         narrow_out = 0;     // 64-bit keys, > 0: keys_out receives (key >> narrow_out) as uint32 (later passes run on 32-bit keys)
 };
 
-// One stable pass = count + scan + scatter kernels.  work: radix_pass_work_bytes(n) of scratch;
-// hmax (optional, device): receives the largest digit count of the pass.
+// One stable pass = count + scan + scatter kernels.  work: radix_pass_work_bytes(n) of scratch.
 size_t radix_pass_work_bytes(int64_t n);
-// after_counts (optional): recorded on `s` once the digit totals of the pass (hmax) are final.
 // group_count (optional, last pass only): uint32 table indexed by (key >> group_shift), zeroed by the
 // caller; receives the number of rows of every group key (see launch_offsets_from_counts).
 int launch_radix_pass(const PassIO& io, const KeyPlan& kp, int key_bytes, int64_t n,
-                      int shift, int bits, uint32_t* work, uint32_t* hmax, cudaStream_t s,
-                      cudaEvent_t after_counts = nullptr, uint32_t* group_count = nullptr, int group_shift = 0);
+                      int shift, int bits, uint32_t* work, cudaStream_t s,
+                      uint32_t* group_count = nullptr, int group_shift = 0);
 
 // Groupby offsets from a per-group-key row count table (small key domains): offsets[] = exclusive
 // scan of the non-zero counts, gkeys[g] = key of group g, *d_ngroups = number of groups.
@@ -169,14 +165,11 @@ int launch_offsets_check(const int32_t* offsets, int64_t ng, int* d_bad, cudaStr
 // Direct-address reducers over a small normalised key domain (see dtb_reduce.cu).
 enum { DIRECT_PLAIN = 0,        // one L2 atomic per row into acc[x]
        DIRECT_SMALL = 1,        // <= 2048 accumulators: per-CTA shared-memory tables (map: uint16 x -> group, or NULL)
-       DIRECT_HOT = 2,          // skewed group sizes: rows of hot keys (map: uint8 hot[x]) fold in shared memory
-       DIRECT_DEVICE_HOT = 3 }; // legacy overlapped mode: hot-key folding decided on the device from hot_count
+       DIRECT_HOT = 2 };        // skewed group sizes: rows of hot keys (map: uint8 hot[x]) fold in shared memory
 struct DirectPlan {
   int kind;
   const void* map;
   int64_t nslots;               // accumulators in use: table, or ngroups for a dense-mapped small table
-  const uint32_t* hot_count;
-  uint32_t hot_thresh;
 };
 size_t direct_map_bytes(int64_t table);
 // Chooses the streaming mode from the group structure (gmax = rows of the largest group) and builds the

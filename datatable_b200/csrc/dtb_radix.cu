@@ -108,10 +108,8 @@ int64_t radix_num_chunks(int64_t n) { return (n + CHUNK_ROWS - 1) / CHUNK_ROWS; 
 template <typename KeyT, typename Src, int NBINS>
 __global__ void __launch_bounds__(PASS_THREADS)
 count_kernel(const __grid_constant__ Src src, int64_t n, int shift, u32 mask, u32* __restrict__ counts,
-             unsigned short* __restrict__ tile_pre, KeyT* __restrict__ keys_out)
+             unsigned short* __restrict__ tile_pre)
 {
-  // keys_out (first pass over a raw column): also store the normalised keys, so that the scatter
-  // kernel of this pass streams 32/64-bit keys like every later pass instead of re-normalising.
   constexpr int BPT = NBINS / PASS_THREADS;
   __shared__ u32 h[NBINS];
   const int64_t cbase = (int64_t)blockIdx.x * CHUNK_ROWS;
@@ -129,16 +127,13 @@ count_kernel(const __grid_constant__ Src src, int64_t n, int shift, u32 mask, u3
       KeyT k[PASS_IPT];
 #pragma unroll
       for (int j = 0; j < PASS_IPT; j++) k[j] = src.load(base + threadIdx.x + j * PASS_THREADS);
-      if (keys_out) {
-#pragma unroll
-        for (int j = 0; j < PASS_IPT; j++) keys_out[base + threadIdx.x + j * PASS_THREADS] = k[j];
-      }
 #pragma unroll
       for (int j = 0; j < PASS_IPT; j++) atomicAdd(&h[(u32)(k[j] >> shift) & mask], 1u);
     } else {
+      // the column's last, partial tile only: unrolling it costs registers in the whole kernel
+#pragma unroll 1
       for (int64_t i = base + threadIdx.x; i < end; i += PASS_THREADS) {
         const KeyT kk = src.load(i);
-        if (keys_out) keys_out[i] = kk;
         atomicAdd(&h[(u32)(kk >> shift) & mask], 1u);
       }
     }
@@ -187,7 +182,7 @@ fold_counts_kernel(const unsigned short* __restrict__ tile_hist, const unsigned 
 
 // ===========================================================================
 // scan: offs[chunk][digit] = sum over earlier chunks (in place); total[digit]
-// then base[digit] = exclusive scan of total[]; hmax = largest total (skew detector)
+// then base[digit] = exclusive scan of total[]
 // ===========================================================================
 __global__ void __launch_bounds__(256)
 chunk_scan_kernel(u32* __restrict__ counts, int64_t nchunks, int nbins, u32* __restrict__ total)
@@ -226,22 +221,18 @@ chunk_scan_kernel(u32* __restrict__ counts, int64_t nchunks, int nbins, u32* __r
 
 template <int NBINS>
 __global__ void __launch_bounds__(256)
-digit_base_kernel(const u32* __restrict__ total, u32* __restrict__ base, u32* __restrict__ hmax)
+digit_base_kernel(const u32* __restrict__ total, u32* __restrict__ base)
 {
   constexpr int BPT = NBINS / 256;                        // thread t owns digits t*BPT .. t*BPT+BPT-1
   __shared__ u32 wsum[8];
-  __shared__ u32 wmax[8];
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-  u32 v[BPT], tsum = 0, m = 0;
+  u32 v[BPT], tsum = 0;
 #pragma unroll
-  for (int j = 0; j < BPT; j++) { v[j] = total[t * BPT + j]; tsum += v[j]; m = v[j] > m ? v[j] : m; }
+  for (int j = 0; j < BPT; j++) { v[j] = total[t * BPT + j]; tsum += v[j]; }
   u32 incl = tsum;
 #pragma unroll
   for (int k = 1; k < 32; k <<= 1) { const u32 o = __shfl_up_sync(0xffffffffu, incl, k); if (lane >= k) incl += o; }
-#pragma unroll
-  for (int k = 16; k > 0; k >>= 1) { const u32 o = __shfl_xor_sync(0xffffffffu, m, k); m = o > m ? o : m; }
   if (lane == 31) wsum[warp] = incl;
-  if (lane == 0) wmax[warp] = m;
   __syncthreads();
   u32 wpre = 0;
 #pragma unroll
@@ -249,11 +240,6 @@ digit_base_kernel(const u32* __restrict__ total, u32* __restrict__ base, u32* __
   u32 e = wpre + incl - tsum;
 #pragma unroll
   for (int j = 0; j < BPT; j++) { base[t * BPT + j] = e; e += v[j]; }
-  if (t == 0 && hmax) {
-    u32 mm = 0;
-    for (int w = 0; w < 8; w++) mm = wmax[w] > mm ? wmax[w] : mm;
-    *hmax = mm;
-  }
 }
 
 // ===========================================================================
@@ -589,8 +575,8 @@ static int run_scatter(Src src, const PassIO& io, int64_t n, int shift, u32 mask
 }
 
 template <typename KeyT, typename Src, int NBINS>
-static int run_pass_nb(Src src, const PassIO& io, int64_t n, int shift, int bits, u32* work, u32* hmax,
-                       cudaStream_t s, cudaEvent_t after_counts, u32* group_count, int group_shift)
+static int run_pass_nb(Src src, const PassIO& io, int64_t n, int shift, int bits, u32* work, cudaStream_t s,
+                       u32* group_count, int group_shift)
 {
   const int64_t nchunks = radix_num_chunks(n);
   const int64_t ntiles = (n + PASS_TILE - 1) / PASS_TILE;
@@ -601,53 +587,42 @@ static int run_pass_nb(Src src, const PassIO& io, int64_t n, int shift, int bits
   const u32 mask = (1u << bits) - 1;
 
   prof_begin("radix_count", s);
-  if (io.raw_hist && (shift != 0 || io.keys_stage)) { set_error("internal: a folded histogram needs shift 0 and no key staging"); return DTB_EINVAL; }
+  if (io.raw_hist && shift != 0) { set_error("internal: a folded histogram needs shift 0"); return DTB_EINVAL; }
   if (io.raw_hist) {
     static_assert(NBINS == 256, "the statistics kernel counts 256 bins per tile");
     const KeyNorm& k = src.key_norm();
     fold_counts_kernel<<<(unsigned)nchunks, 256, 0, s>>>(io.raw_hist, io.raw_na, ntiles, (u32)k.edge & 255u, (u32)k.inc & 255u,
                                                        k.desc, (u32)k.na_value & mask, mask, counts, tile_counts);
   } else {
-    count_kernel<KeyT, Src, NBINS><<<(unsigned)nchunks, PASS_THREADS, 0, s>>>(src, n, shift, mask, counts, tile_counts,
-                                                                               (KeyT*)io.keys_stage);
+    count_kernel<KeyT, Src, NBINS><<<(unsigned)nchunks, PASS_THREADS, 0, s>>>(src, n, shift, mask, counts, tile_counts);
   }
   prof_end(s);
   chunk_scan_kernel<<<NBINS, 256, 0, s>>>(counts, nchunks, NBINS, total);
-  digit_base_kernel<NBINS><<<1, 256, 0, s>>>(total, base, hmax);
+  digit_base_kernel<NBINS><<<1, 256, 0, s>>>(total, base);
   count_launch(3);
-  if (after_counts) DTB_CUDA_CHECK(cudaEventRecord(after_counts, s));
-
-  if (io.keys_stage) {
-    // the count kernel materialised the normalised keys: scatter from them
-    PassIO io2 = io; io2.src_kind = 0; io2.keys_in = io.keys_stage; io2.keys_stage = nullptr;
-    PackedSrc<KeyT> psrc{(const KeyT*)io.keys_stage};
-    return run_scatter<KeyT, PackedSrc<KeyT>, NBINS>(psrc, io2, n, shift, mask, ntiles, counts, base, tile_counts,
-                                                     group_count, group_shift, s);
-  }
   return run_scatter<KeyT, Src, NBINS>(src, io, n, shift, mask, ntiles, counts, base, tile_counts,
                                        group_count, group_shift, s);
 }
 
 template <typename KeyT, typename Src>
-static int run_pass(Src src, const PassIO& io, int64_t n, int shift, int bits, u32* work, u32* hmax, cudaStream_t s,
-                    cudaEvent_t after_counts, u32* group_count, int group_shift)
+static int run_pass(Src src, const PassIO& io, int64_t n, int shift, int bits, u32* work, cudaStream_t s,
+                    u32* group_count, int group_shift)
 {
   if (n == 0) return DTB_OK;
   if (io.idx_in && (reinterpret_cast<uintptr_t>(io.idx_in) & 15)) {
     set_error("internal: row-id buffer must be 16-byte aligned"); return DTB_EINVAL;
   }
-  return run_pass_nb<KeyT, Src, 256>(src, io, n, shift, bits, work, hmax, s, after_counts, group_count, group_shift);
+  return run_pass_nb<KeyT, Src, 256>(src, io, n, shift, bits, work, s, group_count, group_shift);
 }
 
 template <typename KeyT>
 static int run_pass_raw(const PassIO& io, const KeyPlan& kp, int64_t n, int shift, int bits,
-                        u32* work, u32* hmax, cudaStream_t s, cudaEvent_t after_counts,
-                        u32* group_count, int group_shift)
+                        u32* work, cudaStream_t s, u32* group_count, int group_shift)
 {
   const KeyNorm& k = kp.k[0];
 #define DTB_CASE(T)                                                                          \
   { RawSrc<T, KeyT> src; src.init(k);                                                        \
-    return run_pass<KeyT>(src, io, n, shift, bits, work, hmax, s, after_counts, group_count, group_shift); }
+    return run_pass<KeyT>(src, io, n, shift, bits, work, s, group_count, group_shift); }
   switch (k.stype) {
     case DTB_STYPE_BOOL: case DTB_STYPE_INT8:    DTB_CASE(int8_t)
     case DTB_STYPE_INT16:                        DTB_CASE(int16_t)
@@ -668,18 +643,18 @@ size_t radix_pass_work_bytes(int64_t n) {
 }
 
 int launch_radix_pass(const PassIO& io, const KeyPlan& kp, int key_bytes, int64_t n,
-                      int shift, int bits, uint32_t* work, uint32_t* hmax, cudaStream_t s,
-                      cudaEvent_t after_counts, uint32_t* group_count, int group_shift)
+                      int shift, int bits, uint32_t* work, cudaStream_t s,
+                      uint32_t* group_count, int group_shift)
 {
   if (bits < 1 || bits > 8) { set_error("internal: digit width must be 1..8 bits"); return DTB_EINVAL; }
   if (io.src_kind == 0) {
     if (key_bytes == 4) { PackedSrc<u32> src{(const u32*)io.keys_in};
-      return run_pass<u32>(src, io, n, shift, bits, work, hmax, s, after_counts, group_count, group_shift); }
+      return run_pass<u32>(src, io, n, shift, bits, work, s, group_count, group_shift); }
     else { PackedSrc<u64> src{(const u64*)io.keys_in};
-      return run_pass<u64>(src, io, n, shift, bits, work, hmax, s, after_counts, group_count, group_shift); }
+      return run_pass<u64>(src, io, n, shift, bits, work, s, group_count, group_shift); }
   }
-  return key_bytes == 4 ? run_pass_raw<u32>(io, kp, n, shift, bits, work, hmax, s, after_counts, group_count, group_shift)
-                        : run_pass_raw<u64>(io, kp, n, shift, bits, work, hmax, s, after_counts, group_count, group_shift);
+  return key_bytes == 4 ? run_pass_raw<u32>(io, kp, n, shift, bits, work, s, group_count, group_shift)
+                        : run_pass_raw<u64>(io, kp, n, shift, bits, work, s, group_count, group_shift);
 }
 
 __global__ void widen_u32_kernel(const u32* __restrict__ in, int64_t n, int64_t* __restrict__ out) {

@@ -428,58 +428,27 @@ int launch_nrows(const int32_t* offsets, int64_t ng, void* out, cudaStream_t s) 
 // composite key x = X(row) >> group_shift spans at most 2^22 values -- the reducers do not
 // need the RowIndex at all: rows are streamed in storage order (coalesced, no gather), and
 // each row folds its value into acc[x] with one L2 atomic.  One table (<= 32 MB) fits the
-// 50 MB L2 of an H100.  Rows of a warp that share x are combined first
-// (__match_any_sync) so that hot keys do not serialise on one address.  A finalize kernel
-// maps group g -> acc[gkeys[g]] and applies the reference's output stype / NA rules.
+// 50 MB L2 of an H100.  Few keys and skewed group sizes, where one atomic per row would
+// serialise on a handful of addresses, take the kernels further down (plan_direct chooses).
+// A finalize kernel maps group g -> acc[gkeys[g]] and applies the reference's output stype /
+// NA rules.
 //
 // Bound: L2 atomic throughput, then HBM.
 // Algorithmic bytes per row: key column(s) + value column, read once.
-struct HotSpec {            // "may one key own a large share of the rows?"
-  const u32* count;         // device: largest digit count of the first pass (NULL = use `value`)
-  u32 thresh;
-  int value;
-};
-
 template <typename T, int CAT, typename KSrc>
 __global__ void __launch_bounds__(512)
 direct_reduce_kernel(KSrc ksrc, int gshift, const typename RawKey<T>::load_t* __restrict__ v,
-                     int64_t n, u64* acc0, u64* acc1, int flag, HotSpec hs)
+                     int64_t n, u64* acc0, u64* acc1, int flag)
 {
-  const bool HOT = hs.count ? (*hs.count > hs.thresh) : (hs.value != 0);      // warp-uniform
-  const int lane = threadIdx.x & 31;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  const int64_t nround = ((n + 31) / 32) * 32;                // keep whole warps in the loop
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nround; i += stride) {
-    const bool in = i < n;
-    u32 x = 0xffffffffu;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const u32 x = (u32)(ksrc.load(i) >> gshift);
+    // keeps the key load next to the value load: otherwise the compiler sinks it under p_flush's test of the
+    // value, the two loads of a row serialise, and C2's accumulation measured slower
+    asm volatile("" :: "r"(x));
     Partial<CAT> part; p_init(part, flag);
-    if (in) {
-      x = (u32)(ksrc.load(i) >> gshift);
-      p_add<T, CAT>(part, v[i], true, flag);
-    }
-    // HOT: a key may own a large share of the rows (skewed digit histograms): fold equal keys of the
-    // warp before touching L2.  MATCH.ANY is a slow, multi-cycle warp instruction, so the
-    // common spread-out case skips it entirely.
-    const unsigned peers = HOT ? __match_any_sync(0xffffffffu, x) : (1u << lane);
-    if (HOT && __any_sync(0xffffffffu, peers != (1u << lane))) {  // warp-uniform: the body shuffles
-      // rare for spread-out keys: fold the partials of equal keys into the lowest lane
-      const int leader = __ffs(peers) - 1;
-      unsigned rest = peers & ~(1u << leader);
-      Partial<CAT> tot = part;
-      while (__any_sync(0xffffffffu, rest != 0)) {
-        const int src = rest ? (__ffs(rest) - 1) : lane;
-        Partial<CAT> o;
-        if constexpr (CAT == CAT_SUMI) o.s = __shfl_sync(0xffffffffu, part.s, src);
-        else if constexpr (CAT == CAT_SUMF) o.s = __shfl_sync(0xffffffffu, part.s, src);
-        else if constexpr (CAT == CAT_MEAN) { o.s = __shfl_sync(0xffffffffu, part.s, src); o.c = __shfl_sync(0xffffffffu, part.c, src); }
-        else if constexpr (CAT == CAT_MINMAX) o.key = __shfl_sync(0xffffffffu, part.key, src);
-        else o.c = __shfl_sync(0xffffffffu, part.c, src);
-        if (rest && lane == leader) p_merge(tot, o, flag);
-        rest &= rest - 1;
-      }
-      if (lane == leader) part = tot; else p_init(part, flag);
-    }
-    if (in) p_flush(part, (int64_t)x, acc0, acc1, flag);
+    p_add<T, CAT>(part, v[i], true, flag);
+    p_flush(part, (int64_t)x, acc0, acc1, flag);
   }
 }
 
@@ -663,7 +632,7 @@ direct_reduce_hot_kernel(KSrc ksrc, int gshift, const typename RawKey<T>::load_t
     if (hkey[i] != HOT_EMPTY) slot_flush<CAT>(h0[i], h1[i], (int64_t)hkey[i], acc0, acc1, flag);
 }
 
-static thread_local DirectPlan t_dp = {DIRECT_PLAIN, nullptr, 0, nullptr, 0};
+static thread_local DirectPlan t_dp = {DIRECT_PLAIN, nullptr, 0};
 
 template <typename T, int CAT, typename KSrc>
 static int run_direct(const KSrc& ks, int gshift, const void* v, int64_t n, u64* acc0, u64* acc1, int flag,
@@ -687,10 +656,8 @@ static int run_direct(const KSrc& ks, int gshift, const void* v, int64_t n, u64*
     DTB_CUDA_CHECK(cudaGetLastError());
     return DTB_OK;
   }
-  HotSpec hs = {nullptr, 0, 0};
-  if (t_dp.kind == DIRECT_DEVICE_HOT) { hs.count = t_dp.hot_count; hs.thresh = t_dp.hot_thresh; }
   int grid = (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : want);
-  direct_reduce_kernel<T, CAT, KSrc><<<grid, 512, 0, s>>>(ks, gshift, (const L*)v, n, acc0, acc1, flag, hs);
+  direct_reduce_kernel<T, CAT, KSrc><<<grid, 512, 0, s>>>(ks, gshift, (const L*)v, n, acc0, acc1, flag);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;
@@ -752,7 +719,7 @@ size_t direct_map_bytes(int64_t table) { return (size_t)table * sizeof(uint16_t)
 int plan_direct(int64_t table, const uint32_t* gkeys, const int32_t* offsets, int64_t ng, int64_t n,
                 int64_t gmax, void* map_scratch, cudaStream_t s, DirectPlan& dp)
 {
-  dp.kind = DIRECT_PLAIN; dp.map = nullptr; dp.nslots = table; dp.hot_count = nullptr; dp.hot_thresh = 0;
+  dp.kind = DIRECT_PLAIN; dp.map = nullptr; dp.nslots = table;
   if (ng <= 0) return DTB_OK;
   if (table <= SMALL_TABLE) { dp.kind = DIRECT_SMALL; return DTB_OK; }
   if (ng <= SMALL_TABLE) {
@@ -778,9 +745,7 @@ int plan_direct(int64_t table, const uint32_t* gkeys, const int32_t* offsets, in
 }
 
 // Stage 1: stream every row into acc[x] (acc[group] for a dense-mapped small table).  acc0/acc1: device
-// scratch of `table` u64 each.  DIRECT_DEVICE_HOT (reducers overlapped with the sort, before the groups
-// exist): dp.hot_count is the largest digit count of the first radix pass; more than dp.hot_thresh rows
-// in one bin switches on the intra-warp pre-aggregation, decided on the device.
+// scratch of `table` u64 each.
 int launch_direct_accumulate(int op, const KeyPlan& kp, const DirectPlan& dp,
                              const void* value, int stype, int64_t n, int64_t table,
                              u64* acc0, u64* acc1, cudaStream_t s)

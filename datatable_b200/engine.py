@@ -169,7 +169,7 @@ class Groupby:
 
     def __init__(self, cols, flags=None, na_pos=NA_FIRST, reducers=None):
         """reducers: optional [(op, value column or None), ...] evaluated inside the same call
-        (dtb_groupby_create_reduce): with a small key domain they overlap the sort on a side stream."""
+        (dtb_groupby_create_reduce): with a small key domain they stream the rows once the groups are known."""
         cols = [Col(c) for c in cols]
         nk = len(cols)
         n = cols[0].nrows

@@ -170,8 +170,8 @@ DTB_API int dtb_groupby_create(const dtb_col* keys, int nkeys, const int* flags,
 /*
  * Fused variant: group() plus `nreducers` per-group reducers in one call (the j-expressions of
  * DT[:, {sum(f.v), ...}, by(f.k)] are known before group() runs, expr/eval_context.cc:144-172).
- * When the group-key domain is small the reducers only need the key columns, so they run on an
- * engine-owned side stream concurrently with the sort passes.  Results are owned by the handle:
+ * When the group-key domain is small the reducers only need the key columns: once the groups are
+ * known they stream the key and value columns in storage order.  Results are owned by the handle:
  * dtb_groupby_reduced(g, i) = device buffer of ngroups elements of stype
  * dtb_reduce_out_stype(op, value.stype).  Equivalent to dtb_groupby_create + dtb_groupby_reduce.
  */
@@ -351,15 +351,6 @@ DTB_API int dtb_memcpy(void* dst, const void* src, int64_t nbytes, dtb_stream st
  *   "verbose"      1 = print the pass plan to stderr
  *   "profile"      1 = bracket every kernel with CUDA events on the call's stream (the calls do not wait for
  *                  them; dtb_profile_count / dtb_profile_reset do)
- *   "overlap_reducers" 1 = dtb_groupby_create_reduce runs the direct-address reducers on a side stream
- *                  concurrently with the sort passes (default 0: same stream, measured equally fast)
- *   "stage_keys"   0 (default) = the first count and scatter kernels of a single raw key column normalise it on
- *                  the fly (no normalised-key array is written); 1 = the first count kernel materialises the
- *                  normalised keys and the first scatter reads those (round-1 behaviour: one more
- *                  write and read of the keys)
- *   "fuse_stats_hist" 1 (default) = single-column keys: the statistics kernel also counts the low 8 bits of every
- *                  tile and the first radix pass folds that into its digit counts instead of reading the column
- *                  again (DESIGN.md 4.1); 0 = separate statistics and count kernels
  *   "bucketed_reducers" 1 (default) = value columns that would cost two or more L2 atomics per row (mean, or
  *                  several reducers of one column) take the bucketed multi-reducer (dtb_bucket.cu); 0 = always
  *                  one streaming pass per reducer

@@ -282,16 +282,14 @@ def test_direct_reducers_skewed_group_sizes():
     _check_direct_modes(k2, INT32, vals2, "half-hot")
 
 
-@pytest.mark.parametrize("overlap", [0, 1])
 @pytest.mark.parametrize("small_domain", [True, False])
-def test_fused_create_reduce_vs_oracle(small_domain, overlap):
-    """dtb_groupby_create_reduce: reducers evaluated inside the group() call (side-stream overlap for
+def test_fused_create_reduce_vs_oracle(small_domain):
+    """dtb_groupby_create_reduce: reducers evaluated inside the group() call (streaming the rows for
     small key domains, RowIndex path otherwise) must equal separate group + reduce."""
     import torch
     from datatable_b200 import engine
     from oracle import oracle as orc
     n = 600_000
-    engine.set_option("overlap_reducers", overlap)
     rng = np.random.default_rng(5 + small_domain)
     k = make_col(rng, INT32, n, "few" if small_domain else "wide", 0.03)
     v1 = make_col(rng, FLOAT64, n, "unit", 0.1)
@@ -312,7 +310,6 @@ def test_fused_create_reduce_vs_oracle(small_domain, overlap):
             want = orc.reduce(OPS[op], v, want_o, want_f, stype=vst)
             assert_reducer_equal(got, want, op, vst, ctx=f"fused {op} small={small_domain}")
     gb.close()
-    engine.set_option("overlap_reducers", 0)
 
 
 def test_rows_beyond_2_pow_30():
@@ -467,33 +464,10 @@ def test_group64_equals_group_and_crosses_int32():
     assert torch.equal(firsts, torch.arange(1000, device="cuda", dtype=torch.int32))
 
 
-def test_stage_keys_option_gives_identical_results():
-    """Option stage_keys (materialise the normalised keys in the first count kernel, round-1 behaviour) and the
-    default (normalise on the fly in count and scatter) must produce the same RowIndex / offsets."""
-    import torch
-    from datatable_b200 import engine, _lib
-    rng = np.random.default_rng(12)
-    n = 300_017
-    for st in (INT8, INT16, INT32, INT64, FLOAT32, FLOAT64):
-        k = make_col(rng, st, n, "wide" if st in (FLOAT32, FLOAT64) else "unit", 0.05)
-        kd = engine.Col(torch.from_numpy(k).cuda(), st)
-        res = []
-        for sk in (0, 1):
-            engine.set_option("stage_keys", sk)
-            try:
-                for fl, nap in (([0], _lib.NA_FIRST), ([_lib.FLAG_SORT_ONLY | _lib.FLAG_DESCENDING], _lib.NA_LAST)):
-                    o, f, ng = engine.group([kd], fl, nap)
-                    res.append((sk, o.cpu().numpy(), None if f is None else f.cpu().numpy()))
-            finally:
-                engine.set_option("stage_keys", 0)
-        for a, b in zip(res[:2], res[2:]):
-            assert np.array_equal(a[1], b[1]) and (a[2] is None) == (b[2] is None) and (a[2] is None or np.array_equal(a[2], b[2]))
-
-
-def test_fused_stats_histogram_gives_identical_results():
-    """Single-column keys: the statistics kernel's per-tile histogram of the low 8 bits folded into the first
-    pass's digit counts (default) against the separate count kernel (option fuse_stats_hist = 0), and both
-    against the oracle; includes keys with constant low bits (the fold does not apply) and an all-NA column."""
+def test_single_key_first_pass_counts_vs_oracle():
+    """Single-column keys against the oracle.  The first pass's digit counts come from the statistics kernel's
+    per-tile histogram of the low 8 bits; keys with constant low bits take the count kernel instead (the fold
+    does not apply).  Includes an all-NA column."""
     import torch
     from datatable_b200 import engine, _lib
     from oracle import oracle as orc
@@ -508,17 +482,9 @@ def test_fused_stats_histogram_gives_identical_results():
     for st, k in cols:
         kd = engine.Col(torch.from_numpy(k).cuda(), st)
         for fl, nap in (([0], _lib.NA_FIRST), ([DESCENDING], _lib.NA_LAST), ([SORT_ONLY | DESCENDING], _lib.NA_FIRST)):
-            res = []
-            for fuse in (1, 0):
-                engine.set_option("fuse_stats_hist", fuse)
-                try:
-                    o, f, ng = engine.group([kd], fl, nap)
-                    res.append((o.cpu().numpy(), None if f is None else f.cpu().numpy()))
-                finally:
-                    engine.set_option("fuse_stats_hist", 1)
-            assert np.array_equal(res[0][0], res[1][0]), (st, fl, nap)
-            assert (res[0][1] is None) == (res[1][1] is None) and (res[0][1] is None or np.array_equal(res[0][1], res[1][1]))
+            o, f, ng = engine.group([kd], fl, nap)
             oo, of, _ = orc.group([k], fl, nap, stypes=[st])
-            assert np.array_equal(res[0][0], oo), (st, fl, nap)
+            assert np.array_equal(o.cpu().numpy(), oo), (st, fl, nap)
+            assert (f is None) == (of is None), (st, fl, nap)
             if of is not None:
-                assert np.array_equal(res[0][1], of)
+                assert np.array_equal(f.cpu().numpy(), of), (st, fl, nap)
