@@ -802,12 +802,18 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
         }
         DTB_TRY(bstart.alloc(bucket_starts_bytes(n) + sizeof(u32) * (size_t)(nb + 8), s));
         DTB_TRY(bscr.alloc(scr, s));
-        if (!bxk.p) {                                  // single raw key column: its normalised keys, once
+        // the sweep reads bxk[i] >> bshift = the row's group key
+        int bshift = rounds[0].kp.group_shift;
+        if (!bxk.p) {
+          // a single raw key column, or several whose composite is wider than 32 bits (by() + sort()): the
+          // group keys are composed once; a wider composite is stored as the group key itself
+          const int cshift = rounds[0].kp.total_bits > 32 ? bshift : 0;
           DTB_TRY(bxk.alloc(sizeof(u32) * (size_t)n, s));
-          ProfScope ps("compose_keys", s); DTB_TRY(launch_compose_keys(rounds[0].kp, n, nullptr, bxk.p, 4, s));
+          ProfScope ps("compose_keys", s); DTB_TRY(launch_compose_keys(rounds[0].kp, n, nullptr, bxk.p, 4, s, cshift));
+          bshift -= cshift;
         }
         u32* slab_starts = bstart.as<u32>(); u32* start = slab_starts + bucket_starts_bytes(n) / sizeof(u32);
-        DTB_TRY(launch_bucket_starts(bxk.as<u32>(), rounds[0].kp.group_shift, n, nb, slab_starts, start, s));
+        DTB_TRY(launch_bucket_starts(bxk.as<u32>(), bshift, n, nb, slab_starts, start, s));
         for (auto& sw : sweeps) {
           const void* vals[BK_MAXCOLS]; int sts[BK_MAXCOLS]; unsigned long long* words[BK_MAXCOLS][BK_NWORDS];
           const int nc = sw.second - sw.first;
@@ -816,7 +822,7 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
             vals[c] = bc.data; sts[c] = bc.stype;
             for (int w = 0; w < BK_NWORDS; w++) words[c][w] = bc.w[w];
           }
-          DTB_TRY(launch_bucketed_reduce(bxk.as<u32>(), rounds[0].kp.group_shift, dbits, nc, vals, sts, n, slab_starts,
+          DTB_TRY(launch_bucketed_reduce(bxk.as<u32>(), bshift, dbits, nc, vals, sts, n, slab_starts,
                                          start, words, bscr.p, s));
         }
       }
@@ -829,6 +835,15 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
         return stype_supported(sp.value.stype) ? DTB_EINVAL : DTB_ENOTIMPL;
       }
       DevBuf ob; DTB_TRY(ob.alloc_owned((size_t)(ng > 0 ? ng : 1) * stype_bytes(out_st), s));
+      GroupRows rows;                                  // streaming paths: every row is in a group (no NA_REMOVE)
+      rows.v = sp.value.data; rows.nv = n; rows.order = order; rows.offsets = offsets; rows.n = n;
+      DevBuf zscr;                                     // float min / max: the zero lookup's marks
+      const bool zero_sign = (sp.op == DTB_OP_MIN || sp.op == DTB_OP_MAX) &&
+                             (sp.value.stype == DTB_STYPE_FLOAT32 || sp.value.stype == DTB_STYPE_FLOAT64);
+      if (zero_sign && (bcol_of[i] >= 0 || fused_direct)) {
+        DTB_TRY(zscr.alloc(zero_fix_bytes(ng), s));
+        rows.zpos = zscr.as<u64>();
+      }
       if (sp.op == DTB_OP_NROWS) {
         DTB_TRY(launch_nrows(offsets, ng, ob.p, s));
       } else if (bcol_of[i] >= 0) {
@@ -843,7 +858,7 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
           case DTB_OP_COUNT: a0 = bc.w[BK_CNT]; break;
           default: a0 = bc.w[BK_CNTNA]; break;
         }
-        DTB_TRY(launch_direct_finalize(sp.op, sp.value.stype, a0, a1, res.gkeys.as<u32>(), ng, ob.p, s));
+        DTB_TRY(launch_direct_finalize(sp.op, sp.value.stype, a0, a1, res.gkeys.as<u32>(), ng, ob.p, rows, s));
       } else if (fused_direct) {
         u64* a0 = facc.as<u64>() + (size_t)ftable * 2 * i;
         u64* a1 = facc.as<u64>() + (size_t)ftable * (2 * i + 1);
@@ -852,11 +867,12 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
           DTB_TRY(launch_direct_accumulate(sp.op, rounds[0].kp, dp, sp.value.data, sp.value.stype, n, ftable, a0, a1, s));
         }
         DTB_TRY(launch_direct_finalize(sp.op, sp.value.stype, a0, a1,
-                                       (dp.kind == DIRECT_SMALL && dp.map) ? nullptr : res.gkeys.as<u32>(), ng, ob.p, s));
+                                       (dp.kind == DIRECT_SMALL && dp.map) ? nullptr : res.gkeys.as<u32>(), ng, ob.p,
+                                       rows, s));
       } else {
         DevIn dv; DTB_TRY(dv.bind(sp.value.data, (size_t)n * stype_bytes(sp.value.stype), s));
         DevBuf extra;
-        const size_t xb = reduce_extra_bytes(sp.op, ng, n);
+        const size_t xb = reduce_extra_bytes(sp.op, sp.value.stype, ng, n);
         if (xb) DTB_TRY(extra.alloc(xb, s));
         ProfScope ps("reduce", s);
         DTB_TRY(launch_reduce_impl(sp.op, dv.dptr, sp.value.stype, n, order + res.nskip, 0, offsets, ng,
@@ -900,6 +916,9 @@ struct dtb_reduce_state {
   void* dmap = nullptr;       // plan_direct's map (shared-memory table / hot-key modes)
   dtb::DirectPlan dp;
   int64_t rows_added = 0;
+  // float min / max: inverse RowIndex (int32[nrows]) and every group's first valid zero (u64[ngroups], GroupRows)
+  void* inv = nullptr;
+  void* first_zero = nullptr;
 };
 
 extern "C" {
@@ -1141,7 +1160,7 @@ static int reduce_groups(int op, dtb_col value, int64_t nrows_value, const void*
   DevOut d_out; DTB_TRY(d_out.bind(out, (size_t)ngroups * stype_bytes(out_st), s));
   DevBuf acc; DTB_TRY(acc.alloc(sizeof(u64) * (size_t)ngroups * 2, s));
   DevBuf extra;
-  const size_t xb = reduce_extra_bytes(op, ngroups, n);
+  const size_t xb = reduce_extra_bytes(op, value.stype, ngroups, n);
   if (xb) DTB_TRY(extra.alloc(xb, s));
   {
     ProfScope ps("reduce", s);
@@ -1188,9 +1207,17 @@ int dtb_groupby_reduce(dtb_groupby* g, int op, dtb_col value, int64_t nrows_valu
                       g->gmax, dmap.p, s, dp));
   {
     ProfScope ps("reduce_direct", s);
+    GroupRows rows;
+    rows.v = value.data; rows.nv = g->nrows; rows.order = g->order; rows.offsets = (const int32_t*)g->offsets;
+    rows.n = g->nrows;
+    DevBuf zscr;                                       // float min / max: the zero lookup's marks
+    if ((op == DTB_OP_MIN || op == DTB_OP_MAX) && (value.stype == DTB_STYPE_FLOAT32 || value.stype == DTB_STYPE_FLOAT64)) {
+      DTB_TRY(zscr.alloc(zero_fix_bytes(g->ngroups), s));
+      rows.zpos = zscr.as<u64>();
+    }
     DTB_TRY(launch_reduce_direct(op, g->kp, dp, value.data, value.stype, g->nrows, g->table,
                                  (const uint32_t*)g->gkeys, g->ngroups, acc.as<u64>(),
-                                 acc.as<u64>() + g->table, d_out.dptr, s));
+                                 acc.as<u64>() + g->table, d_out.dptr, rows, s));
   }
   if (d_out.staged()) {
     DTB_TRY(d_out.finish((size_t)g->ngroups * stype_bytes(out_st), s));
@@ -1226,8 +1253,22 @@ int dtb_groupby_reduce_begin(dtb_groupby* g, int op, int value_stype, dtb_stream
   if (g->ngroups > 0) {
     rc = plan_direct(g->table, (const uint32_t*)g->gkeys, (const int32_t*)g->offsets, g->ngroups, g->nrows, g->gmax, st->dmap, s, st->dp);
     if (rc == DTB_OK) rc = launch_direct_init(op, st->dp, g->table, (u64*)st->acc, (u64*)st->acc + g->table, s);
+    const bool zero_sign = (op == DTB_OP_MIN || op == DTB_OP_MAX) &&
+                           (value_stype == DTB_STYPE_FLOAT32 || value_stype == DTB_STYPE_FLOAT64);
+    if (rc == DTB_OK && zero_sign) {
+      if (cudaMalloc(&st->inv, sizeof(int32_t) * (size_t)g->nrows) != cudaSuccess ||
+          cudaMalloc(&st->first_zero, sizeof(u64) * (size_t)g->ngroups) != cudaSuccess) {
+        cudaGetLastError(); set_error("out of device memory"); rc = DTB_ENOMEM;
+      }
+      if (rc == DTB_OK) rc = launch_inverse_order((const int32_t*)g->order, g->nrows, (int32_t*)st->inv, s);
+      if (rc == DTB_OK) fill_u64((u64*)st->first_zero, g->ngroups, ~0ull, s);
+    }
   }
-  if (rc != DTB_OK) { cudaFree(st->acc); cudaFree(st->dmap); delete st; return rc; }
+  if (rc != DTB_OK) {
+    cudaStreamSynchronize(s);
+    cudaFree(st->acc); cudaFree(st->dmap); cudaFree(st->inv); cudaFree(st->first_zero); delete st;
+    return rc;
+  }
   *out = st;
   return DTB_OK;
 }
@@ -1246,6 +1287,9 @@ int dtb_groupby_reduce_add(dtb_reduce_state* st, const void* value_rows, int64_t
   ProfScope ps("reduce_direct", s);
   DTB_TRY(launch_direct_accumulate_rows(st->op, kp, st->dp, value_rows, st->stype, nrows, g->table,
                                         (u64*)st->acc, (u64*)st->acc + g->table, s));
+  if (st->first_zero)
+    DTB_TRY(launch_first_zero_rows(value_rows, st->stype, row0, nrows, (const int32_t*)st->inv, (const int32_t*)g->offsets,
+                                   g->ngroups, (u64*)st->first_zero, s));
   st->rows_added += nrows;
   return DTB_OK;
 }
@@ -1264,16 +1308,18 @@ int dtb_groupby_reduce_end(dtb_reduce_state* st, dtb_stream stream, void* out)
       rc = scope.rc;
       DevOut d_out;
       if (rc == DTB_OK) rc = d_out.bind(out, (size_t)g->ngroups * stype_bytes(st->out_stype), s);
+      GroupRows rows;
+      rows.first_zero = (const u64*)st->first_zero;
       if (rc == DTB_OK)
         rc = launch_direct_finalize(st->op, st->stype, (const u64*)st->acc, (const u64*)st->acc + g->table,
                                     (st->dp.kind == DIRECT_SMALL && st->dp.map) ? nullptr : (const uint32_t*)g->gkeys,
-                                    g->ngroups, d_out.dptr, s);
+                                    g->ngroups, d_out.dptr, rows, s);
       if (rc == DTB_OK && d_out.staged()) rc = d_out.finish((size_t)g->ngroups * stype_bytes(st->out_stype), s);
       if (rc == DTB_OK && cudaStreamSynchronize(s) != cudaSuccess) { set_error("cudaStreamSynchronize failed"); rc = DTB_ECUDA; }
     }
   }
   if (rc != DTB_OK) cudaStreamSynchronize(s);       // the tables may still be in use
-  cudaFree(st->acc); cudaFree(st->dmap);
+  cudaFree(st->acc); cudaFree(st->dmap); cudaFree(st->inv); cudaFree(st->first_zero);
   delete st;
   return rc;
 }

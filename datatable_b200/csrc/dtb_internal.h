@@ -94,9 +94,10 @@ struct PassPlan {
   int bits[MAX_PASSES];
 };
 
-// Composite key materialisation for multi-column keys: out[i] = X(row idx[i]) (idx NULL = identity).
+// Composite key materialisation for multi-column keys: out[i] = X(row idx[i]) >> out_shift (idx NULL = identity).
+// 4-byte keys must hold all total_bits - out_shift bits (DTB_EINVAL otherwise: never truncated).
 int launch_compose_keys(const KeyPlan& kp, int64_t n, const int32_t* idx, void* keys_out,
-                        int key_bytes, cudaStream_t s);
+                        int key_bytes, cudaStream_t s, int out_shift = 0);
 
 struct PassIO {
   int         src_kind;     // 0 packed keys + idx_in (idx_in NULL = identity), 1 raw column (identity idx)
@@ -151,13 +152,41 @@ int launch_mark_heads(const void* sorted_keys, int key_bytes, int group_shift, i
 // ---------------------------------------------------------------------------
 // Reducers / gather
 // ---------------------------------------------------------------------------
+// Float min / max whose result is a zero: the reference keeps the first value that is strictly better
+// (column/minmax.h:40-53), so the sign is that of the group's first valid zero in RowIndex order.  The
+// order-preserving images rank -0.0 below +0.0, so the finalize looks that zero up, in one of two ways:
+//   zpos (zero_fix_bytes(ngroups) of device scratch): the finalize marks the groups whose result is a zero, and one
+//        row-parallel pass over the value column seen through order[0 .. n) (order NULL = identity; it returns at
+//        once when no group was marked) finds each marked group's first valid zero;
+//   first_zero (reducers fed piecewise): first_zero[g] = (RowIndex position << 1 | sign bit) of that zero, ~0: none.
+// Neither set: the finalize keeps the zero it has.
+struct GroupRows {
+  const void* v = nullptr;
+  int64_t nv = 0;
+  const void* order = nullptr;
+  int order_is64 = 0;
+  const int32_t* offsets = nullptr;
+  int64_t n = 0;                                   // positions under the groups: offsets[ngroups]
+  unsigned long long* zpos = nullptr;
+  const unsigned long long* first_zero = nullptr;
+};
+size_t zero_fix_bytes(int64_t ngroups);
+
+// pos[g] = min(pos[g], first position p in group g whose row order[p] (order NULL = identity) holds a valid value,
+// and with zero_only a float zero).  Row-parallel: one read of the positions and the values, one atomic per thread
+// and group.  gate != NULL: nothing happens unless *gate != 0.  pos: the caller sets the groups it wants to ~0.
+int launch_first_valid_pos(const void* v, int stype, int64_t nv, const void* order, int order_is64, const int32_t* offsets,
+                           int64_t ngroups, int64_t n, int zero_only, const unsigned long long* gate,
+                           unsigned long long* pos, cudaStream_t s);
+
 // acc0/acc1: device scratch, ngroups uint64 each.  n = offsets[ngroups] (rows under the groups).
 int launch_reduce_impl(int op, const void* value, int stype, int64_t nrows_value,
                        const void* order, int order_is64, const int32_t* offsets, int64_t ngroups,
                        int64_t n, unsigned long long* acc0, unsigned long long* acc1,
                        void* out, cudaStream_t s, void* extra = nullptr);
-// device scratch `extra` that launch_reduce_impl needs for `op` (sd: m2[ng]; nunique: one flag byte per row)
-size_t reduce_extra_bytes(int op, int64_t ng, int64_t n);
+// device scratch `extra` that launch_reduce_impl needs for `op` (sd: m2[ng] and pivots[ng]; nunique: one flag byte per
+// row; float min / max: the zero lookup's marks, see GroupRows)
+size_t reduce_extra_bytes(int op, int stype, int64_t ng, int64_t n);
 int reduce_out_stype_host(int op, int stype);
 // *d_bad (device int, zeroed by the caller) = 1 + index of a group with offsets[g] >= offsets[g+1] (or offsets[0] != 0).
 int launch_offsets_check(const int32_t* offsets, int64_t ng, int* d_bad, cudaStream_t s);
@@ -178,7 +207,8 @@ int plan_direct(int64_t table, const uint32_t* gkeys, const int32_t* offsets, in
                 int64_t gmax, void* map_scratch, cudaStream_t s, DirectPlan& dp);
 int launch_reduce_direct(int op, const KeyPlan& kp, const DirectPlan& dp, const void* value, int stype, int64_t n,
                          int64_t table, const uint32_t* gkeys, int64_t ngroups,
-                         unsigned long long* acc0, unsigned long long* acc1, void* out, cudaStream_t s);
+                         unsigned long long* acc0, unsigned long long* acc1, void* out, const GroupRows& rows,
+                         cudaStream_t s);
 int launch_direct_accumulate(int op, const KeyPlan& kp, const DirectPlan& dp,
                              const void* value, int stype, int64_t n, int64_t table,
                              unsigned long long* acc0, unsigned long long* acc1, cudaStream_t s);
@@ -187,7 +217,13 @@ int launch_direct_init(int op, const DirectPlan& dp, int64_t table, unsigned lon
 int launch_direct_accumulate_rows(int op, const KeyPlan& kp, const DirectPlan& dp, const void* value, int stype, int64_t n,
                                   int64_t table, unsigned long long* acc0, unsigned long long* acc1, cudaStream_t s);
 int launch_direct_finalize(int op, int stype, const unsigned long long* acc0, const unsigned long long* acc1,
-                           const uint32_t* gkeys, int64_t ngroups, void* out, cudaStream_t s);
+                           const uint32_t* gkeys, int64_t ngroups, void* out, const GroupRows& rows, cudaStream_t s);
+// Reducers fed piecewise, float min / max: inv[order[p]] = p over the handle's RowIndex (n int32), then for every
+// piece the RowIndex position and sign of each group's first valid zero (GroupRows::first_zero, ngroups u64
+// set to ~0 by the caller).
+int launch_inverse_order(const int32_t* order, int64_t n, int32_t* inv, cudaStream_t s);
+int launch_first_zero_rows(const void* value_rows, int stype, int64_t row0, int64_t nrows, const int32_t* inv,
+                           const int32_t* offsets, int64_t ngroups, unsigned long long* first_zero, cudaStream_t s);
 int launch_nrows(const int32_t* offsets, int64_t ngroups, void* out, cudaStream_t s);
 int launch_group_keys(const void* sorted_keys, int key_bytes, const int32_t* offsets, int group_shift,
                       int64_t ngroups, uint32_t* gkeys, cudaStream_t s);
@@ -226,9 +262,9 @@ int launch_slice_groups_plan(const int32_t* offsets, int64_t ng, const SlicePara
                              int32_t* gsel, unsigned long long* totals, cudaStream_t s);
 int launch_slice_groups_emit(const int32_t* offsets, const SliceParams& p, const int32_t* offsets_out, const int32_t* gsel,
                              int64_t ng_out, int64_t nout, int32_t* gid, int32_t* rows_out, cudaStream_t s);
-// sum/cnt: the MEAN accumulators of the same column; m2: double[ng], zeroed
+// sum/cnt: u64[ng] each, m2: double[2 * ng] (m2, then the groups' pivots), all zeroed
 int launch_sd(const void* v, int stype, int64_t nv, const int32_t* order, const int32_t* offsets, int64_t ng, int64_t n,
-              const unsigned long long* sum, const unsigned long long* cnt, double* m2, void* out, cudaStream_t s);
+              unsigned long long* sum, unsigned long long* cnt, double* m2, void* out, cudaStream_t s);
 int launch_median(const void* v, int stype, int64_t nv, const int32_t* order, const int32_t* offsets,
                   int64_t ng, void* out, cudaStream_t s);
 int launch_distinct_flags(const void* v, int stype, int64_t nv, const int32_t* order, const int32_t* offsets,

@@ -5,7 +5,8 @@
 //
 //   first / last          expr/head_reduce_unary.cc:120-190   value of the first / last row of a group
 //   sd                    expr/head_reduce_unary.cc:197-245   sample standard deviation (Welford there;
-//                                                             here: mean, then sum of squared deviations)
+//                                                             here: two passes over the values shifted by the
+//                                                             group's first valid value)
 //   median                expr/head_reduce_unary.cc:421-468   over rows sorted inside their group
 //                                                             (Column::sort_grouped, sort.cc:1499-1530)
 //   nunique               expr/head_reduce_unary.cc:383-415   distinct valid values per group
@@ -111,36 +112,125 @@ int launch_expand_gid(const int32_t* offsets, int64_t ng, int64_t n, int32_t* gi
 }
 
 // ===========================================================================
-// sd, pass 2: acc[g] += (x - mean[g])^2 over the valid rows.  The mean comes from the MEAN accumulators
-// (sum, count); squared deviations from the group's own mean do not cancel the way sum(x^2) - n mean^2
-// does, so the result agrees with the reference's Welford recurrence to ~1e-15 relative.
+// first valid position of every group (sd's pivot, the sign of a zero min / max): row-parallel, in the shape of the
+// sd passes -- each thread owns 8 consecutive positions, finds its first group by bisection, and keeps the first
+// position of each of its groups that qualifies; one atomicMin per (thread, group).  A serial walk per group would
+// read a long NA prefix (or a late zero) one row at a time on one thread.
+// ===========================================================================
+template <typename T, typename OrdT>
+__global__ void first_valid_pos_kernel(const typename RawKey<T>::load_t* __restrict__ v, int64_t nv,
+                                       const OrdT* __restrict__ order, const int32_t* __restrict__ offsets, int64_t ng,
+                                       int64_t n, int zero_only, const u64* __restrict__ gate, u64* __restrict__ pos)
+{
+  typedef typename RawKey<T>::load_t L;
+  if (gate && *gate == 0) return;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x * 8;
+  for (int64_t p0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 8; p0 < n; p0 += stride) {
+    int64_t lo = 0, hi = ng;
+    while (hi - lo > 1) { const int64_t mid = (lo + hi) >> 1; if ((int64_t)offsets[mid] <= p0) lo = mid; else hi = mid; }
+    int64_t g = lo, next = offsets[g + 1];
+    u64 best = ~0ull;
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+      const int64_t p = p0 + i;
+      if (p >= n) break;
+      if (p >= next) {
+        if (best != ~0ull) atomicMin(&pos[g], best);
+        best = ~0ull;
+        while (p >= next) { g++; next = offsets[g + 1]; }
+      }
+      if (best != ~0ull) continue;
+      const int64_t j = order ? (int64_t)order[p] : p;
+      if (j < 0 || j >= nv) continue;
+      const L r = v[j];
+      u64 u;
+      if (RawKey<T>::get(r, u) && (!zero_only || (L)(r << 1) == 0)) best = (u64)p;
+    }
+    if (best != ~0ull) atomicMin(&pos[g], best);
+  }
+}
+
+int launch_first_valid_pos(const void* v, int stype, int64_t nv, const void* order, int order_is64, const int32_t* offsets,
+                           int64_t ng, int64_t n, int zero_only, const u64* gate, u64* pos, cudaStream_t s)
+{
+  if (ng == 0 || n == 0) return DTB_OK;
+  const int grid = grid_for((n + 7) / 8);
+#define CALL(T) { typedef typename RawKey<T>::load_t L;                                                             \
+                  if (order_is64) first_valid_pos_kernel<T, int64_t><<<grid, 256, 0, s>>>((const L*)v, nv,          \
+                                    (const int64_t*)order, offsets, ng, n, zero_only, gate, pos);                    \
+                  else            first_valid_pos_kernel<T, int32_t><<<grid, 256, 0, s>>>((const L*)v, nv,          \
+                                    (const int32_t*)order, offsets, ng, n, zero_only, gate, pos); }
+  DTB_DISPATCH_STYPE(stype, CALL)
+#undef CALL
+  count_launch();
+  DTB_CUDA_CHECK(cudaGetLastError());
+  return DTB_OK;
+}
+
+// ===========================================================================
+// sd: the valid rows of every group are shifted by a pivot p, the value of the group's first valid row in
+// RowIndex order, and then folded in two passes:
+//   pass 1: sum += x - p, cnt += 1                 (mean' = sum / cnt, the mean of the shifted values)
+//   pass 2: m2 += ((x - p) - mean')^2
+// A group whose valid values are all equal has x - p = 0 on every row, so its sd is exactly 0, as the
+// reference's Welford recurrence gives (a mean computed from the rounded sum is not the value itself: three
+// rows of 0.1 gave 1.7e-17).  Squared deviations from the group's own mean do not cancel the way
+// sum(x^2) - n mean^2 does, and the shift keeps them accurate when |mean| is much larger than the sd.
 // ===========================================================================
 template <typename T>
-__global__ void sqdev_kernel(const void* __restrict__ v, int64_t nv, const int32_t* __restrict__ order,
-                             const int32_t* __restrict__ offsets, int64_t ng, int64_t n,
-                             const u64* __restrict__ sum, const u64* __restrict__ cnt, double* __restrict__ acc)
+__device__ __forceinline__ double raw_double(typename RawKey<T>::load_t r) {
+  if constexpr (std::is_same<T, float>::value) return (double)__uint_as_float(r);
+  else if constexpr (std::is_same<T, double>::value) return __longlong_as_double((long long)r);
+  else return (double)r;
+}
+
+// pivot[g]: on entry, as u64, the group's first valid position (launch_first_valid_pos; ~0: none); on exit its value
+template <typename T>
+__global__ void sd_pivot_kernel(const void* __restrict__ v, const int32_t* __restrict__ order, int64_t ng,
+                                double* __restrict__ pivot)
+{
+  typedef typename RawKey<T>::load_t L;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += stride) {
+    const u64 p = reinterpret_cast<const u64*>(pivot)[g];
+    const int64_t j = (p == ~0ull) ? -1 : (order ? (int64_t)order[p] : (int64_t)p);
+    pivot[g] = (j >= 0) ? raw_double<T>(((const L*)v)[j]) : 0.0;   // no valid row: cnt stays 0 and the result is NA
+  }
+}
+
+template <typename T, bool SQ>
+__global__ void sd_pass_kernel(const void* __restrict__ v, int64_t nv, const int32_t* __restrict__ order,
+                               const int32_t* __restrict__ offsets, int64_t ng, int64_t n, const double* __restrict__ pivot,
+                               u64* __restrict__ sum, u64* __restrict__ cnt, double* __restrict__ m2)
 {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x * 8;
   for (int64_t p0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 8; p0 < n; p0 += stride) {
     int64_t lo = 0, hi = ng;
     while (hi - lo > 1) { const int64_t mid = (lo + hi) >> 1; if ((int64_t)offsets[mid] <= p0) lo = mid; else hi = mid; }
     int64_t g = lo, next = offsets[g + 1];
-    double mean = __longlong_as_double((long long)sum[g]) / (double)cnt[g];
-    double part = 0.0;
+    double piv = pivot[g], mean = SQ ? __longlong_as_double((long long)sum[g]) / (double)cnt[g] : 0.0;
+    double part = 0.0; u32 c = 0;
 #pragma unroll
     for (int i = 0; i < 8; i++) {
       const int64_t p = p0 + i;
       if (p >= n) break;
       if (p >= next) {
-        if (part != 0.0) atomicAdd(&acc[g], part);
-        part = 0.0;
+        if (SQ) { if (part != 0.0) atomicAdd(&m2[g], part); }
+        else if (c) { atomicAdd(reinterpret_cast<double*>(sum) + g, part); atomicAdd(&cnt[g], (u64)c); }
+        part = 0.0; c = 0;
         while (p >= next) { g++; next = offsets[g + 1]; }
-        mean = __longlong_as_double((long long)sum[g]) / (double)cnt[g];
+        piv = pivot[g];
+        if (SQ) mean = __longlong_as_double((long long)sum[g]) / (double)cnt[g];
       }
       const int64_t j = order ? (int64_t)order[p] : p;
-      if (j >= 0 && j < nv && elem_valid<T>(v, j)) { const double d = elem_double<T>(v, j) - mean; part += d * d; }
+      if (j >= 0 && j < nv && elem_valid<T>(v, j)) {
+        const double d = (elem_double<T>(v, j) - piv) - mean;
+        part += SQ ? d * d : d;
+        c++;
+      }
     }
-    if (part != 0.0) atomicAdd(&acc[g], part);
+    if (SQ) { if (part != 0.0) atomicAdd(&m2[g], part); }
+    else if (c) { atomicAdd(reinterpret_cast<double*>(sum) + g, part); atomicAdd(&cnt[g], (u64)c); }
   }
 }
 
@@ -158,15 +248,20 @@ __global__ void sd_finalize_kernel(const double* __restrict__ m2, const u64* __r
 }
 
 int launch_sd(const void* v, int stype, int64_t nv, const int32_t* order, const int32_t* offsets, int64_t ng, int64_t n,
-              const u64* sum, const u64* cnt, double* m2 /*zeroed*/, void* out, cudaStream_t s)
+              u64* sum, u64* cnt, double* m2, void* out, cudaStream_t s)
 {
   if (ng == 0) return DTB_OK;
   if (n > 0) {
+    double* pivot = m2 + ng;
     const int grid = grid_for((n + 7) / 8);
-#define CALL(T) sqdev_kernel<T><<<grid, 256, 0, s>>>(v, nv, order, offsets, ng, n, sum, cnt, m2)
+    fill_u64((u64*)pivot, ng, ~0ull, s);
+    DTB_TRY(launch_first_valid_pos(v, stype, nv, order, 0, offsets, ng, n, 0, nullptr, (u64*)pivot, s));
+#define CALL(T) sd_pivot_kernel<T><<<grid_for(ng), 256, 0, s>>>(v, order, ng, pivot); \
+                sd_pass_kernel<T, false><<<grid, 256, 0, s>>>(v, nv, order, offsets, ng, n, pivot, sum, cnt, m2); \
+                sd_pass_kernel<T, true><<<grid, 256, 0, s>>>(v, nv, order, offsets, ng, n, pivot, sum, cnt, m2)
     DTB_DISPATCH_STYPE(stype, CALL)
 #undef CALL
-    count_launch();
+    count_launch(3);
   }
   sd_finalize_kernel<<<grid_for(ng), 256, 0, s>>>(m2, cnt, ng, stype == DTB_STYPE_FLOAT32, out);
   count_launch();

@@ -50,7 +50,7 @@ __device__ __forceinline__ void compose_col4(const KeyNorm& k, const int64_t (&r
 
 template <typename KeyT>
 __global__ void __launch_bounds__(256)
-compose_keys_kernel(KeyPlan kp, int64_t n, const int32_t* __restrict__ idx, KeyT* __restrict__ out)
+compose_keys_kernel(KeyPlan kp, int64_t n, const int32_t* __restrict__ idx, KeyT* __restrict__ out, int out_shift)
 {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x * 4;
   for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x * 4 + threadIdx.x; i0 < n; i0 += stride) {
@@ -74,18 +74,22 @@ compose_keys_kernel(KeyPlan kp, int64_t n, const int32_t* __restrict__ idx, KeyT
       }
     }
 #pragma unroll
-    for (int r = 0; r < 4; r++) if (in[r]) out[i0 + (int64_t)r * blockDim.x] = (KeyT)x[r];
+    for (int r = 0; r < 4; r++) if (in[r]) out[i0 + (int64_t)r * blockDim.x] = (KeyT)(x[r] >> out_shift);
   }
 }
 
 int launch_compose_keys(const KeyPlan& kp, int64_t n, const int32_t* idx, void* keys_out, int key_bytes,
-                        cudaStream_t s)
+                        cudaStream_t s, int out_shift)
 {
+  if (key_bytes == 4 && kp.total_bits - out_shift > 32) {
+    set_error("internal: a " + std::to_string(kp.total_bits - out_shift) + "-bit key does not fit 32 bits");
+    return DTB_EINVAL;
+  }
   if (n == 0) return DTB_OK;
   int64_t want = (n + 1023) / 1024;
   int grid = (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : want);
-  if (key_bytes == 4) compose_keys_kernel<u32><<<grid, 256, 0, s>>>(kp, n, idx, (u32*)keys_out);
-  else                compose_keys_kernel<u64><<<grid, 256, 0, s>>>(kp, n, idx, (u64*)keys_out);
+  if (key_bytes == 4) compose_keys_kernel<u32><<<grid, 256, 0, s>>>(kp, n, idx, (u32*)keys_out, out_shift);
+  else                compose_keys_kernel<u64><<<grid, 256, 0, s>>>(kp, n, idx, (u64*)keys_out, out_shift);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;

@@ -222,8 +222,66 @@ __device__ __forceinline__ void store_result(void* out, int out_stype, int64_t g
   }
 }
 
+__device__ __forceinline__ bool is_float_zero(int stype, u64 bits) {
+  return ((stype == DTB_STYPE_FLOAT32) ? (bits << 33) : (bits << 1)) == 0;     // float32 bits sit in the low word
+}
+
+// bits: a float min / max result of group g that is a zero.  Its sign is that of the group's first valid zero in
+// RowIndex order: reducers fed piecewise have recorded it (first_zero); otherwise the group is marked for the
+// row-parallel lookup that follows the finalize (launch_zero_minmax_fix), and the word after the marks says so.
+__device__ __forceinline__ u64 zero_minmax_bits(const GroupRows& gr, int stype, int64_t g, int64_t ng, u64 bits) {
+  if (gr.first_zero) {
+    const u64 sign = (stype == DTB_STYPE_FLOAT32) ? 0x80000000ull : 0x8000000000000000ull;
+    const u64 f = gr.first_zero[g];
+    return f == ~0ull ? bits : ((f & 1) ? sign : 0ull);
+  }
+  if (gr.zpos) { gr.zpos[g] = ~0ull; *reinterpret_cast<volatile u64*>(gr.zpos + ng) = 1ull; }
+  return bits;
+}
+
+// out[g] = the group's first valid zero, for the groups marked by the finalize (zpos[g]: its RowIndex position,
+// found by launch_first_valid_pos).  Returns at once when the finalize marked no group.
+__global__ void zero_fix_kernel(int stype, const GroupRows gr, int64_t ng, void* out) {
+  if (gr.zpos[ng] == 0) return;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += stride) {
+    const u64 bits = (stype == DTB_STYPE_FLOAT32) ? (u64)((const u32*)out)[g] : ((const u64*)out)[g];
+    const u64 p = gr.zpos[g];
+    if (!is_float_zero(stype, bits) || p == ~0ull) continue;     // not marked (its word is not a position then)
+    const int64_t j = gr.order ? (gr.order_is64 ? ((const int64_t*)gr.order)[p] : (int64_t)((const int32_t*)gr.order)[p])
+                               : (int64_t)p;
+    if (stype == DTB_STYPE_FLOAT32) ((u32*)out)[g] = ((const u32*)gr.v)[j];
+    else                            ((u64*)out)[g] = ((const u64*)gr.v)[j];
+  }
+}
+
+size_t zero_fix_bytes(int64_t ng) { return sizeof(u64) * (size_t)((ng > 0 ? ng : 0) + 1); }
+
+static bool wants_zero_fix(int op, int stype, const GroupRows& gr) {
+  return gr.zpos && (op == DTB_OP_MIN || op == DTB_OP_MAX) && (stype == DTB_STYPE_FLOAT32 || stype == DTB_STYPE_FLOAT64);
+}
+
+// before the finalize: no group marked yet
+static int zero_fix_begin(int op, int stype, const GroupRows& gr, int64_t ng, cudaStream_t s) {
+  if (wants_zero_fix(op, stype, gr)) DTB_CUDA_CHECK(cudaMemsetAsync(gr.zpos + ng, 0, sizeof(u64), s));
+  return DTB_OK;
+}
+
+// after the finalize: one pass over the rows (it returns at once when no group was marked) finds the first valid
+// zero of every group, and the marked groups take its bits
+static int zero_fix_end(int op, int stype, const GroupRows& gr, int64_t ng, void* out, cudaStream_t s) {
+  if (!wants_zero_fix(op, stype, gr) || ng == 0) return DTB_OK;
+  DTB_TRY(launch_first_valid_pos(gr.v, stype, gr.nv, gr.order, gr.order_is64, gr.offsets, ng, gr.n, 1,
+                                 gr.zpos + ng, gr.zpos, s));
+  const int fgrid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
+  zero_fix_kernel<<<fgrid, 256, 0, s>>>(stype, gr, ng, out);
+  count_launch();
+  DTB_CUDA_CHECK(cudaGetLastError());
+  return DTB_OK;
+}
+
 __global__ void finalize_kernel(int op, int in_stype, int out_stype, const u64* __restrict__ acc0,
-                                const u64* __restrict__ acc1, int64_t ng, void* out)
+                                const u64* __restrict__ acc1, int64_t ng, void* out, const GroupRows gr)
 {
   const bool in_float = (in_stype == DTB_STYPE_FLOAT32 || in_stype == DTB_STYPE_FLOAT64);
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -246,6 +304,7 @@ __global__ void finalize_kernel(int op, int in_stype, int out_stype, const u64* 
         valid = is_min ? (a != ~0ull) : (a != 0ull);
         if (in_float) bits = (in_stype == DTB_STYPE_FLOAT32) ? (u64)f32_unimage((u32)a) : f64_unimage(a);
         else bits = (is_min ? a + 1 : a) ^ 0x8000000000000000ull;
+        if (in_float && valid && is_float_zero(in_stype, bits)) bits = zero_minmax_bits(gr, in_stype, g, ng, bits);
         break; }
       default: break;                                     // COUNT / COUNTNA: as is
     }
@@ -272,8 +331,10 @@ static int reduce_out_stype(int op, int st) {
   return 0;
 }
 
-size_t reduce_extra_bytes(int op, int64_t ng, int64_t n) {
-  if (op == DTB_OP_SD) return sizeof(double) * (size_t)(ng > 0 ? ng : 1);
+size_t reduce_extra_bytes(int op, int stype, int64_t ng, int64_t n) {
+  if (op == DTB_OP_SD) return 2 * sizeof(double) * (size_t)(ng > 0 ? ng : 1);      // m2, pivots
+  if ((op == DTB_OP_MIN || op == DTB_OP_MAX) && (stype == DTB_STYPE_FLOAT32 || stype == DTB_STYPE_FLOAT64))
+    return zero_fix_bytes(ng);
   if (op == DTB_OP_NUNIQUE) return (size_t)n + 16;
   return 0;
 }
@@ -343,7 +404,6 @@ int launch_reduce_impl(int op, const void* value, int stype, int64_t nv, const v
       fill_u64_kernel<<<fgrid, 256, 0, s>>>(acc1, ng, 0ull);
       fill_u64_kernel<<<fgrid, 256, 0, s>>>((u64*)extra, ng, 0ull);
       count_launch(3);
-      if (n > 0) DTB_TRY(dispatch_T<CAT_MEAN>(stype, value, nv, order, 0, offsets, ng, n, acc0, acc1, 0, s));
       return launch_sd(value, stype, nv, o32, offsets, ng, n, acc0, acc1, (double*)extra, out, s);
     }
     // NUNIQUE: flag the rows that start a new distinct value, then count the flags per group
@@ -352,7 +412,7 @@ int launch_reduce_impl(int op, const void* value, int stype, int64_t nv, const v
     fill_u64_kernel<<<fgrid, 256, 0, s>>>(acc0, ng, 0ull);
     count_launch();
     if (n > 0) DTB_TRY(dispatch_T<CAT_COUNT>(DTB_STYPE_INT8, flag, n, nullptr, 0, offsets, ng, n, acc0, acc1, 0, s));
-    finalize_kernel<<<fgrid, 256, 0, s>>>(DTB_OP_COUNT, DTB_STYPE_INT8, DTB_STYPE_INT64, acc0, acc1, ng, out);
+    finalize_kernel<<<fgrid, 256, 0, s>>>(DTB_OP_COUNT, DTB_STYPE_INT8, DTB_STYPE_INT64, acc0, acc1, ng, out, GroupRows());
     count_launch();
     DTB_CUDA_CHECK(cudaGetLastError());
     return DTB_OK;
@@ -385,10 +445,14 @@ int launch_reduce_impl(int op, const void* value, int stype, int64_t nv, const v
     }
     if (rc != DTB_OK) return rc;
   }
-  finalize_kernel<<<fgrid, 256, 0, s>>>(op, stype, out_st, acc0, acc1, ng, out);
+  GroupRows gr;                                 // extra: the zero lookup's marks, float min / max (reduce_extra_bytes)
+  gr.v = value; gr.nv = nv; gr.order = order; gr.order_is64 = order_is64; gr.offsets = offsets; gr.n = n;
+  gr.zpos = (u64*)extra;
+  DTB_TRY(zero_fix_begin(op, stype, gr, ng, s));
+  finalize_kernel<<<fgrid, 256, 0, s>>>(op, stype, out_st, acc0, acc1, ng, out, gr);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
-  return DTB_OK;
+  return zero_fix_end(op, stype, gr, ng, out, s);
 }
 
 int reduce_out_stype_host(int op, int st) { return reduce_out_stype(op, st); }
@@ -454,7 +518,7 @@ direct_reduce_kernel(KSrc ksrc, int gshift, const typename RawKey<T>::load_t* __
 
 __global__ void finalize_direct_kernel(int op, int in_stype, int out_stype, const u64* __restrict__ acc0,
                                        const u64* __restrict__ acc1, const u32* __restrict__ gkeys,
-                                       int64_t ng, void* out)
+                                       int64_t ng, void* out, const GroupRows gr)
 {
   const bool in_float = (in_stype == DTB_STYPE_FLOAT32 || in_stype == DTB_STYPE_FLOAT64);
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -477,6 +541,7 @@ __global__ void finalize_direct_kernel(int op, int in_stype, int out_stype, cons
         valid = is_min ? (a != ~0ull) : (a != 0ull);
         if (in_float) bits = (in_stype == DTB_STYPE_FLOAT32) ? (u64)f32_unimage((u32)a) : f64_unimage(a);
         else bits = (is_min ? a + 1 : a) ^ 0x8000000000000000ull;
+        if (in_float && valid && is_float_zero(in_stype, bits)) bits = zero_minmax_bits(gr, in_stype, g, ng, bits);
         break; }
       default: break;
     }
@@ -802,26 +867,72 @@ int launch_direct_accumulate_rows(int op, const KeyPlan& kp, const DirectPlan& d
 
 // Stage 2: out[g] = finalize(acc[gkeys[g]]) in the reference's output stype / NA rules.
 int launch_direct_finalize(int op, int stype, const u64* acc0, const u64* acc1, const uint32_t* gkeys,
-                           int64_t ng, void* out, cudaStream_t s)
+                           int64_t ng, void* out, const GroupRows& rows, cudaStream_t s)
 {
   const int out_st = reduce_out_stype(op, stype);
   if (!out_st) { set_error("Invalid column type in reducer"); return DTB_EINVAL; }
   if (ng == 0) return DTB_OK;
   const int fgrid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
-  finalize_direct_kernel<<<fgrid, 256, 0, s>>>(op, stype, out_st, acc0, acc1, gkeys, ng, out);
+  DTB_TRY(zero_fix_begin(op, stype, rows, ng, s));
+  finalize_direct_kernel<<<fgrid, 256, 0, s>>>(op, stype, out_st, acc0, acc1, gkeys, ng, out, rows);
+  count_launch();
+  DTB_CUDA_CHECK(cudaGetLastError());
+  return zero_fix_end(op, stype, rows, ng, out, s);
+}
+
+int launch_reduce_direct(int op, const KeyPlan& kp, const DirectPlan& dp, const void* value, int stype, int64_t n,
+                         int64_t table, const uint32_t* gkeys, int64_t ng, u64* acc0, u64* acc1,
+                         void* out, const GroupRows& rows, cudaStream_t s)
+{
+  if (ng == 0) return DTB_OK;
+  DTB_TRY(launch_direct_accumulate(op, kp, dp, value, stype, n, table, acc0, acc1, s));
+  return launch_direct_finalize(op, stype, acc0, acc1, (dp.kind == DIRECT_SMALL && dp.map) ? nullptr : gkeys,
+                                ng, out, rows, s);
+}
+
+// ---- reducers fed piecewise: the first valid zero of every group, for float min / max ----------------
+__global__ void inverse_order_kernel(const int32_t* __restrict__ order, int64_t n, int32_t* __restrict__ inv) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < n; p += stride) inv[order[p]] = (int32_t)p;
+}
+
+int launch_inverse_order(const int32_t* order, int64_t n, int32_t* inv, cudaStream_t s) {
+  if (n == 0) return DTB_OK;
+  const int grid = (int)((n + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (n + 255) / 256);
+  inverse_order_kernel<<<grid, 256, 0, s>>>(order, n, inv);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;
 }
 
-int launch_reduce_direct(int op, const KeyPlan& kp, const DirectPlan& dp, const void* value, int stype, int64_t n,
-                         int64_t table, const uint32_t* gkeys, int64_t ng, u64* acc0, u64* acc1,
-                         void* out, cudaStream_t s)
-{
-  if (ng == 0) return DTB_OK;
-  DTB_TRY(launch_direct_accumulate(op, kp, dp, value, stype, n, table, acc0, acc1, s));
-  return launch_direct_finalize(op, stype, acc0, acc1, (dp.kind == DIRECT_SMALL && dp.map) ? nullptr : gkeys,
-                                ng, out, s);
+// first_zero[g] = min over the piece's valid zeros of (RowIndex position << 1 | sign bit); g by bisection of offsets
+template <typename T>
+__global__ void first_zero_rows_kernel(const typename RawKey<T>::load_t* __restrict__ v, int64_t row0, int64_t nrows,
+                                       const int32_t* __restrict__ inv, const int32_t* __restrict__ offsets, int64_t ng,
+                                       u64* __restrict__ first_zero) {
+  constexpr int SIGN_SHIFT = sizeof(typename RawKey<T>::load_t) * 8 - 1;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nrows; i += stride) {
+    const typename RawKey<T>::load_t r = v[i];
+    if ((typename RawKey<T>::load_t)(r << 1) != 0) continue;        // not a zero (NaN never is)
+    const int64_t p = inv[row0 + i];
+    int64_t lo = 0, hi = ng;                                         // largest g with offsets[g] <= p
+    while (hi - lo > 1) { const int64_t mid = (lo + hi) >> 1; if ((int64_t)offsets[mid] <= p) lo = mid; else hi = mid; }
+    atomicMin(&first_zero[lo], ((u64)p << 1) | (u64)(r >> SIGN_SHIFT));
+  }
+}
+
+int launch_first_zero_rows(const void* value_rows, int stype, int64_t row0, int64_t nrows, const int32_t* inv,
+                           const int32_t* offsets, int64_t ng, u64* first_zero, cudaStream_t s) {
+  if (nrows == 0 || ng == 0) return DTB_OK;
+  const int grid = (int)((nrows + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (nrows + 255) / 256);
+  if (stype == DTB_STYPE_FLOAT32)
+    first_zero_rows_kernel<float><<<grid, 256, 0, s>>>((const u32*)value_rows, row0, nrows, inv, offsets, ng, first_zero);
+  else
+    first_zero_rows_kernel<double><<<grid, 256, 0, s>>>((const u64*)value_rows, row0, nrows, inv, offsets, ng, first_zero);
+  count_launch();
+  DTB_CUDA_CHECK(cudaGetLastError());
+  return DTB_OK;
 }
 
 // gkeys[g] = sorted_keys[offsets[g]] >> gshift  (the normalised key of every group)

@@ -202,10 +202,14 @@ DTB_API int         dtb_groupby_destroy(dtb_groupby* g, dtb_stream stream);
  *         NA results are written as the stype's NA sentinel.
  *   nrows_value : rows in the value column (bounds the gather).
  *
- * SUM over integers/bool, MIN, MAX, COUNT*, NROWS are bit-exact.  Floating
- * SUM/MEAN are accumulated in float64 with an unspecified association order:
- * within 1e-6 relative of the reference's sequential sum (float32 SUM: the
- * reference accumulates sequentially in float32, so agreement is O(n*2^-24)).
+ * SUM over integers/bool (wrapping modulo 2^64), MIN, MAX (the sign of a zero
+ * included: the group's first valid zero in RowIndex order), COUNT*, NROWS are
+ * bit-exact.  Floating SUM/MEAN are accumulated in float64 in an unspecified
+ * order: a group of m valid rows has a sum within gamma(m-1) * sum|x| of the
+ * exact sum, gamma(k) = k*u / (1 - k*u), u = 2^-53; MEAN is that sum over the
+ * count; float32 results add their final rounding.  A cancelling group can
+ * differ from the reference's sequential sum by that much, in relative terms
+ * without limit.  SD of a group whose valid values are all equal is 0.0.
  */
 DTB_API int dtb_reduce(int op, dtb_col value, int64_t nrows_value,
                const void* order, int order_is64,
@@ -234,6 +238,10 @@ DTB_API int dtb_groupby_reduce(dtb_groupby* g, int op, dtb_col value, int64_t nr
  *            (the caller orders it after the piece's upload); every row exactly once over all calls
  *   _end   : finalises into out (host or device, ngroups elements of dtb_reduce_out_stype) and frees the state
  *            (also on error).  Results as dtb_groupby_reduce.
+ * Float DTB_OP_MIN / DTB_OP_MAX: the sign of a zero result is that of the group's first valid zero in RowIndex
+ * order, and the values are gone by _end.  So the state also holds the inverse RowIndex, int32[nrows] (4 GB at
+ * 1e9 rows, for every such state alive at once), built by _begin, and the first zero of every group
+ * (uint64[ngroups]); every _add makes one more pass over its rows to update it.
  */
 typedef struct dtb_reduce_state dtb_reduce_state;
 DTB_API int dtb_groupby_reduce_begin(dtb_groupby* g, int op, int value_stype, dtb_stream stream, dtb_reduce_state** out);

@@ -21,7 +21,7 @@ def case_flags(case):
 
 
 def assert_reducer_equal(got, want, op, vst, ctx=""):
-    """Integers / counts / min / max bit-exact (NaN == NaN); float sums and means to 1e-6 relative
+    """Integers / counts / min / max bit-exact (NaN == NaN, -0.0 != +0.0); float sums and means to 1e-6 relative
     (north_star tolerance; the reference's own helper uses 1e-7, tests/__init__.py:65-143)."""
     got = np.asarray(got); want = np.asarray(want)
     assert got.shape == want.shape, f"{ctx}: shape {got.shape} != {want.shape}"
@@ -31,10 +31,12 @@ def assert_reducer_equal(got, want, op, vst, ctx=""):
         return
     nan_g, nan_w = np.isnan(got), np.isnan(want)
     assert np.array_equal(nan_g, nan_w), f"{ctx}: NA pattern differs"
-    g, w = got[~nan_g].astype(np.float64), want[~nan_w].astype(np.float64)
     if op in ("min", "max"):
-        assert np.array_equal(g, w), f"{ctx}: min/max must be exact"
+        # bit for bit: the sign of a zero is part of the result (-0.0 == +0.0 would hide it)
+        ui = np.uint32 if got.dtype == np.float32 else np.uint64
+        assert np.array_equal(got[~nan_g].view(ui), want[~nan_w].view(ui)), f"{ctx}: min/max must be bit-exact"
         return
+    g, w = got[~nan_g].astype(np.float64), want[~nan_w].astype(np.float64)
     rtol = 1e-6
     if vst == FLOAT32 and op == "sum":
         # the reference accumulates float32 sums sequentially in float32 (column/sumprod.h:47-54);
