@@ -381,6 +381,9 @@ def _evaluate(DT, j, by_, sort_, isel=None):
     """EvalContext::evaluate (eval_context.cc:144-172) for the hot-path shapes.
     isel: an integer or integer slice for `i` -- applied inside every group under by() / sort()
     (iexpr_->evaluate_iby, eval_context.cc:154-158), to the rows otherwise (evaluate_i, :159-163)."""
+    if by_ is not None and sort_ is not None and sort_.na_position == "remove":
+        # the rows dropped from the front of the RowIndex would still be counted by the groups
+        raise ValueError("na_position = \"remove\" in sort() is not supported together with by()")
     # Host columns are uploaded once (pinned memory -> DMA), the whole query then runs on
     # HBM-resident buffers, and only the result frame travels back.
     if torch is None or not torch.cuda.is_available():

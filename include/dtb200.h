@@ -138,6 +138,11 @@ DTB_API int dtb_init(int device);
  *                               returns an empty Groupby (sort.cc:1491-1493)
  *   *norder_out               : valid entries in order_out
  *
+ * Groups are defined by the LEADING run of columns without SORT_ONLY (sort.cc:1478-1480): a column after
+ * the first SORT_ONLY one only orders the rows, whatever its flag.  DTB_NA_REMOVE is refused with
+ * DTB_EINVAL when groups are requested (flags[0] without SORT_ONLY): the RowIndex would drop rows that
+ * the groups still count.  A single row is never removed (sort.cc:1435-1439).
+ *
  * Bit-exact with the reference for order and offsets.
  */
 DTB_API int dtb_group(const dtb_col* keys, int nkeys, const int* flags, int na_pos,
@@ -356,7 +361,9 @@ DTB_API int dtb_memcpy(void* dst, const void* src, int64_t nbytes, dtb_stream st
  * Engine options, the analogue of dt.options.sort.* (sort.cc:259-349).
  *   "radix_bits"   largest digit width of the LSD passes: 4..8, or 0 (default) = 8 bits (wider digits were
  *                  built and measured slower twice, DESIGN.md 4.2)
- *   "verbose"      1 = print the pass plan to stderr
+ *   "verbose"      1 = print the pass plan to stderr: the key columns' bits and shifts, and per sort round
+ *                  its passes, the pass that narrows 64-bit keys to 32 bits (-1 = none), whether the first pass
+ *                  takes the statistics kernel's histogram, and whether the last pass fills the count table
  *   "profile"      1 = bracket every kernel with CUDA events on the call's stream (the calls do not wait for
  *                  them; dtb_profile_count / dtb_profile_reset do)
  *   "bucketed_reducers" 1 (default) = value columns that would cost two or more L2 atomics per row (mean, or
