@@ -94,9 +94,10 @@ int bucket_num_slabs(int64_t n) { const int64_t r = bucket_slab_rows(n); return 
 int launch_bucket_starts(const u32* xkeys, int gshift, int64_t n, int nb, u32* hist, u32* bstart, cudaStream_t s)
 {
   const int nslabs = bucket_num_slabs(n);
-  prof_begin("bucket_count", s);
-  bucket_count_kernel<<<nslabs, 512, 0, s>>>(xkeys, gshift, n, bucket_slab_rows(n), hist);
-  prof_end(s);
+  {
+    ProfScope ps("bucket_count", s);
+    bucket_count_kernel<<<nslabs, 512, 0, s>>>(xkeys, gshift, n, bucket_slab_rows(n), hist);
+  }
   bucket_scan_kernel<<<1, BK_MAXB, 0, s>>>(hist, nslabs, nb, bstart);
   count_launch(2);
   DTB_CUDA_CHECK(cudaGetLastError());
@@ -400,9 +401,10 @@ int launch_bucketed_reduce(const u32* xkeys, int gshift, int dbits, int ncols, c
   const size_t sm_scatter = (size_t)4 * BK_TILE + (size_t)stage_bytes * (ncols > 1 ? 2 : 1);
   // 1024 threads x 4 rows: 32 registers, two CTAs = every warp slot of the SM (512 x 8 at 64 registers measured slower)
   DTB_CUDA_CHECK(cudaFuncSetAttribute(bucket_scatter_kernel<1024, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 20 * BK_TILE));
-  prof_begin("bucket_scatter", s);
-  bucket_scatter_kernel<1024, 4><<<tiles, 1024, sm_scatter, s>>>(xkeys, gshift, n, slab_rows, cursor, xlow, cols, stage_bytes);
-  prof_end(s);
+  {
+    ProfScope ps("bucket_scatter", s);
+    bucket_scatter_kernel<1024, 4><<<tiles, 1024, sm_scatter, s>>>(xkeys, gshift, n, slab_rows, cursor, xlow, cols, stage_bytes);
+  }
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
 
@@ -410,7 +412,7 @@ int launch_bucketed_reduce(const u32* xkeys, int gshift, int dbits, int ncols, c
   for (int c = 0; c < ncols; c++) {
     BucketAcc acc;
     for (int w = 0; w < BK_NWORDS; w++) acc.w[w] = acc_w[c][w];
-    prof_begin("bucket_aggregate", s);
+    ProfScope ps("bucket_aggregate", s);
     const size_t smem = (size_t)cols.esz[c] * BK_ATILE + sizeof(u32) * BK_KEYS;
 #define DTB_AGG(T) { DTB_CUDA_CHECK(cudaFuncSetAttribute(bucket_aggregate_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
                      bucket_aggregate_kernel<T><<<chunks, BK_THREADS, smem, s>>>(xlow, (const typename RawKey<T>::load_t*)cols.out[c], start, nb, n, acc); }
@@ -424,7 +426,6 @@ int launch_bucketed_reduce(const u32* xkeys, int gshift, int dbits, int ncols, c
       default: set_error("unsupported stype"); return DTB_ENOTIMPL;
     }
 #undef DTB_AGG
-    prof_end(s);
     count_launch();
     DTB_CUDA_CHECK(cudaGetLastError());
   }

@@ -15,9 +15,13 @@ constexpr int MAX_PASSES = 16;
 // Thread-local error slot + launch counter (dtb_api.cu)
 void set_error(const std::string& msg);
 void count_launch(int n = 1);
-// Optional CUDA-event timing of a kernel family (option "profile"); no-ops otherwise.
-void prof_begin(const char* name, cudaStream_t s);
-void prof_end(cudaStream_t s);
+// Optional CUDA-event timing of a kernel family (option "profile"; a no-op otherwise): the work enqueued on `s`
+// while the scope lives, recorded on every way out of it.
+struct ProfScope {
+  ProfScope(const char* name, cudaStream_t s);
+  ~ProfScope();
+  bool on; cudaStream_t s; const char* name; cudaEvent_t a, b;
+};
 
 #define DTB_CUDA_CHECK(expr)                                                     \
   do {                                                                           \
@@ -171,6 +175,8 @@ struct GroupRows {
   const unsigned long long* first_zero = nullptr;
 };
 size_t zero_fix_bytes(int64_t ngroups);
+// The reducer is a float min / max: the sign of a zero result needs the lookup above.
+bool minmax_zero_sign(int op, int stype);
 
 // pos[g] = min(pos[g], first position p in group g whose row order[p] (order NULL = identity) holds a valid value,
 // and with zero_only a float zero).  Row-parallel: one read of the positions and the values, one atomic per thread
@@ -205,19 +211,14 @@ size_t direct_map_bytes(int64_t table);
 // map it needs in map_scratch (direct_map_bytes(table) bytes, device).
 int plan_direct(int64_t table, const uint32_t* gkeys, const int32_t* offsets, int64_t ngroups, int64_t n,
                 int64_t gmax, void* map_scratch, cudaStream_t s, DirectPlan& dp);
-int launch_reduce_direct(int op, const KeyPlan& kp, const DirectPlan& dp, const void* value, int stype, int64_t n,
-                         int64_t table, const uint32_t* gkeys, int64_t ngroups,
-                         unsigned long long* acc0, unsigned long long* acc1, void* out, const GroupRows& rows,
-                         cudaStream_t s);
-int launch_direct_accumulate(int op, const KeyPlan& kp, const DirectPlan& dp,
-                             const void* value, int stype, int64_t n, int64_t table,
-                             unsigned long long* acc0, unsigned long long* acc1, cudaStream_t s);
-// gkeys == NULL: the accumulators are indexed by group (dense-mapped small table).
+// The accumulator tables' identities (once per reducer; the rows may then arrive in pieces), then the rows.
 int launch_direct_init(int op, const DirectPlan& dp, int64_t table, unsigned long long* acc0, unsigned long long* acc1, cudaStream_t s);
 int launch_direct_accumulate_rows(int op, const KeyPlan& kp, const DirectPlan& dp, const void* value, int stype, int64_t n,
-                                  int64_t table, unsigned long long* acc0, unsigned long long* acc1, cudaStream_t s);
+                                  unsigned long long* acc0, unsigned long long* acc1, cudaStream_t s);
+// out[g] from the accumulators of group key gkeys[g], or of group g when dp is a dense-mapped small table.
 int launch_direct_finalize(int op, int stype, const unsigned long long* acc0, const unsigned long long* acc1,
-                           const uint32_t* gkeys, int64_t ngroups, void* out, const GroupRows& rows, cudaStream_t s);
+                           const DirectPlan& dp, const uint32_t* gkeys, int64_t ngroups, void* out, const GroupRows& rows,
+                           cudaStream_t s);
 // Reducers fed piecewise, float min / max: inv[order[p]] = p over the handle's RowIndex (n int32), then for every
 // piece the RowIndex position and sign of each group's first valid zero (GroupRows::first_zero, ngroups u64
 // set to ~0 by the caller).

@@ -570,9 +570,8 @@ static int run_scatter(Src src, const PassIO& io, int64_t n, int shift, u32 mask
       bits <= 6 ? scatter_kernel<KeyT, Src, NBINS, MINB, 6>
     : bits == 7 ? scatter_kernel<KeyT, Src, NBINS, MINB, 7> : scatter_kernel<KeyT, Src, NBINS, MINB, 8>;
   DTB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  prof_begin("radix_scatter", s);
+  ProfScope ps("radix_scatter", s);
   kern<<<(unsigned)ntiles, PASS_THREADS, smem, s>>>(a);
-  prof_end(s);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;
@@ -590,17 +589,18 @@ static int run_pass_nb(Src src, const PassIO& io, int64_t n, int shift, int bits
   unsigned short* tile_counts = reinterpret_cast<unsigned short*>(base + NBINS);   // [ntiles][NBINS]
   const u32 mask = (1u << bits) - 1;
 
-  prof_begin("radix_count", s);
-  if (io.raw_hist && shift != 0) { set_error("internal: a folded histogram needs shift 0"); return DTB_EINVAL; }
-  if (io.raw_hist) {
-    static_assert(NBINS == 256, "the statistics kernel counts 256 bins per tile");
-    const KeyNorm& k = src.key_norm();
-    fold_counts_kernel<<<(unsigned)nchunks, 256, 0, s>>>(io.raw_hist, io.raw_na, ntiles, (u32)k.edge & 255u, (u32)k.inc & 255u,
-                                                       k.desc, (u32)k.na_value & mask, mask, counts, tile_counts);
-  } else {
-    count_kernel<KeyT, Src, NBINS><<<(unsigned)nchunks, PASS_THREADS, 0, s>>>(src, n, shift, mask, counts, tile_counts);
+  {
+    ProfScope ps("radix_count", s);
+    if (io.raw_hist && shift != 0) { set_error("internal: a folded histogram needs shift 0"); return DTB_EINVAL; }
+    if (io.raw_hist) {
+      static_assert(NBINS == 256, "the statistics kernel counts 256 bins per tile");
+      const KeyNorm& k = src.key_norm();
+      fold_counts_kernel<<<(unsigned)nchunks, 256, 0, s>>>(io.raw_hist, io.raw_na, ntiles, (u32)k.edge & 255u, (u32)k.inc & 255u,
+                                                         k.desc, (u32)k.na_value & mask, mask, counts, tile_counts);
+    } else {
+      count_kernel<KeyT, Src, NBINS><<<(unsigned)nchunks, PASS_THREADS, 0, s>>>(src, n, shift, mask, counts, tile_counts);
+    }
   }
-  prof_end(s);
   chunk_scan_kernel<<<NBINS, 256, 0, s>>>(counts, nchunks, NBINS, total);
   digit_base_kernel<NBINS><<<1, 256, 0, s>>>(total, base);
   count_launch(3);

@@ -257,9 +257,11 @@ __global__ void zero_fix_kernel(int stype, const GroupRows gr, int64_t ng, void*
 
 size_t zero_fix_bytes(int64_t ng) { return sizeof(u64) * (size_t)((ng > 0 ? ng : 0) + 1); }
 
-static bool wants_zero_fix(int op, int stype, const GroupRows& gr) {
-  return gr.zpos && (op == DTB_OP_MIN || op == DTB_OP_MAX) && (stype == DTB_STYPE_FLOAT32 || stype == DTB_STYPE_FLOAT64);
+bool minmax_zero_sign(int op, int stype) {
+  return (op == DTB_OP_MIN || op == DTB_OP_MAX) && (stype == DTB_STYPE_FLOAT32 || stype == DTB_STYPE_FLOAT64);
 }
+
+static bool wants_zero_fix(int op, int stype, const GroupRows& gr) { return gr.zpos && minmax_zero_sign(op, stype); }
 
 // before the finalize: no group marked yet
 static int zero_fix_begin(int op, int stype, const GroupRows& gr, int64_t ng, cudaStream_t s) {
@@ -333,8 +335,7 @@ static int reduce_out_stype(int op, int st) {
 
 size_t reduce_extra_bytes(int op, int stype, int64_t ng, int64_t n) {
   if (op == DTB_OP_SD) return 2 * sizeof(double) * (size_t)(ng > 0 ? ng : 1);      // m2, pivots
-  if ((op == DTB_OP_MIN || op == DTB_OP_MAX) && (stype == DTB_STYPE_FLOAT32 || stype == DTB_STYPE_FLOAT64))
-    return zero_fix_bytes(ng);
+  if (minmax_zero_sign(op, stype)) return zero_fix_bytes(ng);
   if (op == DTB_OP_NUNIQUE) return (size_t)n + 16;
   return 0;
 }
@@ -417,12 +418,7 @@ int launch_reduce_impl(int op, const void* value, int stype, int64_t nv, const v
     DTB_CUDA_CHECK(cudaGetLastError());
     return DTB_OK;
   }
-  if (op == DTB_OP_NROWS) {
-    nrows_kernel<<<fgrid, 256, 0, s>>>(offsets, ng, (int64_t*)out);
-    count_launch();
-    DTB_CUDA_CHECK(cudaGetLastError());
-    return DTB_OK;
-  }
+  if (op == DTB_OP_NROWS) return launch_nrows(offsets, ng, out, s);
   const bool isflt = (stype == DTB_STYPE_FLOAT32 || stype == DTB_STYPE_FLOAT64);
   u64 init0 = (op == DTB_OP_MIN) ? ~0ull : 0ull;          // 0.0 == 0 bits for float sums
   fill_u64_kernel<<<fgrid, 256, 0, s>>>(acc0, ng, init0);
@@ -697,25 +693,23 @@ direct_reduce_hot_kernel(KSrc ksrc, int gshift, const typename RawKey<T>::load_t
     if (hkey[i] != HOT_EMPTY) slot_flush<CAT>(h0[i], h1[i], (int64_t)hkey[i], acc0, acc1, flag);
 }
 
-static thread_local DirectPlan t_dp = {DIRECT_PLAIN, nullptr, 0};
-
 template <typename T, int CAT, typename KSrc>
-static int run_direct(const KSrc& ks, int gshift, const void* v, int64_t n, u64* acc0, u64* acc1, int flag,
-                      cudaStream_t s)
+static int run_direct(const DirectPlan& dp, const KSrc& ks, int gshift, const void* v, int64_t n, u64* acc0, u64* acc1,
+                      int flag, cudaStream_t s)
 {
   typedef typename RawKey<T>::load_t L;
   int64_t want = (n + 511) / 512;
-  if (t_dp.kind == DIRECT_SMALL) {
+  if (dp.kind == DIRECT_SMALL) {
     int grid = (int)(want > NUM_SMS * 4 ? NUM_SMS * 4 : want);
-    direct_reduce_small_kernel<T, CAT, KSrc><<<grid, 512, 0, s>>>(ks, gshift, (const L*)v, n, (int)t_dp.nslots,
-                                                                  (const uint16_t*)t_dp.map, acc0, acc1, flag);
+    direct_reduce_small_kernel<T, CAT, KSrc><<<grid, 512, 0, s>>>(ks, gshift, (const L*)v, n, (int)dp.nslots,
+                                                                  (const uint16_t*)dp.map, acc0, acc1, flag);
     count_launch();
     DTB_CUDA_CHECK(cudaGetLastError());
     return DTB_OK;
   }
-  if (t_dp.kind == DIRECT_HOT) {
+  if (dp.kind == DIRECT_HOT) {
     int grid = (int)(want > NUM_SMS * 4 ? NUM_SMS * 4 : want);
-    direct_reduce_hot_kernel<T, CAT, KSrc><<<grid, 512, 0, s>>>(ks, gshift, (const L*)v, n, (const uint8_t*)t_dp.map,
+    direct_reduce_hot_kernel<T, CAT, KSrc><<<grid, 512, 0, s>>>(ks, gshift, (const L*)v, n, (const uint8_t*)dp.map,
                                                                 acc0, acc1, flag);
     count_launch();
     DTB_CUDA_CHECK(cudaGetLastError());
@@ -729,40 +723,40 @@ static int run_direct(const KSrc& ks, int gshift, const void* v, int64_t n, u64*
 }
 
 template <int CAT, typename KSrc>
-static int direct_T(int st, const KSrc& ks, int gshift, const void* v, int64_t n, u64* acc0, u64* acc1,
-                    int flag, cudaStream_t s)
+static int direct_T(const DirectPlan& dp, int st, const KSrc& ks, int gshift, const void* v, int64_t n, u64* acc0,
+                    u64* acc1, int flag, cudaStream_t s)
 {
   switch (st) {
     case DTB_STYPE_BOOL: case DTB_STYPE_INT8:
-      if constexpr (CAT != CAT_SUMF) return run_direct<int8_t, CAT>(ks, gshift, v, n, acc0, acc1, flag, s); break;
+      if constexpr (CAT != CAT_SUMF) return run_direct<int8_t, CAT>(dp, ks, gshift, v, n, acc0, acc1, flag, s); break;
     case DTB_STYPE_INT16:
-      if constexpr (CAT != CAT_SUMF) return run_direct<int16_t, CAT>(ks, gshift, v, n, acc0, acc1, flag, s); break;
+      if constexpr (CAT != CAT_SUMF) return run_direct<int16_t, CAT>(dp, ks, gshift, v, n, acc0, acc1, flag, s); break;
     case DTB_STYPE_INT32:
-      if constexpr (CAT != CAT_SUMF) return run_direct<int32_t, CAT>(ks, gshift, v, n, acc0, acc1, flag, s); break;
+      if constexpr (CAT != CAT_SUMF) return run_direct<int32_t, CAT>(dp, ks, gshift, v, n, acc0, acc1, flag, s); break;
     case DTB_STYPE_INT64:
-      if constexpr (CAT != CAT_SUMF) return run_direct<int64_t, CAT>(ks, gshift, v, n, acc0, acc1, flag, s); break;
+      if constexpr (CAT != CAT_SUMF) return run_direct<int64_t, CAT>(dp, ks, gshift, v, n, acc0, acc1, flag, s); break;
     case DTB_STYPE_FLOAT32:
-      if constexpr (CAT != CAT_SUMI) return run_direct<float, CAT>(ks, gshift, v, n, acc0, acc1, flag, s); break;
+      if constexpr (CAT != CAT_SUMI) return run_direct<float, CAT>(dp, ks, gshift, v, n, acc0, acc1, flag, s); break;
     case DTB_STYPE_FLOAT64:
-      if constexpr (CAT != CAT_SUMI) return run_direct<double, CAT>(ks, gshift, v, n, acc0, acc1, flag, s); break;
+      if constexpr (CAT != CAT_SUMI) return run_direct<double, CAT>(dp, ks, gshift, v, n, acc0, acc1, flag, s); break;
   }
   set_error("internal: reducer/stype combination"); return DTB_EINVAL;
 }
 
 template <typename KSrc>
-static int direct_op(int op, int st, const KSrc& ks, int gshift, const void* v, int64_t n, u64* acc0,
-                     u64* acc1, cudaStream_t s)
+static int direct_op(const DirectPlan& dp, int op, int st, const KSrc& ks, int gshift, const void* v, int64_t n,
+                     u64* acc0, u64* acc1, cudaStream_t s)
 {
   const bool isflt = (st == DTB_STYPE_FLOAT32 || st == DTB_STYPE_FLOAT64);
   switch (op) {
     case DTB_OP_SUM:
-      return isflt ? direct_T<CAT_SUMF>(st, ks, gshift, v, n, acc0, acc1, 0, s)
-                   : direct_T<CAT_SUMI>(st, ks, gshift, v, n, acc0, acc1, 0, s);
-    case DTB_OP_MEAN:    return direct_T<CAT_MEAN>(st, ks, gshift, v, n, acc0, acc1, 0, s);
-    case DTB_OP_MIN:     return direct_T<CAT_MINMAX>(st, ks, gshift, v, n, acc0, acc1, 1, s);
-    case DTB_OP_MAX:     return direct_T<CAT_MINMAX>(st, ks, gshift, v, n, acc0, acc1, 0, s);
-    case DTB_OP_COUNT:   return direct_T<CAT_COUNT>(st, ks, gshift, v, n, acc0, acc1, 0, s);
-    case DTB_OP_COUNTNA: return direct_T<CAT_COUNT>(st, ks, gshift, v, n, acc0, acc1, 1, s);
+      return isflt ? direct_T<CAT_SUMF>(dp, st, ks, gshift, v, n, acc0, acc1, 0, s)
+                   : direct_T<CAT_SUMI>(dp, st, ks, gshift, v, n, acc0, acc1, 0, s);
+    case DTB_OP_MEAN:    return direct_T<CAT_MEAN>(dp, st, ks, gshift, v, n, acc0, acc1, 0, s);
+    case DTB_OP_MIN:     return direct_T<CAT_MINMAX>(dp, st, ks, gshift, v, n, acc0, acc1, 1, s);
+    case DTB_OP_MAX:     return direct_T<CAT_MINMAX>(dp, st, ks, gshift, v, n, acc0, acc1, 0, s);
+    case DTB_OP_COUNT:   return direct_T<CAT_COUNT>(dp, st, ks, gshift, v, n, acc0, acc1, 0, s);
+    case DTB_OP_COUNTNA: return direct_T<CAT_COUNT>(dp, st, ks, gshift, v, n, acc0, acc1, 1, s);
   }
   set_error("unknown reducer"); return DTB_EINVAL;
 }
@@ -810,16 +804,8 @@ int plan_direct(int64_t table, const uint32_t* gkeys, const int32_t* offsets, in
 }
 
 // Stage 1: stream every row into acc[x] (acc[group] for a dense-mapped small table).  acc0/acc1: device
-// scratch of `table` u64 each.
-int launch_direct_accumulate(int op, const KeyPlan& kp, const DirectPlan& dp,
-                             const void* value, int stype, int64_t n, int64_t table,
-                             u64* acc0, u64* acc1, cudaStream_t s)
-{
-  DTB_TRY(launch_direct_init(op, dp, table, acc0, acc1, s));
-  return launch_direct_accumulate_rows(op, kp, dp, value, stype, n, table, acc0, acc1, s);
-}
-
-// the accumulator tables' identities (once per reducer; the rows may then arrive in pieces)
+// scratch of `table` u64 each.  First the accumulator tables' identities (once per reducer; the rows may then
+// arrive in pieces):
 int launch_direct_init(int op, const DirectPlan& dp, int64_t table, u64* acc0, u64* acc1, cudaStream_t s)
 {
   if (dp.kind == DIRECT_SMALL) table = dp.nslots;                // only the used accumulators are initialised
@@ -833,19 +819,16 @@ int launch_direct_init(int op, const DirectPlan& dp, int64_t table, u64* acc0, u
 
 // folds n rows (kp's key columns and `value`, both starting at the piece's first row) into the tables
 int launch_direct_accumulate_rows(int op, const KeyPlan& kp, const DirectPlan& dp,
-                                  const void* value, int stype, int64_t n, int64_t table,
-                                  u64* acc0, u64* acc1, cudaStream_t s)
+                                  const void* value, int stype, int64_t n, u64* acc0, u64* acc1, cudaStream_t s)
 {
   const int out_st = reduce_out_stype(op, stype);
   if (!out_st) { set_error("Invalid column type in reducer"); return DTB_EINVAL; }
-  t_dp = dp;
-  (void)table;
   if (n > 0) {
     int rc;
     if (kp.nkeys == 1) {
       const KeyNorm& k = kp.k[0];
 #define DTB_CASE(TK) { DirectRawKey<TK> ks; ks.src.init(k); \
-                       rc = direct_op(op, stype, ks, kp.group_shift, value, n, acc0, acc1, s); break; }
+                       rc = direct_op(dp, op, stype, ks, kp.group_shift, value, n, acc0, acc1, s); break; }
       switch (k.stype) {
         case DTB_STYPE_BOOL: case DTB_STYPE_INT8:    DTB_CASE(int8_t)
         case DTB_STYPE_INT16:                        DTB_CASE(int16_t)
@@ -858,36 +841,28 @@ int launch_direct_accumulate_rows(int op, const KeyPlan& kp, const DirectPlan& d
 #undef DTB_CASE
     } else {
       DirectComposite ks; ks.kp = kp;
-      rc = direct_op(op, stype, ks, kp.group_shift, value, n, acc0, acc1, s);
+      rc = direct_op(dp, op, stype, ks, kp.group_shift, value, n, acc0, acc1, s);
     }
     if (rc != DTB_OK) return rc;
   }
   return DTB_OK;
 }
 
-// Stage 2: out[g] = finalize(acc[gkeys[g]]) in the reference's output stype / NA rules.
-int launch_direct_finalize(int op, int stype, const u64* acc0, const u64* acc1, const uint32_t* gkeys,
-                           int64_t ng, void* out, const GroupRows& rows, cudaStream_t s)
+// Stage 2: out[g] = finalize(acc[gkeys[g]]) in the reference's output stype / NA rules; a dense-mapped small table
+// holds acc[g] already.
+int launch_direct_finalize(int op, int stype, const u64* acc0, const u64* acc1, const DirectPlan& dp,
+                           const uint32_t* gkeys, int64_t ng, void* out, const GroupRows& rows, cudaStream_t s)
 {
   const int out_st = reduce_out_stype(op, stype);
   if (!out_st) { set_error("Invalid column type in reducer"); return DTB_EINVAL; }
   if (ng == 0) return DTB_OK;
+  if (dp.kind == DIRECT_SMALL && dp.map) gkeys = nullptr;
   const int fgrid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
   DTB_TRY(zero_fix_begin(op, stype, rows, ng, s));
   finalize_direct_kernel<<<fgrid, 256, 0, s>>>(op, stype, out_st, acc0, acc1, gkeys, ng, out, rows);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return zero_fix_end(op, stype, rows, ng, out, s);
-}
-
-int launch_reduce_direct(int op, const KeyPlan& kp, const DirectPlan& dp, const void* value, int stype, int64_t n,
-                         int64_t table, const uint32_t* gkeys, int64_t ng, u64* acc0, u64* acc1,
-                         void* out, const GroupRows& rows, cudaStream_t s)
-{
-  if (ng == 0) return DTB_OK;
-  DTB_TRY(launch_direct_accumulate(op, kp, dp, value, stype, n, table, acc0, acc1, s));
-  return launch_direct_finalize(op, stype, acc0, acc1, (dp.kind == DIRECT_SMALL && dp.map) ? nullptr : gkeys,
-                                ng, out, rows, s);
 }
 
 // ---- reducers fed piecewise: the first valid zero of every group, for float min / max ----------------

@@ -93,12 +93,9 @@ def _alloc(n, st, device):
     return a, a.ctypes.data
 
 
-def group(cols, flags=None, na_pos=NA_FIRST):
-    """group() of the reference: returns (order, offsets, ngroups).
-
-    order   : int32 RowIndex (ARR32) -- stable order of the rows
-    offsets : int32[ngroups+1] Groupby offsets, or None when flags[0] has SORT_ONLY
-    """
+def _keys(cols, flags):
+    """Key columns and flags as the C-ABI takes them: (cols, nrows, flags, ckeys, cflags).  The library reads
+    nrows rows of every key column, so they must all have that many."""
     cols = [Col(c) for c in cols]
     nk = len(cols)
     if nk == 0:
@@ -108,10 +105,19 @@ def group(cols, flags=None, na_pos=NA_FIRST):
         if c.nrows != n:
             raise _lib.DtbValueError("key columns have different numbers of rows")
     flags = list(flags) if flags is not None else [0] * nk
+    return cols, n, flags, (dtb_col * nk)(*[c.c() for c in cols]), (ctypes.c_int * nk)(*flags)
+
+
+def group(cols, flags=None, na_pos=NA_FIRST):
+    """group() of the reference: returns (order, offsets, ngroups).
+
+    order   : int32 RowIndex (ARR32) -- stable order of the rows
+    offsets : int32[ngroups+1] Groupby offsets, or None when flags[0] has SORT_ONLY
+    """
+    cols, n, flags, ckeys, cflags = _keys(cols, flags)
+    nk = len(cols)
     device = all(c.on_device for c in cols)
     do_groups = not (flags[0] & FLAG_SORT_ONLY)
-    ckeys = (dtb_col * nk)(*[c.c() for c in cols])
-    cflags = (ctypes.c_int * nk)(*flags)
     order, optr = _alloc(n, INT32, device)
     offs, fptr = (_alloc(n + 1, INT32, device) if do_groups else (None, 0))
     ng = ctypes.c_int64(-1)
@@ -131,14 +137,10 @@ GROUP64_OFFSETS_GUESS = 1 << 24
 def group64(cols, flags=None, na_pos=NA_FIRST):
     """group() with the ARR64 layout (dtb_group64): int64 RowIndex and int64 Groupby offsets; for frames of
     more than INT32_MAX rows (up to 2^32 on one GPU) or callers that want 64-bit indices."""
-    cols = [Col(c) for c in cols]
+    cols, n, flags, ckeys, cflags = _keys(cols, flags)
     nk = len(cols)
-    n = cols[0].nrows
-    flags = list(flags) if flags is not None else [0] * nk
     device = all(c.on_device for c in cols)
     do_groups = not (flags[0] & FLAG_SORT_ONLY)
-    ckeys = (dtb_col * nk)(*[c.c() for c in cols])
-    cflags = (ctypes.c_int * nk)(*flags)
     order, optr = _alloc(n, INT64, device)
     ng = ctypes.c_int64(-1)
     no = ctypes.c_int64(0)
@@ -170,12 +172,8 @@ class Groupby:
     def __init__(self, cols, flags=None, na_pos=NA_FIRST, reducers=None):
         """reducers: optional [(op, value column or None), ...] evaluated inside the same call
         (dtb_groupby_create_reduce): with a small key domain they stream the rows once the groups are known."""
-        cols = [Col(c) for c in cols]
+        cols, n, flags, ckeys, cflags = _keys(cols, flags)
         nk = len(cols)
-        n = cols[0].nrows
-        flags = list(flags) if flags is not None else [0] * nk
-        ckeys = (dtb_col * nk)(*[c.c() for c in cols])
-        cflags = (ctypes.c_int * nk)(*flags)
         h = ctypes.c_void_p(0)
         self._red = []
         if reducers:

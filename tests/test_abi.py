@@ -74,3 +74,11 @@ def test_argument_validation_before_any_gpu_work():
         d.engine.group([np.array(["a", "b"])])
     with pytest.raises(ValueError):
         d.engine.group([np.arange(3, dtype=np.int32), np.arange(4, dtype=np.int32)])
+    # every entry point that takes key columns checks them before any library call: the library reads nrows rows of
+    # each key column, so a shorter one would be read past its end
+    short = [np.arange(4, dtype=np.int32), np.arange(3, dtype=np.int64)]
+    for call in (d.engine.group, d.engine.group64, d.engine.Groupby):
+        with pytest.raises(ValueError):
+            call(short)
+        with pytest.raises(ValueError):
+            call([])
