@@ -17,6 +17,7 @@ FLAG_NONE, FLAG_DESCENDING, FLAG_SORT_ONLY = 0, 2, 4
 NA_FIRST, NA_LAST, NA_REMOVE = 1, 2, 3
 OP_SUM, OP_MEAN, OP_MIN, OP_MAX, OP_COUNT, OP_COUNTNA, OP_NROWS = 1, 2, 3, 4, 5, 6, 7
 OP_FIRST, OP_LAST, OP_SD, OP_MEDIAN, OP_NUNIQUE = 8, 9, 10, 11, 12
+OP_PROD, OP_COV, OP_CORR = 13, 14, 15
 SET_UNION, SET_INTERSECT, SET_SETDIFF, SET_SYMDIFF = 0, 1, 2, 3
 OK, EINVAL, ENOTIMPL, ECUDA, ENOMEM, ENOSPACE = 0, -1, -2, -3, -4, -5
 
@@ -24,6 +25,7 @@ EXPORTS = [
     "dtb_last_error", "dtb_abi_version", "dtb_stype_size", "dtb_reduce_out_stype", "dtb_init",
     "dtb_group", "dtb_group64", "dtb_groupby_create", "dtb_groupby_create_reduce", "dtb_groupby_reduced", "dtb_groupby_norder", "dtb_groupby_ngroups",
     "dtb_groupby_order", "dtb_groupby_offsets", "dtb_groupby_destroy", "dtb_groupby_reduce", "dtb_reduce",
+    "dtb_reduce2_out_stype", "dtb_reduce2", "dtb_groupby_reduce2",
     "dtb_groupby_reduce_begin", "dtb_groupby_reduce_add", "dtb_groupby_reduce_end", "dtb_slice_groups",
     "dtb_gather", "dtb_memcpy", "dtb_set_option", "dtb_get_option", "dtb_last_call_stats",
     "dtb_profile_count", "dtb_profile_get", "dtb_profile_reset",
@@ -110,6 +112,10 @@ def _load():
                                      c.c_void_p, c.POINTER(c.c_int64), c.POINTER(c.c_int64)]
     lib.dtb_reduce.argtypes = [c.c_int, dtb_col, c.c_int64, c.c_void_p, c.c_int, c.c_void_p,
                                c.c_int64, c.c_void_p, c.c_void_p]
+    lib.dtb_reduce2_out_stype.argtypes = [c.c_int, c.c_int, c.c_int]
+    lib.dtb_reduce2.argtypes = [c.c_int, dtb_col, dtb_col, c.c_int64, c.c_void_p, c.c_int, c.c_void_p,
+                                c.c_int64, c.c_void_p, c.c_void_p]
+    lib.dtb_groupby_reduce2.argtypes = [c.c_void_p, c.c_int, dtb_col, dtb_col, c.c_int64, c.c_void_p, c.c_void_p]
     lib.dtb_gather.argtypes = [dtb_col, c.c_int64, c.c_void_p, c.c_int, c.c_int64, c.c_void_p, c.c_void_p]
     lib.dtb_dense_scatter.argtypes = [c.c_void_p, c.c_int, c.c_void_p, c.c_int64, c.c_int64, c.c_int64,
                                       c.c_void_p, c.c_void_p, c.c_void_p]

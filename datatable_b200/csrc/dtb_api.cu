@@ -360,6 +360,9 @@ struct GroupResult {
 
 // The reducer's output stype, or the error for a column it cannot reduce.
 static int reducer_out_stype(int op, int stype, int& out_st) {
+  if (op == DTB_OP_COV || op == DTB_OP_CORR) {
+    set_error("cov / corr take two columns: use dtb_reduce2 / dtb_groupby_reduce2"); return DTB_EINVAL;
+  }
   out_st = reduce_out_stype_host(op, stype);
   if (out_st) return DTB_OK;
   set_error("Invalid column of stype " + std::to_string(stype) + " in reducer " + std::to_string(op));
@@ -959,13 +962,14 @@ static int group_core(const dtb_col* keys, int nkeys, const int* flags, int na_p
   t_stats.key_bits = gp.kp.total_bits;
   if (gp.kp.total_bits == 0) {          // every key column is constant: identity order, one group (cf. sort.cc:1435-1439)
     DTB_TRY(launch_iota32(order, n, s));
-    return group_offsets(gp, n, order, offsets, b, res, s);
+    DTB_TRY(group_offsets(gp, n, order, offsets, b, res, s));
+  } else {
+    print_plan(gp, n, nkeys, b.st);
+    DTB_TRY(sort_rounds(gp, n, fr ? fr->n : 0, order, s, b));
+    DTB_TL("passes enqueued");
+    DTB_TRY(group_offsets(gp, n, order, offsets, b, res, s));
+    DTB_TL("offsets synced");
   }
-  print_plan(gp, n, nkeys, b.st);
-  DTB_TRY(sort_rounds(gp, n, fr ? fr->n : 0, order, s, b));
-  DTB_TL("passes enqueued");
-  DTB_TRY(group_offsets(gp, n, order, offsets, b, res, s));
-  DTB_TL("offsets synced");
   if (fr && fr->n > 0 && do_groups) DTB_TRY(fused_reduce(gp, n, order, offsets, b, res, *fr, s));
   return DTB_OK;
 }
@@ -1162,10 +1166,14 @@ int dtb_groupby_create_reduce(const dtb_col* keys, int nkeys, const int* flags, 
   if (nreducers > 0 && flags && nkeys > 0 && (flags[0] & DTB_FLAG_SORT_ONLY)) {
     set_error("reducers need a Groupby: the first key column must not be SORT_ONLY"); return DTB_EINVAL;
   }
-  for (int i = 0; i < nreducers; i++)
+  for (int i = 0; i < nreducers; i++) {
+    if (reducers[i].op == DTB_OP_COV || reducers[i].op == DTB_OP_CORR) {
+      set_error("cov / corr take two columns: use dtb_groupby_reduce2 on the handle"); return DTB_EINVAL;
+    }
     if (reducers[i].op == DTB_OP_MEDIAN || reducers[i].op == DTB_OP_NUNIQUE) {
       set_error("median/nunique read rows sorted inside their group: use dtb_sort_grouped + dtb_reduce"); return DTB_EINVAL;
     }
+  }
   ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
   GroupResult res;
   FusedReducers fr; fr.spec = reducers; fr.n = nreducers;
@@ -1215,23 +1223,12 @@ int dtb_groupby_destroy(dtb_groupby* g, dtb_stream stream) {
   return DTB_OK;
 }
 
-// check_offsets = false: the offsets come from group() (a handle's own), so they need no device check
-static int reduce_groups(int op, dtb_col value, int64_t nrows_value, const void* order, int order_is64,
-                         const void* offsets, int64_t ngroups, dtb_stream stream, void* out, bool check_offsets)
+// Binds the caller's Groupby offsets (host or device) and reads n = offsets[ngroups].  check_offsets = false: they come
+// from group() (a handle's own), so they need no device check.
+static int bind_groupby(const void* offsets, int64_t ngroups, bool check_offsets, cudaStream_t s, DevIn& d_off,
+                        int64_t& n)
 {
-  cudaStream_t s = (cudaStream_t)stream;
-  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
-  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
-  if (ngroups < 0) { set_error("ngroups must be non-negative"); return DTB_EINVAL; }
-  if (!offsets) { set_error("offsets is NULL"); return DTB_EINVAL; }
-  if (!out && ngroups > 0) { set_error("out is NULL"); return DTB_EINVAL; }
-  int out_st = 0;
-  DTB_TRY(reducer_out_stype(op, value.stype, out_st));
-  if (op != DTB_OP_NROWS && !value.data && nrows_value > 0) { set_error("value column data is NULL"); return DTB_EINVAL; }
-  DTB_TRY(ensure_context());
-  if (ngroups == 0) return DTB_OK;
-
-  DevIn d_off; DTB_TRY(d_off.bind(offsets, sizeof(int32_t) * (size_t)(ngroups + 1), s));
+  DTB_TRY(d_off.bind(offsets, sizeof(int32_t) * (size_t)(ngroups + 1), s));
   // caller-supplied offsets must be a Groupby: offsets[0] = 0, strictly increasing (groupby.h:41-47)
   int32_t n32 = 0;
   int bad = 0;
@@ -1253,7 +1250,29 @@ static int reduce_groups(int op, dtb_col value, int64_t nrows_value, const void*
               std::to_string(bad - 1) + " is empty or out of order)");
     return DTB_EINVAL;
   }
-  const int64_t n = n32;
+  n = n32;
+  return DTB_OK;
+}
+
+// check_offsets = false: the offsets come from group() (a handle's own), so they need no device check
+static int reduce_groups(int op, dtb_col value, int64_t nrows_value, const void* order, int order_is64,
+                         const void* offsets, int64_t ngroups, dtb_stream stream, void* out, bool check_offsets)
+{
+  cudaStream_t s = (cudaStream_t)stream;
+  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
+  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
+  if (ngroups < 0) { set_error("ngroups must be non-negative"); return DTB_EINVAL; }
+  if (!offsets) { set_error("offsets is NULL"); return DTB_EINVAL; }
+  if (!out && ngroups > 0) { set_error("out is NULL"); return DTB_EINVAL; }
+  int out_st = 0;
+  DTB_TRY(reducer_out_stype(op, value.stype, out_st));
+  if (op != DTB_OP_NROWS && !value.data && nrows_value > 0) { set_error("value column data is NULL"); return DTB_EINVAL; }
+  DTB_TRY(ensure_context());
+  if (ngroups == 0) return DTB_OK;
+
+  DevIn d_off;
+  int64_t n = 0;
+  DTB_TRY(bind_groupby(offsets, ngroups, check_offsets, s, d_off, n));
   DevIn d_ord;
   if (op != DTB_OP_NROWS) DTB_TRY(d_ord.bind(order, (size_t)n * (order_is64 ? 8 : 4), s));
   DevOut d_out; DTB_TRY(d_out.bind(out, (size_t)ngroups * stype_bytes(out_st), s));
@@ -1304,12 +1323,69 @@ int dtb_groupby_reduce(dtb_groupby* g, int op, dtb_col value, int64_t nrows_valu
   return DTB_OK;
 }
 
+int dtb_reduce2_out_stype(int op, int stype_x, int stype_y) { return reduce2_out_stype_host(op, stype_x, stype_y); }
+
+static int reduce2_groups(int op, dtb_col x, dtb_col y, int64_t nrows_value, const void* order, int order_is64,
+                          const void* offsets, int64_t ngroups, dtb_stream stream, void* out, bool check_offsets)
+{
+  cudaStream_t s = (cudaStream_t)stream;
+  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
+  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
+  if (op != DTB_OP_COV && op != DTB_OP_CORR) { set_error("dtb_reduce2 takes DTB_OP_COV or DTB_OP_CORR"); return DTB_EINVAL; }
+  if (ngroups < 0) { set_error("ngroups must be non-negative"); return DTB_EINVAL; }
+  if (!offsets) { set_error("offsets is NULL"); return DTB_EINVAL; }
+  if (!out && ngroups > 0) { set_error("out is NULL"); return DTB_EINVAL; }
+  const int out_st = reduce2_out_stype_host(op, x.stype, y.stype);
+  if (!out_st) {
+    set_error("Invalid columns of stypes " + std::to_string(x.stype) + ", " + std::to_string(y.stype) + " in reducer " +
+              std::to_string(op));
+    return (stype_supported(x.stype) && stype_supported(y.stype)) ? DTB_EINVAL : DTB_ENOTIMPL;
+  }
+  if (nrows_value < 0) { set_error("nrows_value must be non-negative"); return DTB_EINVAL; }
+  if ((!x.data || !y.data) && nrows_value > 0) { set_error("value column data is NULL"); return DTB_EINVAL; }
+  DTB_TRY(ensure_context());
+  if (ngroups == 0) return DTB_OK;
+  DevIn d_off;
+  int64_t n = 0;
+  DTB_TRY(bind_groupby(offsets, ngroups, check_offsets, s, d_off, n));
+  DevIn d_ord, dx, dy;
+  DTB_TRY(d_ord.bind(order, (size_t)n * (order_is64 ? 8 : 4), s));
+  DTB_TRY(dx.bind(x.data, (size_t)nrows_value * stype_bytes(x.stype), s));
+  DTB_TRY(dy.bind(y.data, (size_t)nrows_value * stype_bytes(y.stype), s));
+  DevOut d_out; DTB_TRY(d_out.bind(out, (size_t)ngroups * stype_bytes(out_st), s));
+  DevBuf scr; DTB_TRY(scr.alloc(reduce2_scratch_bytes(ngroups), s));
+  {
+    ProfScope ps("reduce2", s);
+    DTB_TRY(launch_reduce2(op, dx.dptr, x.stype, dy.dptr, y.stype, nrows_value, d_ord.dptr, order_is64,
+                           (const int32_t*)d_off.dptr, ngroups, n, scr.as<u64>(), out_st == DTB_STYPE_FLOAT32, d_out.dptr, s));
+  }
+  if (d_out.staged()) {
+    DTB_TRY(d_out.finish((size_t)ngroups * stype_bytes(out_st), s));
+    DTB_CUDA_CHECK(cudaStreamSynchronize(s));
+  }
+  return DTB_OK;
+}
+
+int dtb_reduce2(int op, dtb_col x, dtb_col y, int64_t nrows_value, const void* order, int order_is64,
+                const void* offsets, int64_t ngroups, dtb_stream stream, void* out)
+{
+  return reduce2_groups(op, x, y, nrows_value, order, order_is64, offsets, ngroups, stream, out, true);
+}
+
+int dtb_groupby_reduce2(dtb_groupby* g, int op, dtb_col x, dtb_col y, int64_t nrows_value, dtb_stream stream, void* out)
+{
+  if (!g) { set_error("groupby handle is NULL"); return DTB_EINVAL; }
+  if (g->ngroups < 0) { set_error("the handle holds no Groupby (sort-only call)"); return DTB_EINVAL; }
+  return reduce2_groups(op, x, y, nrows_value, g->order, 0, g->offsets, g->ngroups, stream, out, false);
+}
+
 int dtb_groupby_reduce_begin(dtb_groupby* g, int op, int value_stype, dtb_stream stream, dtb_reduce_state** out)
 {
   cudaStream_t s = (cudaStream_t)stream;
   if (!g || !out) { set_error("groupby handle / out is NULL"); return DTB_EINVAL; }
   *out = nullptr;
   if (g->ngroups < 0) { set_error("the handle holds no Groupby (sort-only call)"); return DTB_EINVAL; }
+  if (op == DTB_OP_COV || op == DTB_OP_CORR) { set_error("cov / corr take two columns"); return DTB_EINVAL; }
   if (!g->direct.on || op < DTB_OP_SUM || op >= DTB_OP_NROWS) {
     set_error("piecewise reducers exist for the streaming path only (small key domain, device key columns, sum..countna)");
     return DTB_ENOTIMPL;

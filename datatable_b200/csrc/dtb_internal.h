@@ -266,6 +266,13 @@ int launch_slice_groups_emit(const int32_t* offsets, const SliceParams& p, const
 // sum/cnt: u64[ng] each, m2: double[2 * ng] (m2, then the groups' pivots), all zeroed
 int launch_sd(const void* v, int stype, int64_t nv, const int32_t* order, const int32_t* offsets, int64_t ng, int64_t n,
               unsigned long long* sum, unsigned long long* cnt, double* m2, void* out, cudaStream_t s);
+// cov / corr over the pairs (x, y) seen through `order` (int32 or int64 row ids), segmented by offsets.  scratch:
+// reduce2_scratch_bytes(ng) of device memory.  out: float32 when out_f32, else float64 (reduce2_out_stype_host).
+int reduce2_out_stype_host(int op, int stype_x, int stype_y);
+size_t reduce2_scratch_bytes(int64_t ng);
+int launch_reduce2(int op, const void* x, int sx, const void* y, int sy, int64_t nv, const void* order, int order_is64,
+                   const int32_t* offsets, int64_t ng, int64_t n, unsigned long long* scratch, int out_f32, void* out,
+                   cudaStream_t s);
 int launch_median(const void* v, int stype, int64_t nv, const int32_t* order, const int32_t* offsets,
                   int64_t ng, void* out, cudaStream_t s);
 int launch_distinct_flags(const void* v, int stype, int64_t nv, const int32_t* order, const int32_t* offsets,

@@ -270,6 +270,187 @@ int launch_sd(const void* v, int stype, int64_t nv, const int32_t* order, const 
 }
 
 // ===========================================================================
+// cov / corr (expr/head_reduce_binary.cc:114-221): sd's two passes over a pair of columns.  Only the rows where
+// both values are valid count; both are widened to float64 (the reference casts to float32 when both columns are
+// float32, else to float64).  The pivot (px, py) is the pair at the group's first such row in RowIndex order:
+//   pass 1: sx += x - px, sy += y - py, cnt += 1          (mx' = sx / cnt, my' = sy / cnt)
+//   pass 2: sxy += dx dy, and for corr sxx += dx^2, syy += dy^2, with dx = (x - px) - mx', dy = (y - py) - my'
+// A constant column has x - px = 0 on every row, so its sxx is exactly 0 (corr NA) and sxy exactly 0 (cov 0), as the
+// reference's Welford recurrence gives.  One atomic per (thread, group) and word, as in sd.
+// ===========================================================================
+// raw element of a column of stype st -> (valid, float64)
+__device__ __forceinline__ bool elem_f64(const void* v, int st, int64_t j, double& x) {
+  switch (st) {
+    case DTB_STYPE_BOOL: case DTB_STYPE_INT8: { const int8_t t = ((const int8_t*)v)[j]; x = (double)t; return t != INT8_MIN; }
+    case DTB_STYPE_INT16: { const int16_t t = ((const int16_t*)v)[j]; x = (double)t; return t != INT16_MIN; }
+    case DTB_STYPE_INT32: { const int32_t t = ((const int32_t*)v)[j]; x = (double)t; return t != INT32_MIN; }
+    case DTB_STYPE_INT64: { const int64_t t = ((const int64_t*)v)[j]; x = (double)t; return t != INT64_MIN; }
+    case DTB_STYPE_FLOAT32: { const float t = ((const float*)v)[j]; x = (double)t; return !isnan(t); }
+    case DTB_STYPE_FLOAT64: { x = ((const double*)v)[j]; return !isnan(x); }
+  }
+  return false;
+}
+
+struct PairCols { const void* x; const void* y; int sx, sy; int64_t nv; };
+
+template <typename OrdT>
+__device__ __forceinline__ bool pair_at(const PairCols& pc, const OrdT* order, int64_t p, double& x, double& y) {
+  const int64_t j = order ? (int64_t)order[p] : p;
+  if (j < 0 || j >= pc.nv) return false;
+  const bool vx = elem_f64(pc.x, pc.sx, j, x);
+  const bool vy = elem_f64(pc.y, pc.sy, j, y);
+  return vx && vy;
+}
+
+// pos[g] = min(pos[g], first position of group g whose pair is valid): first_valid_pos_kernel for a pair
+template <typename OrdT>
+__global__ void pair_first_pos_kernel(const PairCols pc, const OrdT* __restrict__ order, const int32_t* __restrict__ offsets,
+                                      int64_t ng, int64_t n, u64* __restrict__ pos)
+{
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x * 8;
+  for (int64_t p0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 8; p0 < n; p0 += stride) {
+    int64_t lo = 0, hi = ng;
+    while (hi - lo > 1) { const int64_t mid = (lo + hi) >> 1; if ((int64_t)offsets[mid] <= p0) lo = mid; else hi = mid; }
+    int64_t g = lo, next = offsets[g + 1];
+    u64 best = ~0ull;
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+      const int64_t p = p0 + i;
+      if (p >= n) break;
+      if (p >= next) {
+        if (best != ~0ull) atomicMin(&pos[g], best);
+        best = ~0ull;
+        while (p >= next) { g++; next = offsets[g + 1]; }
+      }
+      double x, y;
+      if (best == ~0ull && pair_at(pc, order, p, x, y)) best = (u64)p;
+    }
+    if (best != ~0ull) atomicMin(&pos[g], best);
+  }
+}
+
+// px[g] / py[g]: on entry px holds, as u64, the group's first valid position (~0: none); on exit the pivot pair
+template <typename OrdT>
+__global__ void pair_pivot_kernel(const PairCols pc, const OrdT* __restrict__ order, int64_t ng, double* __restrict__ px,
+                                  double* __restrict__ py)
+{
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += stride) {
+    const u64 p = reinterpret_cast<const u64*>(px)[g];
+    double x = 0.0, y = 0.0;                                   // no valid pair: cnt stays 0 and the result is NA
+    if (p != ~0ull) pair_at(pc, order, (int64_t)p, x, y);
+    px[g] = x; py[g] = y;
+  }
+}
+
+// acc: sx, sy, cnt, sxy, sxx, syy, ng words each (sx .. syy as double bits, cnt as u64)
+template <typename OrdT, bool PASS2>
+__global__ void pair_pass_kernel(const PairCols pc, const OrdT* __restrict__ order, const int32_t* __restrict__ offsets,
+                                 int64_t ng, int64_t n, const double* __restrict__ px, const double* __restrict__ py,
+                                 u64* __restrict__ acc, int corr)
+{
+  double* sx = reinterpret_cast<double*>(acc);
+  double* sy = sx + ng;
+  u64* cnt = acc + 2 * ng;
+  double* sxy = sx + 3 * ng;
+  double* sxx = sx + 4 * ng;
+  double* syy = sx + 5 * ng;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x * 8;
+  for (int64_t p0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 8; p0 < n; p0 += stride) {
+    int64_t lo = 0, hi = ng;
+    while (hi - lo > 1) { const int64_t mid = (lo + hi) >> 1; if ((int64_t)offsets[mid] <= p0) lo = mid; else hi = mid; }
+    int64_t g = lo, next = offsets[g + 1];
+    double ax = 0.0, ay = 0.0, axy = 0.0;
+    u32 c = 0;
+    double qx = px[g], qy = py[g], mx = 0.0, my = 0.0;
+    if (PASS2) { mx = sx[g] / (double)cnt[g]; my = sy[g] / (double)cnt[g]; }
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+      const int64_t p = p0 + i;
+      if (p >= n) break;
+      if (p >= next) {
+        if (c) {
+          if (PASS2) { atomicAdd(&sxy[g], axy); if (corr) { atomicAdd(&sxx[g], ax); atomicAdd(&syy[g], ay); } }
+          else { atomicAdd(&sx[g], ax); atomicAdd(&sy[g], ay); atomicAdd(&cnt[g], (u64)c); }
+        }
+        ax = ay = axy = 0.0; c = 0;
+        while (p >= next) { g++; next = offsets[g + 1]; }
+        qx = px[g]; qy = py[g];
+        if (PASS2) { mx = sx[g] / (double)cnt[g]; my = sy[g] / (double)cnt[g]; }
+      }
+      double x, y;
+      if (!pair_at(pc, order, p, x, y)) continue;
+      const double dx = (x - qx) - mx, dy = (y - qy) - my;
+      if (PASS2) { axy += dx * dy; ax += dx * dx; ay += dy * dy; }
+      else { ax += dx; ay += dy; }
+      c++;
+    }
+    if (c) {
+      if (PASS2) { atomicAdd(&sxy[g], axy); if (corr) { atomicAdd(&sxx[g], ax); atomicAdd(&syy[g], ay); } }
+      else { atomicAdd(&sx[g], ax); atomicAdd(&sy[g], ay); atomicAdd(&cnt[g], (u64)c); }
+    }
+  }
+}
+
+// cov: NA when cnt <= 1, else sxy / (cnt - 1); corr: NA unless cnt > 1 and sxx * syy > 0, else sxy / sqrt(sxx * syy)
+// (head_reduce_binary.cc:134-136, 196-200; no clamping)
+__global__ void pair_finalize_kernel(int corr, const u64* __restrict__ acc, int64_t ng, int out_f32, void* out)
+{
+  const double* s = reinterpret_cast<const double*>(acc);
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += stride) {
+    const u64 c = acc[2 * ng + g];
+    const double sxy = s[3 * ng + g], vv = s[4 * ng + g] * s[5 * ng + g];
+    bool valid; double r;
+    if (corr) { valid = c > 1 && vv > 0; r = sxy / sqrt(vv); }
+    else      { valid = c > 1; r = sxy / (double)(c - 1); }
+    if (out_f32) ((u32*)out)[g] = valid ? __float_as_uint((float)r) : 0x7FC00000u;
+    else         ((u64*)out)[g] = valid ? (u64)__double_as_longlong(r) : 0x7FF8000000000000ull;
+  }
+}
+
+int reduce2_out_stype_host(int op, int sx, int sy) {
+  auto num = [](int st) { return st == DTB_STYPE_BOOL || st == DTB_STYPE_INT8 || st == DTB_STYPE_INT16 || st == DTB_STYPE_INT32 ||
+                                 st == DTB_STYPE_INT64 || st == DTB_STYPE_FLOAT32 || st == DTB_STYPE_FLOAT64; };
+  if ((op != DTB_OP_COV && op != DTB_OP_CORR) || !num(sx) || !num(sy)) return 0;
+  return (sx == DTB_STYPE_FLOAT32 && sy == DTB_STYPE_FLOAT32) ? DTB_STYPE_FLOAT32 : DTB_STYPE_FLOAT64;   // :154-159
+}
+
+size_t reduce2_scratch_bytes(int64_t ng) { return sizeof(u64) * 8 * (size_t)(ng > 0 ? ng : 1); }
+
+template <typename OrdT>
+static void run_pairs(const PairCols& pc, const OrdT* order, const int32_t* offsets, int64_t ng, int64_t n, u64* acc,
+                      int corr, cudaStream_t s)
+{
+  double* px = reinterpret_cast<double*>(acc + 6 * ng);
+  double* py = px + ng;
+  const int grid = grid_for((n + 7) / 8);
+  pair_first_pos_kernel<OrdT><<<grid, 256, 0, s>>>(pc, order, offsets, ng, n, (u64*)px);
+  pair_pivot_kernel<OrdT><<<grid_for(ng), 256, 0, s>>>(pc, order, ng, px, py);
+  pair_pass_kernel<OrdT, false><<<grid, 256, 0, s>>>(pc, order, offsets, ng, n, px, py, acc, corr);
+  pair_pass_kernel<OrdT, true><<<grid, 256, 0, s>>>(pc, order, offsets, ng, n, px, py, acc, corr);
+  count_launch(4);
+}
+
+int launch_reduce2(int op, const void* x, int sx, const void* y, int sy, int64_t nv, const void* order, int order_is64,
+                   const int32_t* offsets, int64_t ng, int64_t n, u64* scratch, int out_f32, void* out, cudaStream_t s)
+{
+  if (ng == 0) return DTB_OK;
+  fill_u64(scratch, 6 * ng, 0ull, s);                          // sx .. syy
+  fill_u64(scratch + 6 * ng, ng, ~0ull, s);                    // px: first valid positions
+  const int corr = op == DTB_OP_CORR;
+  if (n > 0) {
+    const PairCols pc = {x, y, sx, sy, nv};
+    if (order_is64) run_pairs(pc, (const int64_t*)order, offsets, ng, n, scratch, corr, s);
+    else            run_pairs(pc, (const int32_t*)order, offsets, ng, n, scratch, corr, s);
+  }
+  pair_finalize_kernel<<<grid_for(ng), 256, 0, s>>>(corr, scratch, ng, out_f32, out);
+  count_launch();
+  DTB_CUDA_CHECK(cudaGetLastError());
+  return DTB_OK;
+}
+
+// ===========================================================================
 // median over rows already sorted inside their group (NA first): one thread per group
 // ===========================================================================
 template <typename T>

@@ -22,7 +22,7 @@
 
 namespace dtb {
 
-enum { CAT_SUMI = 0, CAT_SUMF = 1, CAT_MEAN = 2, CAT_MINMAX = 3, CAT_COUNT = 4 };
+enum { CAT_SUMI = 0, CAT_SUMF = 1, CAT_MEAN = 2, CAT_MINMAX = 3, CAT_COUNT = 4, CAT_PRODI = 5, CAT_PRODF = 6 };
 
 constexpr int RT = 256;          // threads per tile
 constexpr int RIPT = 8;          // consecutive rows per thread
@@ -34,6 +34,23 @@ template <> struct Partial<CAT_SUMF> { double s; };
 template <> struct Partial<CAT_MEAN> { double s; u32 c; };
 template <> struct Partial<CAT_MINMAX> { u64 key; };
 template <> struct Partial<CAT_COUNT> { u32 c; };
+template <> struct Partial<CAT_PRODI> { u64 p; };                    // wraps modulo 2^64
+// A float product kept as |prod| = m * 2^e, m in [1, 2): no intermediate product overflows or underflows.  f: bit 0
+// a zero was seen, bit 1 an infinity was seen, bit 2 the sign parity.
+template <> struct Partial<CAT_PRODF> { double m; int64_t e; u32 f; };
+
+// In the accumulators a float product is two words: acc0 = f << 52 | the 52 fraction bits of m, acc1 = e.
+constexpr u64 PRODF_FRAC = (1ull << 52) - 1;
+__device__ __forceinline__ double prodf_sig(u64 w) {
+  return __longlong_as_double((long long)((w & PRODF_FRAC) | 0x3FF0000000000000ull));
+}
+__device__ __forceinline__ void prodf_mul(Partial<CAT_PRODF>& a, double m, int64_t e, u32 f) {
+  const double r = a.m * m;                                       // [1, 4): one rounding
+  const bool carry = r >= 2.0;
+  a.m = carry ? r * 0.5 : r;                                      // exact
+  a.e += e + (carry ? 1 : 0);
+  a.f = ((a.f | f) & 3u) | ((a.f ^ f) & 4u);
+}
 
 template <int CAT>
 __device__ __forceinline__ void p_init(Partial<CAT>& p, int flag) {
@@ -41,6 +58,8 @@ __device__ __forceinline__ void p_init(Partial<CAT>& p, int flag) {
   else if constexpr (CAT == CAT_SUMF) p.s = 0.0;
   else if constexpr (CAT == CAT_MEAN) { p.s = 0.0; p.c = 0; }
   else if constexpr (CAT == CAT_MINMAX) p.key = flag ? ~0ull : 0ull;   // flag: 1 = MIN
+  else if constexpr (CAT == CAT_PRODI) p.p = 1;
+  else if constexpr (CAT == CAT_PRODF) { p.m = 1.0; p.e = 0; p.f = 0; }
   else p.c = 0;
 }
 
@@ -50,6 +69,8 @@ __device__ __forceinline__ void p_merge(Partial<CAT>& a, const Partial<CAT>& b, 
   else if constexpr (CAT == CAT_SUMF) a.s += b.s;
   else if constexpr (CAT == CAT_MEAN) { a.s += b.s; a.c += b.c; }
   else if constexpr (CAT == CAT_MINMAX) a.key = flag ? (b.key < a.key ? b.key : a.key) : (b.key > a.key ? b.key : a.key);
+  else if constexpr (CAT == CAT_PRODI) a.p *= b.p;
+  else if constexpr (CAT == CAT_PRODF) prodf_mul(a, b.m, b.e, b.f);
   else a.c += b.c;
 }
 
@@ -60,6 +81,10 @@ __device__ __forceinline__ Partial<CAT> p_shfl_up(const Partial<CAT>& a, int d) 
   else if constexpr (CAT == CAT_SUMF) r.s = __shfl_up_sync(0xffffffffu, a.s, d);
   else if constexpr (CAT == CAT_MEAN) { r.s = __shfl_up_sync(0xffffffffu, a.s, d); r.c = __shfl_up_sync(0xffffffffu, a.c, d); }
   else if constexpr (CAT == CAT_MINMAX) r.key = __shfl_up_sync(0xffffffffu, a.key, d);
+  else if constexpr (CAT == CAT_PRODI) r.p = __shfl_up_sync(0xffffffffu, a.p, d);
+  else if constexpr (CAT == CAT_PRODF) {
+    r.m = __shfl_up_sync(0xffffffffu, a.m, d); r.e = __shfl_up_sync(0xffffffffu, a.e, d); r.f = __shfl_up_sync(0xffffffffu, a.f, d);
+  }
   else r.c = __shfl_up_sync(0xffffffffu, a.c, d);
   return r;
 }
@@ -75,7 +100,37 @@ __device__ __forceinline__ void p_flush(const Partial<CAT>& p, int64_t g, u64* a
     if (flag) { if (p.key != ~0ull) atomicMin(&acc0[g], p.key); }
     else      { if (p.key != 0ull)  atomicMax(&acc0[g], p.key); }
   }
+  else if constexpr (CAT == CAT_PRODI) {                         // no atomic multiply: a CAS loop
+    if (p.p != 1) { u64 old = acc0[g], seen; do { seen = old; old = atomicCAS(&acc0[g], seen, seen * p.p); } while (old != seen); }
+  }
+  else if constexpr (CAT == CAT_PRODF) {
+    if (p.m == 1.0 && p.e == 0 && p.f == 0) return;
+    // the significand and the flags by CAS; the exponent, with the significand's carry, by one atomicAdd
+    Partial<CAT_PRODF> q;
+    u64 old = acc0[g], seen;
+    do {
+      seen = old;
+      q.m = prodf_sig(seen); q.e = 0; q.f = (u32)(seen >> 52);
+      prodf_mul(q, p.m, 0, p.f);
+      old = atomicCAS(&acc0[g], seen, ((u64)q.f << 52) | ((u64)__double_as_longlong(q.m) & PRODF_FRAC));
+    } while (old != seen);
+    if (p.e + q.e) atomicAdd(&acc1[g], (u64)(p.e + q.e));
+  }
   else { if (p.c) atomicAdd(&acc0[g], (u64)p.c); }
+}
+
+// PROD: a tile's first and last groups may go on in other tiles, and a group of 1e9 rows would have every warp of
+// the grid retry its CAS on one word.  So the runs of those two groups fold into two slots in shared memory, each
+// tile writes its slots out, and prod_finalize_kernel multiplies them into the group's result.  Only the groups
+// strictly inside a tile are flushed to the accumulators directly.  slot: u64[4] = word 0 of slots 0 / 1, then
+// word 1 of slots 0 / 1.
+template <int CAT>
+__device__ __forceinline__ void flush_run(const Partial<CAT>& p, int64_t g, int64_t g_lo, int64_t g_hi, u64* slot,
+                                          u64* acc0, u64* acc1, int flag) {
+  if constexpr (CAT == CAT_PRODI || CAT == CAT_PRODF) {
+    if (g == g_lo || g == g_hi) { p_flush(p, (int64_t)(g == g_lo ? 0 : 1), slot, slot + 2, flag); return; }
+  }
+  p_flush(p, g, acc0, acc1, flag);
 }
 
 // fold one (possibly NA) raw element into a partial
@@ -93,6 +148,18 @@ __device__ __forceinline__ void p_add(Partial<CAT>& p, typename RawKey<T>::load_
     else x = (double)(int64_t)u;
     p.s += x;
     if constexpr (CAT == CAT_MEAN) p.c += 1;
+  }
+  else if constexpr (CAT == CAT_PRODI) p.p *= u;
+  else if constexpr (CAT == CAT_PRODF) {
+    // |x| = m * 2^e exactly, from the bits (a float32 is widened first; a float64 subnormal is scaled up by 2^64)
+    u64 b = std::is_same<T, float>::value ? (u64)__double_as_longlong((double)__uint_as_float((u32)raw)) : (u64)raw;
+    const u32 sign = (u32)(b >> 63) << 2;
+    b &= ~0x8000000000000000ull;
+    if (b == 0) { p.f = (p.f | 1u) ^ sign; return; }
+    if (b == 0x7FF0000000000000ull) { p.f = (p.f | 2u) ^ sign; return; }
+    int64_t ex = (int64_t)(b >> 52);
+    if (ex == 0) { b = (u64)__double_as_longlong(__longlong_as_double((long long)b) * 0x1p64); ex = (int64_t)(b >> 52) - 64; }
+    prodf_mul(p, __longlong_as_double((long long)((b & PRODF_FRAC) | 0x3FF0000000000000ull)), ex - 1023, sign);
   }
   else if constexpr (CAT == CAT_MINMAX) {
     u64 key = ISF ? u : (u ^ 0x8000000000000000ull);      // order-preserving unsigned key, never 0 for ints
@@ -117,6 +184,12 @@ reduce_kernel(const typename RawKey<T>::load_t* __restrict__ v, int64_t nv,
   const int64_t t1 = (t0 + RTILE < n) ? t0 + RTILE : n;
 
   if (tid < RTILE / 32) s_bits[tid] = 0;
+  u64* s_slot = nullptr;                                       // PROD: the tile's two slots (flush_run)
+  if constexpr (CAT == CAT_PRODI || CAT == CAT_PRODF) {
+    __shared__ u64 s_prod[4];
+    s_slot = s_prod;
+    if (tid < 4) s_prod[tid] = (CAT == CAT_PRODI && tid < 2) ? 1ull : 0ull;
+  }
   if (tid == 0 || tid == 32) {
     // largest g with offsets[g] <= pos
     const int64_t pos = (tid == 0) ? t0 : (t1 - 1);
@@ -169,7 +242,7 @@ reduce_kernel(const typename RawKey<T>::load_t* __restrict__ v, int64_t nv,
 #pragma unroll
   for (int i = 0; i < RIPT; i++) {
     if (mybits & (1u << i)) {                 // a new group starts at this row: close the previous run
-      p_flush(part, g_cur, acc0, acc1, flag);
+      flush_run(part, g_cur, g_lo, g_hi, s_slot, acc0, acc1, flag);
       p_init(part, flag);
       g_cur++;
     }
@@ -185,7 +258,13 @@ reduce_kernel(const typename RawKey<T>::load_t* __restrict__ v, int64_t nv,
     if (lane >= d && ok == key) p_merge(part, o, flag);
   }
   const int64_t nkey = __shfl_down_sync(0xffffffffu, key, 1);
-  if (key >= 0 && (lane == 31 || nkey != key)) p_flush(part, key, acc0, acc1, flag);
+  if (key >= 0 && (lane == 31 || nkey != key)) flush_run(part, key, g_lo, g_hi, s_slot, acc0, acc1, flag);
+  if constexpr (CAT == CAT_PRODI || CAT == CAT_PRODF) {
+    // tile t's slots go to acc1[ng + 2t + slot] (word 0) and acc1[ng + 2 * ntiles + 2t + slot] (word 1)
+    __syncthreads();
+    u64* c = acc1 + ng + (tid >> 1) * 2 * (int64_t)gridDim.x;
+    if (tid < 4) c[2 * (int64_t)blockIdx.x + (tid & 1)] = s_slot[tid];
+  }
 }
 
 // ---- accumulator init / finalize ------------------------------------------------
@@ -329,12 +408,15 @@ static int reduce_out_stype(int op, int st) {
     case DTB_OP_SD: case DTB_OP_MEDIAN:                                           // head_reduce_unary.cc:224-245, 480-506
       return isint ? DTB_STYPE_FLOAT64 : (isflt ? st : 0);
     case DTB_OP_NUNIQUE: return stype_bytes(st) ? DTB_STYPE_INT64 : 0;            // head_reduce_unary.cc:398-415
+    case DTB_OP_PROD: return isint ? DTB_STYPE_INT64 : (isflt ? st : 0);          // fexpr_sumprod.cc:47-67
   }
   return 0;
 }
 
 size_t reduce_extra_bytes(int op, int stype, int64_t ng, int64_t n) {
   if (op == DTB_OP_SD) return 2 * sizeof(double) * (size_t)(ng > 0 ? ng : 1);      // m2, pivots
+  if (op == DTB_OP_PROD)                                                          // acc1, then the tiles' slots
+    return sizeof(u64) * (size_t)((ng > 0 ? ng : 1) + 4 * ((n + RTILE - 1) / RTILE));
   if (minmax_zero_sign(op, stype)) return zero_fix_bytes(ng);
   if (op == DTB_OP_NUNIQUE) return (size_t)n + 16;
   return 0;
@@ -361,27 +443,123 @@ static int dispatch_T(int st, const void* v, int64_t nv, const void* order, int 
                       const int32_t* offsets, int64_t ng, int64_t n, u64* acc0, u64* acc1,
                       int flag, cudaStream_t s)
 {
+  constexpr bool INTS = CAT != CAT_SUMF && CAT != CAT_PRODF, FLOATS = CAT != CAT_SUMI && CAT != CAT_PRODI;
   switch (st) {
     case DTB_STYPE_BOOL: case DTB_STYPE_INT8:
-      if constexpr (CAT != CAT_SUMF) return run_reduce<int8_t, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
+      if constexpr (INTS) return run_reduce<int8_t, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
       break;
     case DTB_STYPE_INT16:
-      if constexpr (CAT != CAT_SUMF) return run_reduce<int16_t, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
+      if constexpr (INTS) return run_reduce<int16_t, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
       break;
     case DTB_STYPE_INT32:
-      if constexpr (CAT != CAT_SUMF) return run_reduce<int32_t, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
+      if constexpr (INTS) return run_reduce<int32_t, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
       break;
     case DTB_STYPE_INT64:
-      if constexpr (CAT != CAT_SUMF) return run_reduce<int64_t, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
+      if constexpr (INTS) return run_reduce<int64_t, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
       break;
     case DTB_STYPE_FLOAT32:
-      if constexpr (CAT != CAT_SUMI) return run_reduce<float, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
+      if constexpr (FLOATS) return run_reduce<float, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
       break;
     case DTB_STYPE_FLOAT64:
-      if constexpr (CAT != CAT_SUMI) return run_reduce<double, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
+      if constexpr (FLOATS) return run_reduce<double, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
       break;
   }
   set_error("internal: reducer/stype combination"); return DTB_EINVAL;
+}
+
+template <int CAT>
+__device__ __forceinline__ Partial<CAT> prod_word(const u64* w0, const u64* w1, int64_t i) {
+  Partial<CAT> p;
+  if constexpr (CAT == CAT_PRODI) p.p = w0[i];
+  else { const u64 w = w0[i]; p.m = prodf_sig(w); p.e = (int64_t)w1[i]; p.f = (u32)(w >> 52); }
+  return p;
+}
+
+template <int CAT>
+__device__ __forceinline__ Partial<CAT> p_shfl_xor(const Partial<CAT>& a, int d) {
+  Partial<CAT> r;
+  if constexpr (CAT == CAT_PRODI) r.p = __shfl_xor_sync(0xffffffffu, a.p, d);
+  else {
+    r.m = __shfl_xor_sync(0xffffffffu, a.m, d); r.e = __shfl_xor_sync(0xffffffffu, a.e, d); r.f = __shfl_xor_sync(0xffffffffu, a.f, d);
+  }
+  return r;
+}
+
+// out[g] = the product of group g: its accumulators (the runs strictly inside a tile) times the slots of the tiles it
+// reaches into.  Group g covers positions [a, b), tiles ta .. tb: in tile ta it is slot 0 (it starts the tile) or
+// slot 1 (it ends the tile) or neither; in every later tile it is slot 0.  A group that reaches into more than 32
+// tiles is folded by its whole warp, 32 tiles at a time.  The slots are assigned from the offsets alone, which relies on
+// the Groupby invariant that no group is empty (an empty group at a tile start would take the next group's slot 0):
+// group() never makes one, and caller-supplied offsets are checked first (offsets_check_kernel).  Float results: zero and infinity together give NA
+// (0 * inf), otherwise a zero or an infinity with the sign parity, otherwise m * 2^e rounded once.
+template <int CAT>
+__global__ void prod_finalize_kernel(const int32_t* __restrict__ offsets, int64_t ng, int64_t n, const u64* __restrict__ acc0,
+                                     const u64* __restrict__ acc1, int64_t ntiles, int out_stype, void* out)
+{
+  const u64* c0 = acc1 + ng;
+  const u64* c1 = c0 + 2 * ntiles;
+  const int lane = threadIdx.x & 31;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const int64_t gend = (ng + 31) & ~(int64_t)31;             // whole warps stay in the loop
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < gend; g += stride) {
+    Partial<CAT> p; p_init(p, 0);
+    int64_t t1 = 0, t2 = -1;                                   // the later tiles: slot 0 of t1 .. t2
+    if (g < ng) {
+      p = prod_word<CAT>(acc0, acc1, g);
+      const int64_t a = offsets[g], b = offsets[g + 1];
+      const int64_t ta = a / RTILE, tend = (ta + 1) * RTILE < n ? (ta + 1) * RTILE : n;
+      if (a == ta * RTILE) p_merge(p, prod_word<CAT>(c0, c1, 2 * ta), 0);
+      else if (b >= tend)  p_merge(p, prod_word<CAT>(c0, c1, 2 * ta + 1), 0);
+      t1 = ta + 1; t2 = (b - 1) / RTILE;
+    }
+    const bool wide = t2 - t1 >= 32;
+    if (!wide) for (int64_t t = t1; t <= t2; t++) p_merge(p, prod_word<CAT>(c0, c1, 2 * t), 0);
+    for (unsigned todo = __ballot_sync(0xffffffffu, wide); todo; todo &= todo - 1) {
+      const int src = __ffs(todo) - 1;
+      const int64_t s1 = __shfl_sync(0xffffffffu, t1, src), s2 = __shfl_sync(0xffffffffu, t2, src);
+      Partial<CAT> q; p_init(q, 0);
+      for (int64_t t = s1 + lane; t <= s2; t += 32) p_merge(q, prod_word<CAT>(c0, c1, 2 * t), 0);
+#pragma unroll
+      for (int d = 16; d >= 1; d >>= 1) p_merge(q, p_shfl_xor(q, d), 0);
+      if (lane == src) p_merge(p, q, 0);
+    }
+    if (g >= ng) continue;
+    if constexpr (CAT == CAT_PRODI) {
+      ((int64_t*)out)[g] = (int64_t)p.p;
+    } else {
+      const bool neg = (p.f & 4u) != 0;
+      double r;
+      if (p.f & 1u) r = neg ? -0.0 : 0.0;
+      else if (p.f & 2u) r = neg ? -INFINITY : INFINITY;
+      else r = ldexp(neg ? -p.m : p.m, (int)(p.e < -4000 ? -4000 : (p.e > 4000 ? 4000 : p.e)));
+      const bool valid = (p.f & 3u) != 3u;
+      // float32: the float64 r is exact wherever a float32 result is not 0, so this rounds once
+      if (out_stype == DTB_STYPE_FLOAT32) ((u32*)out)[g] = valid ? __float_as_uint((float)r) : 0x7FC00000u;
+      else ((u64*)out)[g] = valid ? (u64)__double_as_longlong(r) : 0x7FF8000000000000ull;
+    }
+  }
+}
+
+// PROD (column/sumprod.h:34-59): integers wrap modulo 2^64, bit-exact in any order; floats are exponent-tracked (see
+// Partial<CAT_PRODF>) and rounded once.  acc1 = extra (reduce_extra_bytes): the exponents, then the tiles' slots.
+static int launch_prod(const void* value, int stype, int64_t nv, const void* order, int order_is64,
+                       const int32_t* offsets, int64_t ng, int64_t n, u64* acc0, u64* acc1, int out_st, void* out,
+                       cudaStream_t s)
+{
+  const bool isflt = (stype == DTB_STYPE_FLOAT32 || stype == DTB_STYPE_FLOAT64);
+  const int64_t ntiles = (n + RTILE - 1) / RTILE;            // every tile writes both its slots
+  fill_u64(acc0, ng, isflt ? 0ull : 1ull, s);
+  fill_u64(acc1, ng, 0ull, s);
+  DTB_CUDA_CHECK(cudaGetLastError());
+  if (n > 0)
+    DTB_TRY(isflt ? dispatch_T<CAT_PRODF>(stype, value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 0, s)
+                  : dispatch_T<CAT_PRODI>(stype, value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 0, s));
+  const int fgrid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
+  if (isflt) prod_finalize_kernel<CAT_PRODF><<<fgrid, 256, 0, s>>>(offsets, ng, n, acc0, acc1, ntiles, out_st, out);
+  else       prod_finalize_kernel<CAT_PRODI><<<fgrid, 256, 0, s>>>(offsets, ng, n, acc0, acc1, ntiles, out_st, out);
+  count_launch();
+  DTB_CUDA_CHECK(cudaGetLastError());
+  return DTB_OK;
 }
 
 // acc0/acc1: device scratch of ng u64 each (allocated by the caller in dtb_api.cu)
@@ -419,6 +597,10 @@ int launch_reduce_impl(int op, const void* value, int stype, int64_t nv, const v
     return DTB_OK;
   }
   if (op == DTB_OP_NROWS) return launch_nrows(offsets, ng, out, s);
+  if (op == DTB_OP_PROD) {
+    if (!extra) { set_error("internal: reducer scratch missing"); return DTB_EINVAL; }
+    return launch_prod(value, stype, nv, order, order_is64, offsets, ng, n, acc0, (u64*)extra, out_st, out, s);
+  }
   const bool isflt = (stype == DTB_STYPE_FLOAT32 || stype == DTB_STYPE_FLOAT64);
   u64 init0 = (op == DTB_OP_MIN) ? ~0ull : 0ull;          // 0.0 == 0 bits for float sums
   fill_u64_kernel<<<fgrid, 256, 0, s>>>(acc0, ng, init0);

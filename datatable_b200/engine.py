@@ -250,6 +250,21 @@ class Groupby:
             _memcpy_d2d(t.data_ptr(), lib.dtb_groupby_reduced(self._h, i), t.numel() * t.element_size())
         return t
 
+    def reduce2(self, op, x, y, out=None):
+        """cov / corr (OP_COV / OP_CORR) of the columns x and y over the handle's groups (dtb_groupby_reduce2)."""
+        cx, cy = Col(x), Col(y)
+        if cx.nrows != cy.nrows:
+            raise _lib.DtbValueError("cov / corr need two columns of the same length")
+        out_st = reduce2_out_stype(op, cx.stype, cy.stype)
+        if not out_st:
+            raise _lib.DtbValueError(f"Invalid columns of stypes {cx.stype}, {cy.stype} in reducer {op}")
+        if out is None:
+            out, optr = _alloc(self.ngroups, out_st, cx.on_device and cy.on_device)
+        else:
+            optr = out.data_ptr() if is_tensor(out) else out.ctypes.data
+        check(lib.dtb_groupby_reduce2(self._h, op, cx.c(), cy.c(), cx.nrows, _stream(), ctypes.c_void_p(optr)))
+        return out
+
     def sort_grouped(self, value):
         """RowIndex with the rows of every group ordered by `value` (NA first): what median / nunique read."""
         v = Col(value)
@@ -338,6 +353,31 @@ def reduce(op, value, order, offsets, stype=None):
     check(lib.dtb_reduce(op, dtb_col(ctypes.c_void_p(vptr), vst, 0), vn,
                          ctypes.c_void_p(o.ptr) if o is not None else None, is64,
                          ctypes.c_void_p(f.ptr), ngroups, _stream(), ctypes.c_void_p(optr)))
+    return out
+
+
+def reduce2_out_stype(op, stype_x, stype_y):
+    return lib.dtb_reduce2_out_stype(op, stype_x, stype_y)
+
+
+def reduce2(op, x, y, order, offsets, stype_x=None, stype_y=None):
+    """cov / corr (OP_COV / OP_CORR) per group of the columns x and y viewed through RowIndex `order` (None =
+    identity; int32 or int64), segmented by `offsets` (dtb_reduce2)."""
+    ngroups = int(offsets.shape[0]) - 1
+    cx, cy = Col(x, stype_x), Col(y, stype_y)
+    if cx.nrows != cy.nrows:
+        raise _lib.DtbValueError("cov / corr need two columns of the same length")
+    out_st = reduce2_out_stype(op, cx.stype, cy.stype)
+    if not out_st:
+        raise _lib.DtbValueError(f"Invalid columns of stypes {cx.stype}, {cy.stype} in reducer {op}")
+    out, optr = _alloc(ngroups, out_st, cx.on_device and cy.on_device)
+    o = None if order is None else Col(order)
+    if o is not None and o.stype not in (INT32, INT64):
+        raise _lib.DtbValueError("order must be int32 or int64")
+    f = Col(offsets)
+    check(lib.dtb_reduce2(op, cx.c(), cy.c(), cx.nrows, ctypes.c_void_p(o.ptr) if o is not None else None,
+                          1 if o is not None and o.stype == INT64 else 0, ctypes.c_void_p(f.ptr), ngroups, _stream(),
+                          ctypes.c_void_p(optr)))
     return out
 
 

@@ -66,6 +66,7 @@ class Reducer:
 
 
 def sum(x): return Reducer(_lib.OP_SUM, "sum", x)          # noqa: A001  (mirrors dt.sum)
+def prod(x): return Reducer(_lib.OP_PROD, "prod", x)
 def mean(x): return Reducer(_lib.OP_MEAN, "mean", x)
 def min(x): return Reducer(_lib.OP_MIN, "min", x)          # noqa: A001
 def max(x): return Reducer(_lib.OP_MAX, "max", x)          # noqa: A001
@@ -76,6 +77,32 @@ def last(x): return Reducer(_lib.OP_LAST, "last", x)
 def sd(x): return Reducer(_lib.OP_SD, "sd", x)
 def median(x): return Reducer(_lib.OP_MEDIAN, "median", x)
 def nunique(x): return Reducer(_lib.OP_NUNIQUE, "nunique", x) if isinstance(x, (ColRef, str)) else _frame_nunique(x)
+
+
+class Reducer2(Reducer):
+    """A reducer of two columns (cov / corr, expr/head_reduce_binary.cc): arg = x, arg2 = y."""
+    def __init__(self, op, name, x, y):
+        super().__init__(op, name, _as_ref(x))
+        self.arg2 = _as_ref(y)
+
+
+def _binary(op, name, x, y):
+    """One reducer per pair; a list argument broadcasts: both lists of the same length, or one of them of length 1
+    (head_reduce_binary.cc:236-259)."""
+    xs = list(x) if isinstance(x, (list, tuple)) else [x]
+    ys = list(y) if isinstance(y, (list, tuple)) else [y]
+    if not isinstance(x, (list, tuple)) and not isinstance(y, (list, tuple)):
+        return Reducer2(op, name, x, y)
+    n1, n2 = len(xs), len(ys)
+    if n1 != n2 and n1 != 1 and n2 != 1:
+        raise ValueError(f"Cannot apply reducer function {name}: argument 1 has {n1} columns, while argument 2 has "
+                         f"{n2} columns")
+    n = n1 if n1 != 1 else n2
+    return [Reducer2(op, name, xs[i if n1 > 1 else 0], ys[i if n2 > 1 else 0]) for i in range(n)]
+
+
+def cov(x, y): return _binary(_lib.OP_COV, "cov", x, y)
+def corr(x, y): return _binary(_lib.OP_CORR, "corr", x, y)
 
 
 def count(x=None):
@@ -403,6 +430,8 @@ def _evaluate(DT, j, by_, sort_, isel=None):
         nm = e.arg.name if isinstance(e, Reducer) and e.arg is not None else getattr(e, "name", None)
         if nm is not None:
             needed.append(nm)
+        if isinstance(e, Reducer2):
+            needed.append(e.arg2.name)
     copy_stream = None
     pending = {}
     pieces = {}               # large value columns travel in pieces, each with its own event (see the late path)
@@ -501,7 +530,7 @@ def _evaluate(DT, j, by_, sort_, isel=None):
             # the reducers of j are known before group() runs: hand them over so that the engine can
             # overlap them with the sort (dtb_groupby_create_reduce)
             # (median / nunique read the rows sorted inside their group: evaluated after group(), below)
-            fused = [e for e in exprs if isinstance(e, Reducer) and e.op not in _SORTED_OPS]
+            fused = [e for e in exprs if isinstance(e, Reducer) and e.op not in _SORTED_OPS and not isinstance(e, Reducer2)]
             # Host frame whose value columns are still on their way over PCIe: group() first (the sort runs
             # under the upload), the reducers afterwards through the handle, each waiting only for its own
             # column.  Handing the reducers to group() would make the stream wait for every value column
@@ -552,6 +581,7 @@ def _evaluate(DT, j, by_, sort_, isel=None):
         out._cols[name] = data
         out._stypes[name] = st
 
+    bynames_ = [r.name for r in by_.cols] if by_ is not None else []
     if by_ is not None:
         if has_reducer and sliced:
             first = engine.gather(order, offsets[:-1])
@@ -561,7 +591,7 @@ def _evaluate(DT, j, by_, sort_, isel=None):
             for name, e in zip(names, exprs):
                 if not isinstance(e, Reducer):
                     raise NotImplementedError("mixing reducers and plain columns under by() is outside the hot path")
-                add(name, _reduce(dcol, e, order, offsets), _red_stype(dcol, e))
+                add(name, _reduce(dcol, e, order, offsets, bynames_), _red_stype(dcol, e))
             for n_ in out._cols:
                 if out._stypes[n_] is None:
                     out._stypes[n_] = engine.Col(out._cols[n_]).stype
@@ -579,7 +609,10 @@ def _evaluate(DT, j, by_, sort_, isel=None):
                     add(ref.name, engine.gather(c, first), c.stype)
             ired = 0
             for name, e in zip(names, exprs):
-                if isinstance(e, Reducer) and e.op in _SORTED_OPS:
+                if isinstance(e, Reducer2):
+                    add(name, _reduce2_grouped(dcol, e, bynames_, ngroups, lambda x, y: gb.reduce2(e.op, x, y)),
+                        _red_stype(dcol, e))
+                elif isinstance(e, Reducer) and e.op in _SORTED_OPS:
                     c = dcol(e.arg.name)                      # Median_ColumnImpl::pre_materialize_hook: sort_grouped first
                     add(name, gb.reduce_ordered(e.op, c, gb.sort_grouped(c)), _red_stype(dcol, e))
                 elif isinstance(e, Reducer):
@@ -636,14 +669,23 @@ def _resolve_j(DT, j):
     if j_is_all(j):
         return list(DT.names), [ColRef(n) for n in DT.names]
     if isinstance(j, dict):
-        return list(j.keys()), [_as_expr(v) for v in j.values()]
+        names, es = [], []
+        for k, v in j.items():
+            vs = v if isinstance(v, list) else [v]              # a broadcast cov / corr: k, k.0, k.1, ... (see add)
+            names += [k] * len(vs)
+            es += [_as_expr(x) for x in vs]
+        return names, es
     if isinstance(j, (list, tuple)):
-        es = [_as_expr(v) for v in j]
+        es = [_as_expr(x) for v in j for x in (v if isinstance(v, list) else [v])]
     else:
-        es = [_as_expr(j)]
+        es = [_as_expr(x) for x in (j if isinstance(j, list) else [j])]
     names = []
+    nbin = 0
     for e in es:
-        if isinstance(e, Reducer):
+        if isinstance(e, Reducer2):
+            names.append(f"C{nbin}")                                  # unnamed cov / corr columns: C0, C1, ...
+            nbin += 1
+        elif isinstance(e, Reducer):
             names.append("count" if e.arg is None else e.arg.name)     # reducers keep the column's name
         else:
             names.append(e.name)
@@ -667,13 +709,29 @@ def _red_stype(dcol, e):
     """Output stype of a reducer column (bool8 min/max stay bool8, fexpr_minmax.cc:50-72)."""
     if e.op == _lib.OP_NROWS or e.arg is None:
         return INT64
+    if isinstance(e, Reducer2):
+        return engine.reduce2_out_stype(e.op, dcol(e.arg.name).stype, dcol(e.arg2.name).stype)
     return engine.reduce_out_stype(e.op, dcol(e.arg.name).stype)
 
 
 _SORTED_OPS = (_lib.OP_MEDIAN, _lib.OP_NUNIQUE)
 
 
-def _reduce(dcol, e, order, offsets):
+def _reduce2_grouped(dcol, e, bynames, ngroups, run):
+    """cov / corr: an all-NA column when either argument is a by() column (make_na_result, head_reduce_binary.cc:48-52,
+    240-251), else run(x, y)."""
+    if e.arg.name in bynames or e.arg2.name in bynames:
+        st = engine.reduce2_out_stype(e.op, dcol(e.arg.name).stype, dcol(e.arg2.name).stype)
+        if not st:
+            raise _lib.DtbValueError(f"Invalid columns in reducer {e.opname}")
+        return torch.full((ngroups,), float("nan"), dtype=torch.float32 if st == FLOAT32 else torch.float64, device="cuda")
+    return run(dcol(e.arg.name), dcol(e.arg2.name))
+
+
+def _reduce(dcol, e, order, offsets, bynames=()):
+    if isinstance(e, Reducer2):
+        return _reduce2_grouped(dcol, e, bynames, int(offsets.shape[0]) - 1,
+                                lambda x, y: engine.reduce2(e.op, x, y, order, offsets))
     if e.op == _lib.OP_NROWS:
         return engine.reduce(e.op, None, order, offsets)
     c = dcol(e.arg.name)

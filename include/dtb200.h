@@ -75,6 +75,10 @@ extern "C" {
 #define DTB_OP_SD      10   /* sd_reducer                     head_reduce_unary.cc:197-219: sample sd, count <= 1 -> NA    */
 #define DTB_OP_MEDIAN  11   /* Median_ColumnImpl              head_reduce_unary.cc:421-468: needs dtb_sort_grouped's order */
 #define DTB_OP_NUNIQUE 12   /* op_nunique                     head_reduce_unary.cc:383-394: needs dtb_sort_grouped's order */
+#define DTB_OP_PROD    13   /* SumProd_ColumnImpl<T,false,..> column/sumprod.h:34-59, fexpr_sumprod.cc:47-67       */
+/* two-column reducers: dtb_reduce2 / dtb_groupby_reduce2 only (the one-column entry points return DTB_EINVAL) */
+#define DTB_OP_COV     14   /* cov_reducer                    head_reduce_binary.cc:114-138: sample covariance       */
+#define DTB_OP_CORR    15   /* corr_reducer                   head_reduce_binary.cc:168-200: Pearson correlation     */
 
 /* set operations, set_funcs.cc:126-456 */
 #define DTB_SET_UNION      0
@@ -215,6 +219,23 @@ DTB_API int         dtb_groupby_destroy(dtb_groupby* g, dtb_stream stream);
  * count; float32 results add their final rounding.  A cancelling group can
  * differ from the reference's sequential sum by that much, in relative terms
  * without limit.  SD of a group whose valid values are all equal is 0.0.
+ *
+ * PROD skips NA rows and starts at 1, so a group without valid rows gives 1.
+ * Over integers/bool it is an INT64 product wrapping modulo 2^64, bit-exact.
+ * Over floats (FLOAT32 -> FLOAT32, FLOAT64 -> FLOAT64) the engine keeps the
+ * significand and the binary exponent apart, in float64, so no intermediate
+ * product overflows or underflows: a group of m valid finite non-zero rows
+ * gives the exact product times (1 + d), |d| <= gamma(m-1), rounded once to
+ * the output stype.  A zero and an infinity in the same group give NA (the
+ * reference's 0 * inf = NaN); a zero alone gives 0 and an infinity alone gives
+ * inf, signed by the parity of the negative rows.  Two deviations from the
+ * reference, which multiplies in order in the column's own type: float32
+ * groups are multiplied in float64, and where the reference's running product
+ * overflows to inf or underflows to 0 part-way although the exact product is
+ * in range, the engine returns the in-range value (so such a group that also
+ * holds a zero or an inf is not NA here).  Streaming and piecewise paths do
+ * not exist for PROD: dtb_groupby_reduce and dtb_groupby_create_reduce take
+ * the RowIndex, and dtb_groupby_reduce_begin returns DTB_ENOTIMPL.
  */
 DTB_API int dtb_reduce(int op, dtb_col value, int64_t nrows_value,
                const void* order, int order_is64,
@@ -252,6 +273,28 @@ typedef struct dtb_reduce_state dtb_reduce_state;
 DTB_API int dtb_groupby_reduce_begin(dtb_groupby* g, int op, int value_stype, dtb_stream stream, dtb_reduce_state** out);
 DTB_API int dtb_groupby_reduce_add(dtb_reduce_state* st, const void* value_rows, int64_t row0, int64_t nrows, dtb_stream stream);
 DTB_API int dtb_groupby_reduce_end(dtb_reduce_state* st, dtb_stream stream, void* out);
+
+/*
+ * dtb_reduce2 -- cov / corr per group (expr/head_reduce_binary.cc:114-221): the columns x and y, both viewed
+ * through the RowIndex `order` (NULL = identity; order_is64: int64 row ids), segmented by `offsets`.  Host or device
+ * pointers, offsets validated as dtb_reduce does.  nrows_value: rows in each of x and y (bounds the gather).
+ *   out : ngroups elements of stype dtb_reduce2_out_stype(op, x.stype, y.stype): FLOAT32 when both columns are
+ *         FLOAT32, FLOAT64 otherwise (bool and integer columns included); 0 = invalid combination.
+ * Only rows where both values are valid count; m = their number.  COV is NA when m <= 1, else
+ * sum (x - mx)(y - my) / (m - 1).  CORR is NA unless m > 1 and sxx * syy > 0, else sxy / sqrt(sxx * syy), not
+ * clamped.  Accuracy: both columns are widened to float64 (deviation: the reference computes in float32 when both
+ * are float32) and the groups are folded in two passes over the values shifted by the group's first valid pair
+ * (px, py) -- sums of x - px, y - py, then of the products of the deviations from those shifted means -- instead of
+ * the reference's Welford recurrence, in an unspecified order.  Each accumulated sum has the error of a float64
+ * summation in any order, gamma(m-1) * sum of |terms|; the result is rounded once to the output stype.  A group
+ * whose x (or y) values are all equal gives exactly cov = 0 and corr = NA, as the reference does.
+ */
+DTB_API int dtb_reduce2_out_stype(int op, int stype_x, int stype_y);
+DTB_API int dtb_reduce2(int op, dtb_col x, dtb_col y, int64_t nrows_value, const void* order, int order_is64,
+                const void* offsets, int64_t ngroups, dtb_stream stream, void* out);
+/* dtb_reduce2 over the handle's RowIndex / offsets (always through the RowIndex: there is no streaming variant). */
+DTB_API int dtb_groupby_reduce2(dtb_groupby* g, int op, dtb_col x, dtb_col y, int64_t nrows_value,
+                        dtb_stream stream, void* out);
 
 /*
  * dtb_gather -- replaces materialisation of ArrayView_ColumnImpl<int32/int64>
