@@ -30,7 +30,7 @@ EXPORTS = [
     "dtb_gather", "dtb_memcpy", "dtb_set_option", "dtb_get_option", "dtb_last_call_stats",
     "dtb_profile_count", "dtb_profile_get", "dtb_profile_reset",
     "dtb_dense_scatter", "dtb_dense_compact",
-    "dtb_sort_grouped", "dtb_set_select", "dtb_largest_group", "dtb_join", "dtb_cache_begin", "dtb_cache_end", "dtb_lower_bound",
+    "dtb_sort_grouped", "dtb_qcut", "dtb_set_select", "dtb_largest_group", "dtb_join", "dtb_cache_begin", "dtb_cache_end", "dtb_lower_bound",
 ]
 
 
@@ -122,6 +122,7 @@ def _load():
     lib.dtb_dense_compact.argtypes = [c.c_void_p, c.c_void_p, c.c_int64, c.c_int64, c.c_int, c.c_void_p, c.c_void_p,
                                       c.POINTER(c.c_int64), c.c_void_p]
     lib.dtb_sort_grouped.argtypes = [dtb_col, c.c_int64, c.c_void_p, c.c_void_p, c.c_int64, c.c_void_p, c.c_void_p]
+    lib.dtb_qcut.argtypes = [dtb_col, c.c_int64, c.c_void_p, c.c_void_p, c.c_int64, c.c_int, c.c_void_p, c.c_void_p]
     lib.dtb_set_select.argtypes = [c.c_int, c.c_void_p, c.c_void_p, c.c_int64, c.POINTER(c.c_int64), c.c_int,
                                    c.c_void_p, c.c_void_p, c.POINTER(c.c_int64)]
     lib.dtb_largest_group.argtypes = [c.c_void_p, c.c_int64, c.c_int64, c.c_void_p, c.POINTER(c.c_int64),

@@ -1543,6 +1543,32 @@ int dtb_dense_compact(const void* table, const void* present, int64_t table_size
   return DTB_OK;
 }
 
+// group() of the rows of every group of (order, offsets) by the composite key (group id, value), NA first: the group
+// id and the value seen through the RowIndex at every one of its n positions.  flag = DTB_FLAG_SORT_ONLY: the RowIndex
+// alone (dtb_sort_grouped); 0: also the Groupby, whose groups are the distinct values inside every group (dtb_qcut).
+// gv.res.order holds RowIndex positions; gv.ord is the RowIndex itself (a materialised identity when order is NULL).
+struct GroupedByValue {
+  DevBuf gid, vg, iota;
+  const void* ord = nullptr;
+  GroupResult res;
+};
+
+static int group_by_value(dtb_col value, int64_t nrows_value, const void* order, const int32_t* offsets,
+                          int64_t ngroups, int64_t n, int flag, cudaStream_t s, GroupedByValue& gv)
+{
+  DTB_TRY(gv.gid.alloc((size_t)n * 4, s));
+  DTB_TRY(gv.vg.alloc((size_t)n * stype_bytes(value.stype), s));
+  DTB_TRY(launch_expand_gid(offsets, ngroups, n, gv.gid.as<int32_t>(), s));
+  gv.ord = order;
+  if (!gv.ord) {
+    DTB_TRY(gv.iota.alloc((size_t)n * 4, s)); DTB_TRY(launch_iota32(gv.iota.as<int32_t>(), n, s)); gv.ord = gv.iota.p;
+  }
+  DTB_TRY(launch_gather(value.data, value.stype, nrows_value, gv.ord, 0, n, gv.vg.p, s));
+  dtb_col keys[2] = {{gv.gid.p, DTB_STYPE_INT32, 0}, {gv.vg.p, value.stype, 0}};
+  const int flags[2] = {flag, flag};
+  return group_core(keys, 2, flags, DTB_NA_FIRST, n, s, nullptr, nullptr, gv.res);
+}
+
 int dtb_sort_grouped(dtb_col value, int64_t nrows_value, const void* order, const void* offsets, int64_t ngroups,
                      dtb_stream stream, void* order_out)
 {
@@ -1564,20 +1590,49 @@ int dtb_sort_grouped(dtb_col value, int64_t nrows_value, const void* order, cons
   DTB_TRY(d_val.bind(value.data, (size_t)nrows_value * esz, s));
   DTB_TRY(d_ord.bind(order, (size_t)n * 4, s));
   DevOut d_out; DTB_TRY(d_out.bind(order_out, (size_t)n * 4, s));
-  // sort by (group id, value): the group id of every sorted position and the value seen through the RowIndex
-  DevBuf gid, vg, iota;
-  DTB_TRY(gid.alloc((size_t)n * 4, s));
-  DTB_TRY(vg.alloc((size_t)n * esz, s));
-  DTB_TRY(launch_expand_gid((const int32_t*)d_off.dptr, ngroups, n, gid.as<int32_t>(), s));
-  const void* ord = d_ord.dptr;
-  if (!ord) { DTB_TRY(iota.alloc((size_t)n * 4, s)); DTB_TRY(launch_iota32(iota.as<int32_t>(), n, s)); ord = iota.p; }
-  DTB_TRY(launch_gather(d_val.dptr, value.stype, nrows_value, ord, 0, n, vg.p, s));
-  dtb_col keys[2] = {{gid.p, DTB_STYPE_INT32, 0}, {vg.p, value.stype, 0}};
-  const int flags[2] = {DTB_FLAG_SORT_ONLY, DTB_FLAG_SORT_ONLY};
-  GroupResult res;
-  DTB_TRY(group_core(keys, 2, flags, DTB_NA_FIRST, n, s, nullptr, nullptr, res));
+  GroupedByValue gv;
+  DTB_TRY(group_by_value(dtb_col{d_val.dptr, value.stype, 0}, nrows_value, d_ord.dptr, (const int32_t*)d_off.dptr,
+                         ngroups, n, DTB_FLAG_SORT_ONLY, s, gv));
   // positions -> rows
-  DTB_TRY(launch_gather(ord, DTB_STYPE_INT32, n, res.order.p, 0, n, d_out.dptr, s));
+  DTB_TRY(launch_gather(gv.ord, DTB_STYPE_INT32, n, gv.res.order.p, 0, n, d_out.dptr, s));
+  if (d_out.staged()) DTB_TRY(d_out.finish((size_t)n * 4, s));
+  DTB_CUDA_CHECK(cudaStreamSynchronize(s));
+  return DTB_OK;
+}
+
+int dtb_qcut(dtb_col value, int64_t nrows_value, const void* order, const void* offsets, int64_t ngroups,
+             int nquantiles, dtb_stream stream, void* out)
+{
+  cudaStream_t s = (cudaStream_t)stream;
+  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
+  const int esz = stype_bytes(value.stype);
+  if (!esz) { set_error("qcut() cannot be applied to columns of stype " + std::to_string(value.stype)); return DTB_ENOTIMPL; }
+  if (nquantiles <= 0) {
+    set_error("Number of quantiles must be positive, instead got: " + std::to_string(nquantiles)); return DTB_EINVAL;
+  }
+  if (ngroups < 0) { set_error("ngroups must be non-negative"); return DTB_EINVAL; }
+  if (!offsets) { set_error("offsets is NULL"); return DTB_EINVAL; }
+  if (nrows_value < 0) { set_error("nrows_value must be non-negative"); return DTB_EINVAL; }
+  if (!value.data && nrows_value > 0) { set_error("value column data is NULL"); return DTB_EINVAL; }
+  DTB_TRY(ensure_context());
+  if (ngroups == 0) return DTB_OK;
+  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
+  DevIn d_off;
+  int64_t n = 0;
+  DTB_TRY(bind_groupby(offsets, ngroups, true, s, d_off, n));
+  if (!out) { set_error("out is NULL"); return DTB_EINVAL; }
+  if (!order && n > nrows_value) { set_error("offsets cover more rows than the value column has"); return DTB_EINVAL; }
+  DevIn d_val, d_ord;
+  DTB_TRY(d_val.bind(value.data, (size_t)nrows_value * esz, s));
+  DTB_TRY(d_ord.bind(order, (size_t)n * 4, s));
+  DevOut d_out; DTB_TRY(d_out.bind(out, (size_t)n * 4, s));
+  GroupedByValue gv;
+  DTB_TRY(group_by_value(dtb_col{d_val.dptr, value.stype, 0}, nrows_value, d_ord.dptr, (const int32_t*)d_off.dptr,
+                         ngroups, n, 0, s, gv));
+  const int64_t nc = gv.res.ngroups;
+  DevBuf scr; DTB_TRY(scr.alloc(qcut_scratch_bytes(nc, ngroups), s));
+  DTB_TRY(launch_qcut(gv.vg.p, value.stype, gv.res.order.as<int32_t>(), gv.res.offsets.as<int32_t>(), nc,
+                      gv.gid.as<int32_t>(), ngroups, n, nquantiles, scr.p, (int32_t*)d_out.dptr, s));
   if (d_out.staged()) DTB_TRY(d_out.finish((size_t)n * 4, s));
   DTB_CUDA_CHECK(cudaStreamSynchronize(s));
   return DTB_OK;

@@ -277,6 +277,12 @@ int launch_median(const void* v, int stype, int64_t nv, const int32_t* order, co
                   int64_t ng, void* out, cudaStream_t s);
 int launch_distinct_flags(const void* v, int stype, int64_t nv, const int32_t* order, const int32_t* offsets,
                           int64_t ng, int64_t n, int8_t* flag, cudaStream_t s);
+// qcut inside every group (dtb_qcut): cord / coff / nc are group() of the composite key (gid, vg), with gid / vg the
+// outer group id and the value at every RowIndex position (n of them, ng outer groups); out[pos]: int32 bins in the
+// outer RowIndex's layout.  scratch: qcut_scratch_bytes(nc, ng) of device memory.
+size_t qcut_scratch_bytes(int64_t nc, int64_t ng);
+int launch_qcut(const void* vg, int stype, const int32_t* cord, const int32_t* coff, int64_t nc, const int32_t* gid,
+                int64_t ng, int64_t n, int q, void* scratch, int32_t* out, cudaStream_t s);
 int launch_set_select(const int32_t* order, const int32_t* offsets, int64_t ng, const int64_t* d_sizes, int K,
                       int mode, uint8_t* flags, cudaStream_t s);
 int launch_set_emit(const int32_t* pos, int64_t nsel, const int32_t* order, const int32_t* offsets, int32_t* out_rows,

@@ -557,6 +557,110 @@ int launch_distinct_flags(const void* v, int stype, int64_t nv, const int32_t* o
 }
 
 // ===========================================================================
+// qcut (column/qcut.h:78-155) inside every group, over group() of the composite key (group id, value): cord / coff
+// are that group()'s RowIndex (sorted position -> RowIndex position of the outer Groupby) and offsets.  The group id
+// leads the key, so the composite groups of one outer group are contiguous; inside it they are its distinct values by
+// group()'s identity (bit patterns: -0.0 and +0.0 differ, every NaN is NA), NA first.
+//   qcut_starts_kernel  per composite group c: cog[c] = its outer group, cstart[og] = first composite group of og
+//   qcut_coef_kernel    per outer group: G, has_na and the coefficients a, b of Qcut_ColumnImpl::materialize
+//   qcut_emit_kernel    per sorted position (a single value may hold most rows): out[pos] = int32(a * i + b) with
+//                       i = c - cstart[og], NA for the NA group
+// a * i + b is a multiply and an add, each rounded (__dmul_rn / __dadd_rn), as the reference computes it: a
+// contracted FMA could round differently.
+// ===========================================================================
+__global__ void qcut_starts_kernel(const int32_t* __restrict__ cord, const int32_t* __restrict__ coff, int64_t nc,
+                                   const int32_t* __restrict__ gid, int64_t ng, int32_t* __restrict__ cog,
+                                   int32_t* __restrict__ cstart)
+{
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < nc; c += stride) {
+    const int32_t og = gid[cord[coff[c]]];
+    cog[c] = og;
+    if (c == 0 || gid[cord[coff[c - 1]]] != og) cstart[og] = (int32_t)c;
+    if (c == nc - 1) cstart[ng] = (int32_t)nc;
+  }
+}
+
+template <typename T>
+__global__ void qcut_coef_kernel(const void* __restrict__ vg, const int32_t* __restrict__ cord,
+                                 const int32_t* __restrict__ coff, const int32_t* __restrict__ cstart, int64_t ng,
+                                 int q, double2* __restrict__ coef, uint8_t* __restrict__ has_na)
+{
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += stride) {
+    const int64_t c0 = cstart[g];
+    const int64_t G = (int64_t)cstart[g + 1] - c0;
+    const bool na = !elem_valid<T>(vg, cord[coff[c0]]);      // NA first: the group's first value
+    const int64_t V = G - (na ? 1 : 0);
+    double a, b;
+    if (V <= 1) {                                              // one valid value (or none: only the NA group)
+      a = 0.0;
+      b = (double)((q - 1) / 2);
+    } else {                                                   // q * (1 - FLT_EPSILON) / (V - 1), b = -a * has_na
+      a = __ddiv_rn(__dmul_rn((double)q, 1.0 - 1.0 / 8388608.0), (double)(V - 1));     // FLT_EPSILON = 2^-23
+      b = __dmul_rn(-a, na ? 1.0 : 0.0);
+    }
+    coef[g] = make_double2(a, b);
+    has_na[g] = na ? 1 : 0;
+  }
+}
+
+__global__ void qcut_emit_kernel(const int32_t* __restrict__ cord, const int32_t* __restrict__ coff, int64_t nc,
+                                 int64_t n, const int32_t* __restrict__ cog, const int32_t* __restrict__ cstart,
+                                 const double2* __restrict__ coef, const uint8_t* __restrict__ has_na,
+                                 int32_t* __restrict__ out)
+{
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x * 8;
+  for (int64_t k0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 8; k0 < n; k0 += stride) {
+    int64_t lo = 0, hi = nc;                       // largest c with coff[c] <= k0
+    while (hi - lo > 1) { const int64_t mid = (lo + hi) >> 1; if ((int64_t)coff[mid] <= k0) lo = mid; else hi = mid; }
+    int64_t c = lo, next = coff[c + 1];
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+      const int64_t k = k0 + j;
+      if (k >= n) break;
+      while (k >= next) { c++; next = coff[c + 1]; }
+      const int32_t og = cog[c];
+      const int64_t i = c - cstart[og];
+      int32_t bin = INT32_MIN;
+      if (i > 0 || !has_na[og]) {
+        const double2 ab = coef[og];
+        bin = (int32_t)__dadd_rn(__dmul_rn(ab.x, (double)i), ab.y);
+      }
+      out[cord[k]] = bin;
+    }
+  }
+}
+
+size_t qcut_scratch_bytes(int64_t nc, int64_t ng) {
+  return sizeof(double2) * (size_t)ng + sizeof(int32_t) * (size_t)(ng + 1 + nc) + (size_t)ng;
+}
+
+int launch_qcut(const void* vg, int stype, const int32_t* cord, const int32_t* coff, int64_t nc, const int32_t* gid,
+                int64_t ng, int64_t n, int q, void* scratch, int32_t* out, cudaStream_t s)
+{
+  if (n == 0 || ng == 0) return DTB_OK;
+  double2* coef = (double2*)scratch;
+  int32_t* cstart = (int32_t*)(coef + ng);
+  int32_t* cog = cstart + ng + 1;
+  uint8_t* has_na = (uint8_t*)(cog + nc);
+  {
+    ProfScope ps("qcut_coef", s);
+    qcut_starts_kernel<<<grid_for(nc), 256, 0, s>>>(cord, coff, nc, gid, ng, cog, cstart);
+#define CALL(T) qcut_coef_kernel<T><<<grid_for(ng), 256, 0, s>>>(vg, cord, coff, cstart, ng, q, coef, has_na)
+    DTB_DISPATCH_STYPE(stype, CALL)
+#undef CALL
+    count_launch(2);
+    DTB_CUDA_CHECK(cudaGetLastError());
+  }
+  ProfScope ps("qcut_emit", s);
+  qcut_emit_kernel<<<grid_for((n + 7) / 8), 256, 0, s>>>(cord, coff, nc, n, cog, cstart, coef, has_na, out);
+  count_launch();
+  DTB_CUDA_CHECK(cudaGetLastError());
+  return DTB_OK;
+}
+
+// ===========================================================================
 // Set operations (set_funcs.cc): the K input columns were concatenated (column k holds the rows
 // sizes[k-1] .. sizes[k]-1) and grouped; a group is kept depending on which inputs its rows come from.
 // Inside a group the RowIndex ascends, so the rows of input k are contiguous.

@@ -414,6 +414,26 @@ def sort_grouped(value, order, offsets, stype=None):
     return out
 
 
+def qcut(value, order, offsets, nquantiles=10, stype=None):
+    """Qcut_ColumnImpl (column/qcut.h:78-155) inside every group of (order, offsets), as dt.qcut under by()
+    (expr/fexpr_qcut.cc:118-146); one group [0, n] without by().  Returns the int32 bins, one per position of the
+    RowIndex (order None = identity), NA as INT32_MIN; in HBM when the inputs are."""
+    v = Col(value, stype)
+    f = Col(offsets)
+    ngroups = f.nrows - 1
+    o = None if order is None else Col(order)
+    if o is not None and o.stype != INT32:
+        raise _lib.DtbValueError("order must be int32")
+    if not -2**31 <= int(nquantiles) < 2**31:
+        raise _lib.DtbValueError(f"nquantiles does not fit in an int32: {nquantiles}")
+    n = (int(offsets[-1].item()) if is_tensor(offsets) else int(offsets[-1])) if ngroups > 0 else 0
+    device = v.on_device and f.on_device and (o is None or o.on_device)
+    out, optr = _alloc(n, INT32, device)
+    check(lib.dtb_qcut(v.c(), v.nrows, ctypes.c_void_p(o.ptr) if o is not None else None, ctypes.c_void_p(f.ptr),
+                       ngroups, int(nquantiles), _stream(), ctypes.c_void_p(optr)))
+    return out
+
+
 def set_select(mode, order, offsets, cum_sizes):
     """Group selection of union / intersect / setdiff / symdiff (set_funcs.cc:126-456): the first-row
     indices of the groups the operation keeps (int32, same memory kind as `order`)."""

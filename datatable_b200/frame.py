@@ -109,6 +109,66 @@ def count(x=None):
     return Reducer(_lib.OP_NROWS if x is None else _lib.OP_COUNT, "count", x)
 
 
+class Qcut:
+    """dt.qcut(cols, nquantiles=None) (expr/fexpr_qcut.cc:41-181): the column references and nquantiles as given; the
+    columns are resolved, and nquantiles checked, when the query runs (FExpr_Qcut::evaluate_n)."""
+    def __init__(self, cols, nquantiles):
+        self.cols, self.nquantiles = cols, nquantiles
+
+
+class QcutCol:
+    """One column of a qcut(): the bins of column `name` into `nquantiles` quantiles, per group under by()."""
+    def __init__(self, name, nquantiles):
+        self.name, self.nquantiles = name, nquantiles
+
+
+def qcut(cols, nquantiles=None):
+    return Qcut(cols, nquantiles)
+
+
+def _to_int32_strict(x):
+    """py::robj::to_int32_strict: an int (not a bool) that fits in an int32."""
+    if not isinstance(x, int) or isinstance(x, bool):
+        raise TypeError(f"Expected an integer, instead got {type(x)}")
+    if x > 2**31 - 1:
+        raise ValueError(f"Value is too large to fit in an int32: {x}")
+    if x < -2**31:
+        raise ValueError(f"Value is too small to fit in an int32: {x}")
+    return x
+
+
+def _qcut_cols(DT, e, bynames):
+    """FExpr_Qcut::evaluate_n (fexpr_qcut.cc:64-115): one QcutCol per input column, with the reference's checks of
+    nquantiles.  f[:] under by() leaves out the by() columns."""
+    refs = []
+    for c in _flatten([e.cols]):
+        if isinstance(c, ColRef) and isinstance(c.name, slice):
+            if c.name != slice(None):
+                raise NotImplementedError("column slices other than f[:] are outside the GPU hot path")
+            refs += [ColRef(nm) for nm in DT.names if nm not in bynames]
+        else:
+            refs.append(_as_ref(c))
+    nq = e.nquantiles
+    if isinstance(nq, (list, tuple)):
+        if len(nq) != len(refs):
+            raise ValueError(f"When nquantiles is a list or a tuple, its length must be the same as the number of "
+                             f"input columns, i.e. {len(refs)}, instead got: {len(nq)}")
+        qs = []
+        for i, x in enumerate(nq):
+            x = _to_int32_strict(x)
+            if x <= 0:
+                raise ValueError(f"All elements in nquantiles must be positive, got nquantiles[{i}]: {x}")
+            qs.append(x)
+    else:
+        q = 10
+        if nq is not None:
+            q = _to_int32_strict(nq)
+            if q <= 0:
+                raise ValueError(f"Number of quantiles must be positive, instead got: {q}")
+        qs = [q] * len(refs)
+    return [QcutCol(r.name, q) for r, q in zip(refs, qs)]
+
+
 class by:
     def __init__(self, *cols):
         self.cols = [_as_ref(c) for c in _flatten(cols)]
@@ -411,13 +471,13 @@ def _evaluate(DT, j, by_, sort_, isel=None):
     if by_ is not None and sort_ is not None and sort_.na_position == "remove":
         # the rows dropped from the front of the RowIndex would still be counted by the groups
         raise ValueError("na_position = \"remove\" in sort() is not supported together with by()")
+    names, exprs = _resolve_j(DT, j, [r.name for r in by_.cols] if by_ is not None else ())
     # Host columns are uploaded once (pinned memory -> DMA), the whole query then runs on
     # HBM-resident buffers, and only the result frame travels back.
     if torch is None or not torch.cuda.is_available():
         raise _lib.DtbCudaError("no usable CUDA device: datatable_b200 has no CPU fallback")
     host_frame = not any(engine.is_tensor(c) and c.is_cuda for c in DT._cols.values())
     cache = {}
-    names, exprs = _resolve_j(DT, j)
 
     # Host columns: start every upload the query needs on a copy stream, key columns first, so
     # that the PCIe transfer of the value columns overlaps the sort of the keys; each column is
@@ -635,7 +695,10 @@ def _evaluate(DT, j, by_, sort_, isel=None):
             if e.name in bynames and j_is_all(j):
                 continue
             c = dcol(e.name)
-            add(name, engine.gather(c, order), c.stype)
+            if isinstance(e, QcutCol):                     # qcut inside every group, in the grouped order (GtoALL)
+                add(name, engine.qcut(c, order, offsets, e.nquantiles), INT32)
+            else:
+                add(name, engine.gather(c, order), c.stype)
         out._nrows = len(order)
         return out
 
@@ -651,7 +714,12 @@ def _evaluate(DT, j, by_, sort_, isel=None):
         return out
 
     for name, e in zip(names, exprs):
-        if order is None:
+        if isinstance(e, QcutCol):
+            # no Groupby (sort() alone, an `i` slice, or neither): one qcut over the selected rows in their order
+            nsel = DT.nrows if order is None else len(order)
+            offs = torch.tensor([0, nsel] if nsel else [0], dtype=torch.int32, device="cuda")
+            add(name, engine.qcut(dcol(e.name), order, offs, e.nquantiles), INT32)
+        elif order is None:
             c = DT._col(e.name)
             out._cols[name] = c.data; out._stypes[name] = c.stype
         else:
@@ -665,20 +733,27 @@ def j_is_all(j):
     return isinstance(j, slice) and j == slice(None)
 
 
-def _resolve_j(DT, j):
+def _resolve_j(DT, j, bynames=()):
     if j_is_all(j):
         return list(DT.names), [ColRef(n) for n in DT.names]
     if isinstance(j, dict):
         names, es = [], []
         for k, v in j.items():
             vs = v if isinstance(v, list) else [v]              # a broadcast cov / corr: k, k.0, k.1, ... (see add)
-            names += [k] * len(vs)
-            es += [_as_expr(x) for x in vs]
+            for x in vs:
+                if isinstance(x, Qcut):                         # several columns: k.x, k.y, ...
+                    qc = _qcut_cols(DT, x, bynames)
+                    names += [k] if len(qc) == 1 else [f"{k}.{c.name}" for c in qc]
+                    es += qc
+                else:
+                    names.append(k)
+                    es.append(_as_expr(x))
         return names, es
     if isinstance(j, (list, tuple)):
         es = [_as_expr(x) for v in j for x in (v if isinstance(v, list) else [v])]
     else:
         es = [_as_expr(x) for x in (j if isinstance(j, list) else [j])]
+    es = [c for e in es for c in (_qcut_cols(DT, e, bynames) if isinstance(e, Qcut) else [e])]
     names = []
     nbin = 0
     for e in es:
@@ -693,7 +768,7 @@ def _resolve_j(DT, j):
 
 
 def _as_expr(v):
-    if isinstance(v, (Reducer, ColRef)):
+    if isinstance(v, (Reducer, ColRef, Qcut)):
         return v
     if isinstance(v, str):
         return ColRef(v)

@@ -331,6 +331,25 @@ DTB_API int dtb_sort_grouped(dtb_col value, int64_t nrows_value, const void* ord
                      int64_t ngroups, dtb_stream stream, void* order_out);
 
 /*
+ * dtb_qcut -- replaces Qcut_ColumnImpl::materialize (column/qcut.h:78-155) run on every group, as
+ * FExpr_Qcut::evaluate_n does under by() (expr/fexpr_qcut.cc:64-158).  The value column is seen through `order`
+ * (int32 RowIndex; NULL = identity) and cut by `offsets` (int32[ngroups+1], a Groupby: offsets[0] = 0, strictly
+ * increasing; one group [0, n] for a call without by()).  Inside every group the distinct values are numbered
+ * i = 0 .. G-1 in group()'s order, NA first; has_na = the first one is NA, V = G - has_na, q = nquantiles:
+ *   V <= 1:  a = 0, b = (q - 1) / 2 (integer division)
+ *   else:    a = q * (1 - FLT_EPSILON) / (V - 1), b = -a * has_na
+ * and every row of value i gets int32(a * i + b), truncated; the rows of the NA value get NA.
+ *   - Values are told apart as group() tells them: -0.0 and +0.0 are different values, every NaN is the NA value.
+ *   - a * i + b is a multiply and an add, each rounded to nearest (no fused multiply-add), as the reference
+ *     computes it.
+ * out: int32[offsets[ngroups]], out[p] = the bin of the row at position p of the RowIndex (the GtoALL layout of
+ * the grouped frame).  Host or device pointers.  nquantiles <= 0: DTB_EINVAL; an stype without a fixed width:
+ * DTB_ENOTIMPL.  Up to INT32_MAX rows.
+ */
+DTB_API int dtb_qcut(dtb_col value, int64_t nrows_value, const void* order, const void* offsets, int64_t ngroups,
+                     int nquantiles, dtb_stream stream, void* out);
+
+/*
  * dtb_set_select -- the group-selection step of union / intersect / setdiff / symdiff
  * (set_funcs.cc:126-456).  The caller concatenated K single-column inputs (input k holds the rows
  * cum_sizes[k-1] .. cum_sizes[k]-1), grouped the result with dtb_group and passes its (order, offsets).
