@@ -30,7 +30,7 @@ EXPORTS = [
     "dtb_gather", "dtb_memcpy", "dtb_set_option", "dtb_get_option", "dtb_last_call_stats",
     "dtb_profile_count", "dtb_profile_get", "dtb_profile_reset",
     "dtb_dense_scatter", "dtb_dense_compact",
-    "dtb_sort_grouped", "dtb_qcut", "dtb_set_select", "dtb_largest_group", "dtb_join", "dtb_cache_begin", "dtb_cache_end", "dtb_lower_bound",
+    "dtb_sort_grouped", "dtb_qcut", "dtb_cumulative_out_stype", "dtb_cumulative", "dtb_set_select", "dtb_largest_group", "dtb_join", "dtb_cache_begin", "dtb_cache_end", "dtb_lower_bound",
 ]
 
 
@@ -123,6 +123,9 @@ def _load():
                                       c.POINTER(c.c_int64), c.c_void_p]
     lib.dtb_sort_grouped.argtypes = [dtb_col, c.c_int64, c.c_void_p, c.c_void_p, c.c_int64, c.c_void_p, c.c_void_p]
     lib.dtb_qcut.argtypes = [dtb_col, c.c_int64, c.c_void_p, c.c_void_p, c.c_int64, c.c_int, c.c_void_p, c.c_void_p]
+    lib.dtb_cumulative_out_stype.argtypes = [c.c_int, c.c_int]
+    lib.dtb_cumulative.argtypes = [c.c_int, c.c_int, dtb_col, c.c_int64, c.c_void_p, c.c_int, c.c_void_p, c.c_int64,
+                                   c.c_void_p, c.c_void_p]
     lib.dtb_set_select.argtypes = [c.c_int, c.c_void_p, c.c_void_p, c.c_int64, c.POINTER(c.c_int64), c.c_int,
                                    c.c_void_p, c.c_void_p, c.POINTER(c.c_int64)]
     lib.dtb_largest_group.argtypes = [c.c_void_p, c.c_int64, c.c_int64, c.c_void_p, c.POINTER(c.c_int64),

@@ -1379,6 +1379,53 @@ int dtb_groupby_reduce2(dtb_groupby* g, int op, dtb_col x, dtb_col y, int64_t nr
   return reduce2_groups(op, x, y, nrows_value, g->order, 0, g->offsets, g->ngroups, stream, out, false);
 }
 
+int dtb_cumulative_out_stype(int op, int stype) { return cumulative_out_stype(op, stype); }
+
+int dtb_cumulative(int op, int reverse, dtb_col value, int64_t nrows_value, const void* order, int order_is64,
+                   const void* offsets, int64_t ngroups, dtb_stream stream, void* out)
+{
+  cudaStream_t s = (cudaStream_t)stream;
+  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
+  if (op != DTB_OP_SUM && op != DTB_OP_PROD && op != DTB_OP_MIN && op != DTB_OP_MAX) {
+    set_error("dtb_cumulative takes DTB_OP_SUM, DTB_OP_PROD, DTB_OP_MIN or DTB_OP_MAX"); return DTB_EINVAL;
+  }
+  const int esz = stype_bytes(value.stype);
+  if (!esz) { set_error("cumulative functions cannot be applied to columns of stype " + std::to_string(value.stype)); return DTB_ENOTIMPL; }
+  const int out_st = cumulative_out_stype(op, value.stype);
+  if (!out_st) {
+    set_error("Invalid column of stype " + std::to_string(value.stype) + " in cumulative function " + std::to_string(op));
+    return DTB_EINVAL;
+  }
+  if (ngroups < 0) { set_error("ngroups must be non-negative"); return DTB_EINVAL; }
+  if (!offsets) { set_error("offsets is NULL"); return DTB_EINVAL; }
+  if (nrows_value < 0) { set_error("nrows_value must be non-negative"); return DTB_EINVAL; }
+  if (!value.data && nrows_value > 0) { set_error("value column data is NULL"); return DTB_EINVAL; }
+  DTB_TRY(ensure_context());
+  if (ngroups == 0) return DTB_OK;
+  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
+  DevIn d_off;
+  int64_t n = 0;
+  DTB_TRY(bind_groupby(offsets, ngroups, true, s, d_off, n));
+  if (!out) { set_error("out is NULL"); return DTB_EINVAL; }
+  if (!order && n > nrows_value) { set_error("offsets cover more rows than the value column has"); return DTB_EINVAL; }
+  DevIn d_val, d_ord;
+  DTB_TRY(d_val.bind(value.data, (size_t)nrows_value * esz, s));
+  DTB_TRY(d_ord.bind(order, (size_t)n * (order_is64 ? 8 : 4), s));
+  const size_t out_bytes = (size_t)n * stype_bytes(out_st);
+  DevOut d_out; DTB_TRY(d_out.bind(out, out_bytes, s));
+  DevBuf scr; DTB_TRY(scr.alloc(cumulative_scratch_bytes(n), s));
+  {
+    ProfScope ps("cumulative", s);
+    DTB_TRY(launch_cumulative(op, reverse, d_val.dptr, value.stype, nrows_value, d_ord.dptr, order_is64,
+                              (const int32_t*)d_off.dptr, ngroups, n, scr.p, d_out.dptr, s));
+  }
+  if (d_out.staged()) {
+    DTB_TRY(d_out.finish(out_bytes, s));
+    DTB_CUDA_CHECK(cudaStreamSynchronize(s));
+  }
+  return DTB_OK;
+}
+
 int dtb_groupby_reduce_begin(dtb_groupby* g, int op, int value_stype, dtb_stream stream, dtb_reduce_state** out)
 {
   cudaStream_t s = (cudaStream_t)stream;

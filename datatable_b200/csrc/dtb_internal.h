@@ -283,6 +283,13 @@ int launch_distinct_flags(const void* v, int stype, int64_t nv, const int32_t* o
 size_t qcut_scratch_bytes(int64_t nc, int64_t ng);
 int launch_qcut(const void* vg, int stype, const int32_t* cord, const int32_t* coff, int64_t nc, const int32_t* gid,
                 int64_t ng, int64_t n, int q, void* scratch, int32_t* out, cudaStream_t s);
+// cumsum / cumprod / cummin / cummax inside every group (dtb_cumulative, dtb_reduce.cu): op DTB_OP_SUM / PROD / MIN /
+// MAX; out[p]: n elements of cumulative_out_stype(op, stype) (0: the op refuses the stype) for RowIndex position p.
+// scratch: cumulative_scratch_bytes(n) of device memory.
+int cumulative_out_stype(int op, int stype);
+size_t cumulative_scratch_bytes(int64_t n);
+int launch_cumulative(int op, int reverse, const void* v, int stype, int64_t nv, const void* order, int order_is64,
+                      const int32_t* offsets, int64_t ng, int64_t n, void* scratch, void* out, cudaStream_t s);
 int launch_set_select(const int32_t* order, const int32_t* offsets, int64_t ng, const int64_t* d_sizes, int K,
                       int mode, uint8_t* flags, cudaStream_t s);
 int launch_set_emit(const int32_t* pos, int64_t nsel, const int32_t* order, const int32_t* offsets, int32_t* out_rows,

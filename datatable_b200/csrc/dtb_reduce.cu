@@ -52,6 +52,18 @@ __device__ __forceinline__ void prodf_mul(Partial<CAT_PRODF>& a, double m, int64
   a.f = ((a.f | f) & 3u) | ((a.f ^ f) & 4u);
 }
 
+// The value of a float product: zero and infinity together give NA (0 * inf, valid = false), otherwise a zero or an
+// infinity with the sign parity, otherwise m * 2^e rounded once to float64.
+__device__ __forceinline__ double prodf_value(const Partial<CAT_PRODF>& p, bool& valid) {
+  const bool neg = (p.f & 4u) != 0;
+  double r;
+  if (p.f & 1u) r = neg ? -0.0 : 0.0;
+  else if (p.f & 2u) r = neg ? -INFINITY : INFINITY;
+  else r = ldexp(neg ? -p.m : p.m, (int)(p.e < -4000 ? -4000 : (p.e > 4000 ? 4000 : p.e)));
+  valid = (p.f & 3u) != 3u;
+  return r;
+}
+
 template <int CAT>
 __device__ __forceinline__ void p_init(Partial<CAT>& p, int flag) {
   if constexpr (CAT == CAT_SUMI) p.s = 0;
@@ -168,6 +180,36 @@ __device__ __forceinline__ void p_add(Partial<CAT>& p, typename RawKey<T>::load_
   }
 }
 
+// The head bitmap of the tile of positions [t0, t1): bit p of s_bits is set where a group starts at t0 + p, p >= 1
+// (s_bits zeroed by the caller).  g_lo / g_hi: the groups of the tile's first and last positions.  REV: positions
+// are mirrored (p -> n - 1 - p), so group g starts at n - offsets[ng - g].
+template <bool REV>
+__device__ __forceinline__ int64_t head_offset(const int32_t* __restrict__ offsets, int64_t ng, int64_t n, int64_t g) {
+  return REV ? n - (int64_t)offsets[ng - g] : (int64_t)offsets[g];
+}
+
+template <bool REV>
+__device__ __forceinline__ void tile_heads(const int32_t* __restrict__ offsets, int64_t ng, int64_t n, int64_t t0,
+                                           int64_t t1, int tid, int64_t* s_g, u32* s_bits, int64_t& g_lo, int64_t& g_hi) {
+  if (tid == 0 || tid == 32) {
+    // largest g with offsets[g] <= pos
+    const int64_t pos = (tid == 0) ? t0 : (t1 - 1);
+    int64_t lo = 0, hi = ng;             // offsets[0] = 0 <= pos < offsets[ng] = n
+    while (hi - lo > 1) {
+      int64_t mid = (lo + hi) >> 1;
+      if (head_offset<REV>(offsets, ng, n, mid) <= pos) lo = mid; else hi = mid;
+    }
+    s_g[tid ? 1 : 0] = lo;
+  }
+  __syncthreads();
+  g_lo = s_g[0]; g_hi = s_g[1];
+  for (int64_t g = g_lo + 1 + tid; g <= g_hi; g += RT) {
+    const int p = (int)(head_offset<REV>(offsets, ng, n, g) - t0);    // 1 .. RTILE-1
+    atomicOr(&s_bits[p >> 5], 1u << (p & 31));
+  }
+  __syncthreads();
+}
+
 template <typename T, int CAT, typename OrdT>
 __global__ void __launch_bounds__(RT)
 reduce_kernel(const typename RawKey<T>::load_t* __restrict__ v, int64_t nv,
@@ -190,23 +232,8 @@ reduce_kernel(const typename RawKey<T>::load_t* __restrict__ v, int64_t nv,
     s_slot = s_prod;
     if (tid < 4) s_prod[tid] = (CAT == CAT_PRODI && tid < 2) ? 1ull : 0ull;
   }
-  if (tid == 0 || tid == 32) {
-    // largest g with offsets[g] <= pos
-    const int64_t pos = (tid == 0) ? t0 : (t1 - 1);
-    int64_t lo = 0, hi = ng;             // offsets[0] = 0 <= pos < offsets[ng] = n
-    while (hi - lo > 1) {
-      int64_t mid = (lo + hi) >> 1;
-      if ((int64_t)offsets[mid] <= pos) lo = mid; else hi = mid;
-    }
-    s_g[tid ? 1 : 0] = lo;
-  }
-  __syncthreads();
-  const int64_t g_lo = s_g[0], g_hi = s_g[1];
-  for (int64_t g = g_lo + 1 + tid; g <= g_hi; g += RT) {
-    const int p = (int)((int64_t)offsets[g] - t0);          // 1 .. RTILE-1
-    atomicOr(&s_bits[p >> 5], 1u << (p & 31));
-  }
-  __syncthreads();
+  int64_t g_lo, g_hi;
+  tile_heads<false>(offsets, ng, n, t0, t1, tid, s_g, s_bits, g_lo, g_hi);
   if (tid < 32) {
     // exclusive prefix of popcounts over the RTILE/32 = 64 bitmap words (2 per lane)
     u32 a = __popc(s_bits[2 * lane]), b = __popc(s_bits[2 * lane + 1]);
@@ -527,12 +554,8 @@ __global__ void prod_finalize_kernel(const int32_t* __restrict__ offsets, int64_
     if constexpr (CAT == CAT_PRODI) {
       ((int64_t*)out)[g] = (int64_t)p.p;
     } else {
-      const bool neg = (p.f & 4u) != 0;
-      double r;
-      if (p.f & 1u) r = neg ? -0.0 : 0.0;
-      else if (p.f & 2u) r = neg ? -INFINITY : INFINITY;
-      else r = ldexp(neg ? -p.m : p.m, (int)(p.e < -4000 ? -4000 : (p.e > 4000 ? 4000 : p.e)));
-      const bool valid = (p.f & 3u) != 3u;
+      bool valid;
+      const double r = prodf_value(p, valid);
       // float32: the float64 r is exact wherever a float32 result is not 0, so this rounds once
       if (out_stype == DTB_STYPE_FLOAT32) ((u32*)out)[g] = valid ? __float_as_uint((float)r) : 0x7FC00000u;
       else ((u64*)out)[g] = valid ? (u64)__double_as_longlong(r) : 0x7FF8000000000000ull;
@@ -661,6 +684,380 @@ int launch_nrows(const int32_t* offsets, int64_t ng, void* out, cudaStream_t s) 
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;
+}
+
+// ===========================================================================
+// Cumulative functions per group: cumsum / cumprod / cummin / cummax (dtb_cumulative)
+// ===========================================================================
+// Replaces CumSumProd_ColumnImpl (column/cumsumprod.h) and CumMinMax_ColumnImpl (column/cumminmax.h), which scan
+// every group sequentially.  Here it is a segmented scan over the RowIndex positions in fixed tiles of RTILE, so a
+// single long group does not serialise it, and the combining order is fixed (two calls give the same bytes):
+//   cum_tile_kernel   gathers every position's value through the RowIndex once, writes its contribution to the
+//                     scan into out[p] (every output type holds its input type), and the tile's segmented aggregate
+//                     (the fold since its last group head) with a flag "the tile holds a head";
+//   cum_carry_kernel  one CTA: segmented scan of the tiles' aggregates into every tile's carry-in;
+//   cum_emit_kernel   reads the contributions back in order and writes the prefixes, carry-in included.
+// REV (reverse=True) mirrors the positions, p -> n - 1 - p, and the offsets with them.
+// Bound: HBM (one random gather per row, like dtb_gather, plus one sequential read and write of out).
+
+// One cumulative function over input type T: the scan state S, the element type O of out, the contribution of one
+// row (what the tile kernel writes into out), the fold, the merge (a = a then b) and the result of a state.
+enum { CUM_SUMI, CUM_SUMF, CUM_PRODI, CUM_PRODF, CUM_MIN, CUM_MAX };
+
+template <typename T> struct CumMM { typename RawKey<T>::load_t b; };   // the latest extreme, or T's NA = none
+
+template <int K, typename T> struct Cum;
+
+template <typename T> struct Cum<CUM_SUMI, T> {            // wraps modulo 2^64; an NA row adds 0
+  typedef Partial<CAT_SUMI> S; typedef u64 O;
+  static __device__ __forceinline__ O contrib(typename RawKey<T>::load_t raw, bool row_valid) {
+    u64 u; return (RawKey<T>::get(raw, u) && row_valid) ? u : 0ull;
+  }
+  static __device__ __forceinline__ void init(S& a) { p_init(a, 0); }
+  static __device__ __forceinline__ void add(S& a, O c) { a.s += c; }
+  static __device__ __forceinline__ void merge(S& a, const S& b) { p_merge(a, b, 0); }
+  static __device__ __forceinline__ S shfl_up(const S& a, int d) { return p_shfl_up(a, d); }
+  static __device__ __forceinline__ O result(const S& a) { return a.s; }
+};
+
+// Float sums run in float64 and each prefix is rounded once.  An NA row adds +0.0 and the scan starts at -0.0, the
+// identity, so a prefix of zeros is -0.0 exactly when every row so far is -0.0, as in the reference's loop.
+template <typename T> struct Cum<CUM_SUMF, T> {
+  typedef Partial<CAT_SUMF> S; typedef typename RawKey<T>::load_t O;
+  static __device__ __forceinline__ O contrib(O raw, bool row_valid) {
+    u64 u; return (RawKey<T>::get(raw, u) && row_valid) ? raw : (O)0;
+  }
+  static __device__ __forceinline__ void init(S& a) { a.s = -0.0; }
+  static __device__ __forceinline__ void add(S& a, O c) {
+    if constexpr (std::is_same<T, float>::value) a.s += (double)__uint_as_float((u32)c);
+    else a.s += __longlong_as_double((long long)c);
+  }
+  static __device__ __forceinline__ void merge(S& a, const S& b) { p_merge(a, b, 0); }
+  static __device__ __forceinline__ S shfl_up(const S& a, int d) { return p_shfl_up(a, d); }
+  static __device__ __forceinline__ O result(const S& a) {
+    if constexpr (std::is_same<T, float>::value) return (O)__float_as_uint((float)a.s);
+    else return (O)__double_as_longlong(a.s);
+  }
+};
+
+template <typename T> struct Cum<CUM_PRODI, T> {           // wraps modulo 2^64; an NA row multiplies by 1
+  typedef Partial<CAT_PRODI> S; typedef u64 O;
+  static __device__ __forceinline__ O contrib(typename RawKey<T>::load_t raw, bool row_valid) {
+    u64 u; return (RawKey<T>::get(raw, u) && row_valid) ? u : 1ull;
+  }
+  static __device__ __forceinline__ void init(S& a) { p_init(a, 0); }
+  static __device__ __forceinline__ void add(S& a, O c) { a.p *= c; }
+  static __device__ __forceinline__ void merge(S& a, const S& b) { p_merge(a, b, 0); }
+  static __device__ __forceinline__ S shfl_up(const S& a, int d) { return p_shfl_up(a, d); }
+  static __device__ __forceinline__ O result(const S& a) { return a.p; }
+};
+
+// Float products keep the significand and the exponent apart (Partial<CAT_PRODF>); an NA row multiplies by 1.0.
+template <typename T> struct Cum<CUM_PRODF, T> {
+  typedef Partial<CAT_PRODF> S; typedef typename RawKey<T>::load_t O;
+  static constexpr O ONE = std::is_same<T, float>::value ? (O)0x3F800000u : (O)0x3FF0000000000000ull;
+  static __device__ __forceinline__ O contrib(O raw, bool row_valid) {
+    u64 u; return (RawKey<T>::get(raw, u) && row_valid) ? raw : ONE;
+  }
+  static __device__ __forceinline__ void init(S& a) { p_init(a, 0); }
+  static __device__ __forceinline__ void add(S& a, O c) { p_add<T, CAT_PRODF>(a, c, true, 0); }
+  static __device__ __forceinline__ void merge(S& a, const S& b) { p_merge(a, b, 0); }
+  static __device__ __forceinline__ S shfl_up(const S& a, int d) { return p_shfl_up(a, d); }
+  static __device__ __forceinline__ O result(const S& a) {
+    bool valid;
+    const double r = prodf_value(a, valid);
+    if constexpr (std::is_same<T, float>::value) return valid ? (O)__float_as_uint((float)r) : (O)0x7FC00000u;
+    else return valid ? (O)__double_as_longlong(r) : (O)0x7FF8000000000000ull;
+  }
+};
+
+// cummin / cummax: the state is the latest row holding the extreme so far, compared in T (prev < val ? prev : val
+// for min, > for max), so of equal values -- -0.0 and +0.0 included -- the later one wins.  "Latest among the
+// extremes" is associative.  An NA row leaves the state as it is; before the first valid row the state is NA.
+template <int K, typename T> struct CumMinMax {
+  typedef CumMM<T> S; typedef typename RawKey<T>::load_t O;
+  static __device__ __forceinline__ O contrib(O raw, bool row_valid) { return row_valid ? raw : na(); }
+  static __device__ __forceinline__ O na() {
+    if constexpr (std::is_same<T, float>::value) return (O)0x7FC00000u;
+    else if constexpr (std::is_same<T, double>::value) return (O)0x7FF8000000000000ull;
+    else return NaOf<T>::v();
+  }
+  static __device__ __forceinline__ bool valid(O b) { u64 u; return RawKey<T>::get(b, u); }
+  static __device__ __forceinline__ T val(O b) {
+    if constexpr (std::is_same<T, float>::value) return __uint_as_float((u32)b);
+    else if constexpr (std::is_same<T, double>::value) return __longlong_as_double((long long)b);
+    else return b;
+  }
+  static __device__ __forceinline__ void init(S& a) { a.b = na(); }
+  static __device__ __forceinline__ void add(S& a, O c) {
+    if (!valid(c)) return;
+    if (valid(a.b) && (K == CUM_MIN ? val(a.b) < val(c) : val(a.b) > val(c))) return;
+    a.b = c;
+  }
+  static __device__ __forceinline__ void merge(S& a, const S& b) { add(a, b.b); }
+  static __device__ __forceinline__ S shfl_up(const S& a, int d) { S r; r.b = __shfl_up_sync(0xffffffffu, a.b, d); return r; }
+  static __device__ __forceinline__ O result(const S& a) { return a.b; }
+};
+template <typename T> struct Cum<CUM_MIN, T> : CumMinMax<CUM_MIN, T> {};
+template <typename T> struct Cum<CUM_MAX, T> : CumMinMax<CUM_MAX, T> {};
+
+// (a, f) = (pa, pf) then (a, f): a segment state is the fold since the last head, f = a head was seen
+template <class C>
+__device__ __forceinline__ void seg_after(typename C::S& a, u32& f, const typename C::S& pa, u32 pf) {
+  if (!f) { typename C::S t = pa; C::merge(t, a); a = t; }
+  f |= pf;
+}
+
+// Segmented scan over the CTA's threads in thread order (NW warps).  In: the thread's own (a, f).  Out: (a, f) =
+// the exclusive prefix of the threads before it, and (ta, tf) = the CTA's total.  s_a / s_f: NW + 1 slots.
+template <class C, int NW>
+__device__ __forceinline__ void block_seg_scan(typename C::S& a, u32& f, typename C::S* s_a, u32* s_f,
+                                               typename C::S& ta, u32& tf) {
+  typedef typename C::S S;
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const S o = C::shfl_up(a, d);
+    const u32 of = __shfl_up_sync(0xffffffffu, f, d);
+    if (lane >= d) seg_after<C>(a, f, o, of);
+  }
+  if (lane == 31) { s_a[w] = a; s_f[w] = f; }
+  S e = C::shfl_up(a, 1);
+  u32 ef = __shfl_up_sync(0xffffffffu, f, 1);
+  if (lane == 0) { C::init(e); ef = 0; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    S run; C::init(run); u32 rf = 0;
+    for (int i = 0; i < NW; i++) {
+      S x = s_a[i]; u32 xf = s_f[i];
+      s_a[i] = run; s_f[i] = rf;
+      seg_after<C>(x, xf, run, rf);
+      run = x; rf = xf;
+    }
+    s_a[NW] = run; s_f[NW] = rf;
+  }
+  __syncthreads();
+  seg_after<C>(e, ef, s_a[w], s_f[w]);
+  a = e; f = ef;
+  ta = s_a[NW]; tf = s_f[NW];
+}
+
+// The tile's head bits of this thread's RIPT positions; bit 0 of thread 0 is set when a group starts at the tile's
+// first position (tile_heads leaves that one out).
+template <bool REV>
+__device__ __forceinline__ u32 cum_heads(const int32_t* __restrict__ offsets, int64_t ng, int64_t n, int64_t t0,
+                                         int64_t t1, int64_t* s_g, u32* s_bits) {
+  const int tid = threadIdx.x;
+  if (tid < RTILE / 32) s_bits[tid] = 0;
+  int64_t g_lo, g_hi;
+  tile_heads<REV>(offsets, ng, n, t0, t1, tid, s_g, s_bits, g_lo, g_hi);
+  const int c0 = tid * RIPT;
+  u32 bits = (s_bits[c0 >> 5] >> (c0 & 31)) & 0xffu;
+  if (tid == 0 && head_offset<REV>(offsets, ng, n, g_lo) == t0) bits |= 1u;
+  return bits;
+}
+
+template <int K, typename T, bool REV, typename OrdT>
+__global__ void __launch_bounds__(RT, 1)
+cum_tile_kernel(const typename RawKey<T>::load_t* __restrict__ v, int64_t nv, const OrdT* __restrict__ order,
+                const int32_t* __restrict__ offsets, int64_t ng, int64_t n, typename Cum<K, T>::O* __restrict__ out,
+                typename Cum<K, T>::S* __restrict__ tagg, u32* __restrict__ thead)
+{
+  typedef Cum<K, T> C;
+  typedef typename C::S S;
+  typedef typename RawKey<T>::load_t L;
+  __shared__ int64_t s_g[2];
+  __shared__ u32 s_bits[RTILE / 32];
+  __shared__ S s_a[RT / 32 + 1];
+  __shared__ u32 s_f[RT / 32 + 1];
+  const int64_t t0 = (int64_t)blockIdx.x * RTILE;
+  const int64_t t1 = (t0 + RTILE < n) ? t0 + RTILE : n;
+  const u32 bits = cum_heads<REV>(offsets, ng, n, t0, t1, s_g, s_bits);
+
+  // gather: all index loads first, then all value loads
+  const int64_t q0 = t0 + threadIdx.x * RIPT, p0 = REV ? n - 1 - q0 : q0;   // position q is p0 -+ (q - q0)
+  int64_t row[RIPT];
+#pragma unroll
+  for (int i = 0; i < RIPT; i++) {
+    const int64_t p = REV ? p0 - i : p0 + i;
+    row[i] = (q0 + i < n) ? (order ? (int64_t)order[p] : p) : -2;
+  }
+  L val[RIPT];
+#pragma unroll
+  for (int i = 0; i < RIPT; i++) val[i] = (row[i] >= 0 && row[i] < nv) ? v[row[i]] : (L)0;
+
+  S a; C::init(a);
+  u32 f = 0;
+#pragma unroll
+  for (int i = 0; i < RIPT; i++) {
+    if (q0 + i < n) {
+      const typename C::O c = C::contrib(val[i], row[i] >= 0 && row[i] < nv);
+      out[REV ? p0 - i : p0 + i] = c;
+      if (bits & (1u << i)) { C::init(a); f = 1; }
+      C::add(a, c);
+    }
+  }
+  S ta; u32 tf;
+  block_seg_scan<C, RT / 32>(a, f, s_a, s_f, ta, tf);
+  if (threadIdx.x == 0) { tagg[blockIdx.x] = ta; thead[blockIdx.x] = tf; }
+}
+
+// tagg[t] <- the state of the group open at tile t's first position, before it (the carry-in); one CTA of CARRY_T
+// threads, each over a run of consecutive tiles
+constexpr int CARRY_T = 1024;
+
+template <int K, typename T>
+__global__ void __launch_bounds__(CARRY_T)
+cum_carry_kernel(typename Cum<K, T>::S* __restrict__ tagg, const u32* __restrict__ thead, int64_t ntiles)
+{
+  typedef Cum<K, T> C;
+  typedef typename C::S S;
+  __shared__ S s_a[CARRY_T / 32 + 1];
+  __shared__ u32 s_f[CARRY_T / 32 + 1];
+  const int64_t per = (ntiles + CARRY_T - 1) / CARRY_T;
+  const int64_t b = (int64_t)threadIdx.x * per, e = (b + per < ntiles) ? b + per : ntiles;
+  S a; C::init(a);
+  u32 f = 0;
+  for (int64_t t = b; t < e; t++) {
+    S x = tagg[t]; u32 xf = thead[t];
+    seg_after<C>(x, xf, a, f);
+    a = x; f = xf;
+  }
+  S ta; u32 tf;
+  block_seg_scan<C, CARRY_T / 32>(a, f, s_a, s_f, ta, tf);
+  for (int64_t t = b; t < e; t++) {
+    const S x = tagg[t];
+    const u32 xf = thead[t];
+    tagg[t] = a;
+    if (xf) a = x; else C::merge(a, x);
+  }
+}
+
+template <int K, typename T, bool REV>
+__global__ void __launch_bounds__(RT)
+cum_emit_kernel(const int32_t* __restrict__ offsets, int64_t ng, int64_t n, typename Cum<K, T>::O* __restrict__ out,
+                const typename Cum<K, T>::S* __restrict__ tcarry)
+{
+  typedef Cum<K, T> C;
+  typedef typename C::S S;
+  typedef typename C::O O;
+  __shared__ int64_t s_g[2];
+  __shared__ u32 s_bits[RTILE / 32];
+  __shared__ S s_a[RT / 32 + 1];
+  __shared__ u32 s_f[RT / 32 + 1];
+  const int64_t t0 = (int64_t)blockIdx.x * RTILE;
+  const int64_t t1 = (t0 + RTILE < n) ? t0 + RTILE : n;
+  const u32 bits = cum_heads<REV>(offsets, ng, n, t0, t1, s_g, s_bits);
+
+  const int64_t q0 = t0 + threadIdx.x * RIPT, p0 = REV ? n - 1 - q0 : q0;
+  O c[RIPT];
+#pragma unroll
+  for (int i = 0; i < RIPT; i++) c[i] = (q0 + i < n) ? out[REV ? p0 - i : p0 + i] : (O)0;
+  S a; C::init(a);
+  u32 f = 0;
+#pragma unroll
+  for (int i = 0; i < RIPT; i++) {
+    if (q0 + i < n) {
+      if (bits & (1u << i)) { C::init(a); f = 1; }
+      C::add(a, c[i]);
+    }
+  }
+  S ta; u32 tf;
+  block_seg_scan<C, RT / 32>(a, f, s_a, s_f, ta, tf);
+  seg_after<C>(a, f, tcarry[blockIdx.x], 0);              // the running state before this thread's first position
+#pragma unroll
+  for (int i = 0; i < RIPT; i++) {
+    if (q0 + i < n) {
+      if (bits & (1u << i)) C::init(a);
+      C::add(a, c[i]);
+      out[REV ? p0 - i : p0 + i] = C::result(a);
+    }
+  }
+}
+
+int cumulative_out_stype(int op, int st) {
+  const bool isint = (st == DTB_STYPE_BOOL || st == DTB_STYPE_INT8 || st == DTB_STYPE_INT16 ||
+                      st == DTB_STYPE_INT32 || st == DTB_STYPE_INT64);
+  const bool isflt = (st == DTB_STYPE_FLOAT32 || st == DTB_STYPE_FLOAT64);
+  switch (op) {
+    case DTB_OP_SUM: case DTB_OP_PROD:                        // fexpr_cumsumprod.cc: evaluate1
+      return isint ? DTB_STYPE_INT64 : (isflt ? st : 0);
+    case DTB_OP_MIN: case DTB_OP_MAX:                         // fexpr_cumminmax.cc: the column's own stype
+      return (isint || isflt || st == DTB_STYPE_DATE32 || st == DTB_STYPE_TIME64) ? st : 0;
+  }
+  return 0;
+}
+
+// tagg: the largest scan state (Partial<CAT_PRODF>) per tile, then the tiles' head flags
+size_t cumulative_scratch_bytes(int64_t n) {
+  const size_t ntiles = (size_t)((n + RTILE - 1) / RTILE);
+  return ntiles * (sizeof(Partial<CAT_PRODF>) + sizeof(u32));
+}
+
+template <int K, typename T, bool REV>
+static int run_cumulative(const void* v, int64_t nv, const void* order, int order_is64, const int32_t* offsets,
+                          int64_t ng, int64_t n, void* scratch, void* out, cudaStream_t s)
+{
+  typedef Cum<K, T> C;
+  typedef typename RawKey<T>::load_t L;
+  const int64_t ntiles = (n + RTILE - 1) / RTILE;
+  typename C::S* tagg = (typename C::S*)scratch;
+  u32* thead = (u32*)((char*)scratch + (size_t)ntiles * sizeof(Partial<CAT_PRODF>));
+  typename C::O* o = (typename C::O*)out;
+  if (order_is64)
+    cum_tile_kernel<K, T, REV, int64_t><<<(unsigned)ntiles, RT, 0, s>>>((const L*)v, nv, (const int64_t*)order,
+                                                                         offsets, ng, n, o, tagg, thead);
+  else
+    cum_tile_kernel<K, T, REV, int32_t><<<(unsigned)ntiles, RT, 0, s>>>((const L*)v, nv, (const int32_t*)order,
+                                                                         offsets, ng, n, o, tagg, thead);
+  cum_carry_kernel<K, T><<<1, CARRY_T, 0, s>>>(tagg, thead, ntiles);
+  cum_emit_kernel<K, T, REV><<<(unsigned)ntiles, RT, 0, s>>>(offsets, ng, n, o, tagg);
+  count_launch(3);
+  DTB_CUDA_CHECK(cudaGetLastError());
+  return DTB_OK;
+}
+
+template <int K, typename T>
+static int run_cumulative_dir(int reverse, const void* v, int64_t nv, const void* order, int order_is64,
+                              const int32_t* offsets, int64_t ng, int64_t n, void* scratch, void* out, cudaStream_t s)
+{
+  return reverse ? run_cumulative<K, T, true>(v, nv, order, order_is64, offsets, ng, n, scratch, out, s)
+                 : run_cumulative<K, T, false>(v, nv, order, order_is64, offsets, ng, n, scratch, out, s);
+}
+
+// out: n elements of cumulative_out_stype(op, stype), out[p] for RowIndex position p; scratch:
+// cumulative_scratch_bytes(n) of device memory.  The stype is checked by the caller.
+int launch_cumulative(int op, int reverse, const void* v, int stype, int64_t nv, const void* order, int order_is64,
+                      const int32_t* offsets, int64_t ng, int64_t n, void* scratch, void* out, cudaStream_t s)
+{
+  if (n <= 0) return DTB_OK;
+#define DTB_CUM_ARGS reverse, v, nv, order, order_is64, offsets, ng, n, scratch, out, s
+#define DTB_CUM_INT(T) \
+  switch (op) {                                                                                    \
+    case DTB_OP_SUM:  return run_cumulative_dir<CUM_SUMI, T>(DTB_CUM_ARGS);                        \
+    case DTB_OP_PROD: return run_cumulative_dir<CUM_PRODI, T>(DTB_CUM_ARGS);                       \
+    case DTB_OP_MIN:  return run_cumulative_dir<CUM_MIN, T>(DTB_CUM_ARGS);                         \
+    case DTB_OP_MAX:  return run_cumulative_dir<CUM_MAX, T>(DTB_CUM_ARGS);                         \
+  } break;
+#define DTB_CUM_FLT(T) \
+  switch (op) {                                                                                    \
+    case DTB_OP_SUM:  return run_cumulative_dir<CUM_SUMF, T>(DTB_CUM_ARGS);                        \
+    case DTB_OP_PROD: return run_cumulative_dir<CUM_PRODF, T>(DTB_CUM_ARGS);                       \
+    case DTB_OP_MIN:  return run_cumulative_dir<CUM_MIN, T>(DTB_CUM_ARGS);                         \
+    case DTB_OP_MAX:  return run_cumulative_dir<CUM_MAX, T>(DTB_CUM_ARGS);                         \
+  } break;
+  switch (stype) {
+    case DTB_STYPE_BOOL: case DTB_STYPE_INT8: DTB_CUM_INT(int8_t)
+    case DTB_STYPE_INT16: DTB_CUM_INT(int16_t)
+    case DTB_STYPE_INT32: case DTB_STYPE_DATE32: DTB_CUM_INT(int32_t)
+    case DTB_STYPE_INT64: case DTB_STYPE_TIME64: DTB_CUM_INT(int64_t)
+    case DTB_STYPE_FLOAT32: DTB_CUM_FLT(float)
+    case DTB_STYPE_FLOAT64: DTB_CUM_FLT(double)
+  }
+#undef DTB_CUM_FLT
+#undef DTB_CUM_INT
+#undef DTB_CUM_ARGS
+  set_error("internal: cumulative function / stype combination"); return DTB_EINVAL;
 }
 
 // ===========================================================================

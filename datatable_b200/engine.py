@@ -15,7 +15,7 @@ import ctypes
 import numpy as np
 
 from . import _lib
-from ._lib import (BOOL, INT8, INT16, INT32, INT64, FLOAT32, FLOAT64, FLAG_DESCENDING,
+from ._lib import (BOOL, INT8, INT16, INT32, INT64, FLOAT32, FLOAT64, DATE32, TIME64, FLAG_DESCENDING,
                    FLAG_SORT_ONLY, NA_FIRST, NA_LAST, NA_REMOVE, check, dtb_col, lib)
 
 try:  # torch is plumbing only: device memory + streams
@@ -27,12 +27,12 @@ _NP2ST = {np.dtype(np.bool_): BOOL, np.dtype(np.int8): INT8, np.dtype(np.int16):
           np.dtype(np.int32): INT32, np.dtype(np.int64): INT64,
           np.dtype(np.float32): FLOAT32, np.dtype(np.float64): FLOAT64}
 _ST2NP = {BOOL: np.int8, INT8: np.int8, INT16: np.int16, INT32: np.int32, INT64: np.int64,
-          FLOAT32: np.float32, FLOAT64: np.float64}
+          FLOAT32: np.float32, FLOAT64: np.float64, DATE32: np.int32, TIME64: np.int64}
 
 
 def _torch_dtype(st):
-    return {BOOL: torch.int8, INT8: torch.int8, INT16: torch.int16, INT32: torch.int32,
-            INT64: torch.int64, FLOAT32: torch.float32, FLOAT64: torch.float64}[st]
+    return {BOOL: torch.int8, INT8: torch.int8, INT16: torch.int16, INT32: torch.int32, INT64: torch.int64,
+            FLOAT32: torch.float32, FLOAT64: torch.float64, DATE32: torch.int32, TIME64: torch.int64}[st]
 
 
 def is_tensor(x):
@@ -431,6 +431,33 @@ def qcut(value, order, offsets, nquantiles=10, stype=None):
     out, optr = _alloc(n, INT32, device)
     check(lib.dtb_qcut(v.c(), v.nrows, ctypes.c_void_p(o.ptr) if o is not None else None, ctypes.c_void_p(f.ptr),
                        ngroups, int(nquantiles), _stream(), ctypes.c_void_p(optr)))
+    return out
+
+
+def cumulative_out_stype(op, stype):
+    return lib.dtb_cumulative_out_stype(op, stype)
+
+
+def cumulative(op, value, order, offsets, reverse=False, stype=None):
+    """cumsum / cumprod / cummin / cummax (OP_SUM / OP_PROD / OP_MIN / OP_MAX) inside every group of (order, offsets),
+    as CumSumProd_ColumnImpl / CumMinMax_ColumnImpl under by() (dtb_cumulative); one group [0, n] without by().
+    `order`: None = identity, int32 or int64.  Returns one value per position of the RowIndex, of stype
+    cumulative_out_stype(op, stype); in HBM when the inputs are."""
+    v = Col(value, stype)
+    f = Col(offsets)
+    ngroups = f.nrows - 1
+    out_st = cumulative_out_stype(op, v.stype)
+    if not out_st:
+        raise _lib.DtbValueError(f"Invalid column of stype {v.stype} in cumulative function {op}")
+    o = None if order is None else Col(order)
+    if o is not None and o.stype not in (INT32, INT64):
+        raise _lib.DtbValueError("order must be int32 or int64")
+    n = (int(offsets[-1].item()) if is_tensor(offsets) else int(offsets[-1])) if ngroups > 0 else 0
+    device = v.on_device and f.on_device and (o is None or o.on_device)
+    out, optr = _alloc(n, out_st, device)
+    check(lib.dtb_cumulative(op, 1 if reverse else 0, v.c(), v.nrows, ctypes.c_void_p(o.ptr) if o is not None else None,
+                             1 if o is not None and o.stype == INT64 else 0, ctypes.c_void_p(f.ptr), ngroups, _stream(),
+                             ctypes.c_void_p(optr)))
     return out
 
 

@@ -297,6 +297,38 @@ DTB_API int dtb_groupby_reduce2(dtb_groupby* g, int op, dtb_col x, dtb_col y, in
                         dtb_stream stream, void* out);
 
 /*
+ * dtb_cumulative -- cumsum / cumprod / cummin / cummax inside every group: replaces CumSumProd_ColumnImpl
+ * (column/cumsumprod.h) and CumMinMax_ColumnImpl (column/cumminmax.h) as FExpr_CumSumProd / FExpr_CumMinMax run
+ * them (expr/fexpr_cumsumprod.cc, expr/fexpr_cumminmax.cc).  op: DTB_OP_SUM, DTB_OP_PROD, DTB_OP_MIN or DTB_OP_MAX.
+ * The value column is seen through `order` (NULL = identity; order_is64: int64 row ids) and cut by `offsets`
+ * (int32[ngroups+1], a Groupby, validated as dtb_reduce validates it; one group [0, n] for a call without by()).
+ * reverse != 0 scans every group from its last position to its first.  Host or device pointers.
+ *   out : offsets[ngroups] elements of stype dtb_cumulative_out_stype(op, value.stype), out[p] for position p of
+ *         the RowIndex (the GtoALL layout of the grouped frame): SUM / PROD give INT64 for bool and int8-64 and keep FLOAT32 /
+ *         FLOAT64; MIN / MAX keep the column's stype (bool, int8-64, float32/64, date32, time64).  0 = refused.
+ * Errors: another op, or a stype the op refuses, gives DTB_EINVAL; an stype without a fixed width DTB_ENOTIMPL.
+ *
+ * SUM / PROD: an NA row adds 0 or multiplies by 1, so no result is NA except a NaN the arithmetic makes (inf - inf,
+ * 0 * inf), which then stays for the rest of the group.  Integer results wrap modulo 2^64 and are bit-exact.
+ * MIN / MAX: an NA row repeats the previous result, which is NA until the group's first valid row; the update is
+ * prev < val ? prev : val (> for MAX), so of equal values the later row wins (-0.0 and +0.0 are equal).  Bit-exact.
+ * Float SUM is accumulated in float64 in a fixed, unspecified order, starting at -0.0: the prefix of k rows is
+ * within gamma(k-1) * sum|x| of the exact prefix sum, gamma(k) = k*u / (1 - k*u), u = 2^-53, rounded once to the
+ * output stype.  Float PROD keeps the significand and the binary exponent apart, as dtb_reduce's PROD does: the
+ * prefix of k valid finite non-zero rows is the exact product times (1 + d), |d| <= gamma(k-1), rounded once; a zero
+ * and an infinity in the prefix give NA; a zero alone gives 0 and an infinity alone inf, signed by the parity of the
+ * negative rows.  Deviations from the reference, which sums and multiplies in order in the column's own type:
+ * float32 is accumulated in float64; a cancelling prefix sum can differ from the sequential one by the bound above,
+ * in relative terms without limit; where the reference's running sum or product overflows or underflows part-way
+ * although the exact prefix is in range, the engine returns the in-range value (so such a prefix that also holds a
+ * zero or an inf is not NA here).  Results are deterministic: two calls on the same input give the same bytes.
+ * Up to INT32_MAX positions.
+ */
+DTB_API int dtb_cumulative_out_stype(int op, int stype);
+DTB_API int dtb_cumulative(int op, int reverse, dtb_col value, int64_t nrows_value, const void* order,
+                           int order_is64, const void* offsets, int64_t ngroups, dtb_stream stream, void* out);
+
+/*
  * dtb_gather -- replaces materialisation of ArrayView_ColumnImpl<int32/int64>
  * (column/view.cc:88-155): out[i] = order[i] < 0 ? NA : src[order[i]].
  */
