@@ -425,7 +425,11 @@ struct RoundPlan {
   bool     has_by;            // holds a by-column: its group boundaries count
   int      key_bytes;         // 4 or 8: the width of its composite keys
   PassPlan pp;
-  int      narrow_after;      // the pass that writes its 64-bit keys as their upper 32 bits, -1: none
+  int      narrow_after;      // 64-bit keys: the passes are planned so that this pass leaves 32 key bits, -1: none
+  int      kin_bytes[MAX_PASSES];   // width of the keys pass p reads (pass 0: of the composite)
+  int      kout_bytes[MAX_PASSES];  // width of the keys pass p writes, 0: none
+  int      kdrop[MAX_PASSES];       // low key bits the keys pass p reads no longer hold (consumed earlier)
+  int      low_bits;          // count-table last pass: the low key bits it recovers from the rows' slots, 0: none
   bool     fold;              // the first pass takes its histogram from the statistics kernel
   bool     want_sorted_keys;  // the last pass writes the sorted keys (the offsets and the group keys read them)
   bool     keep_composite;    // the composite keys go to a buffer that the bucketed reducers read again
@@ -598,8 +602,8 @@ static void plan_group(const dtb_col* keys, int nkeys, const int* flags, int na_
     plan_passes(r.kp.total_bits, width, r.pp);
     r.want_sorted_keys = ri == nrounds - 1 && gp.groups_k && r.has_by && !gp.count_table;
     // 64-bit keys whose sorted values are not needed afterwards: the passes over the low T-32 bits run
-    // on 64-bit keys, the last of them writes only the upper 32 bits, and the remaining passes run on
-    // 32-bit keys (8 instead of 12 bytes per row and pass in flight).  Never more passes than before.
+    // on 64-bit keys, the last of them leaves 32 bits, and the remaining passes run on 32-bit keys (8 instead
+    // of 12 bytes per row and pass in flight).  Never more passes than before.
     r.narrow_after = -1;
     if (r.key_bytes == 8 && !r.want_sorted_keys && !gp.count_table && width == 8 && r.kp.total_bits > 32) {
       PassPlan lo, hi;
@@ -608,9 +612,29 @@ static void plan_group(const dtb_col* keys, int nkeys, const int* flags, int na_
       if (lo.npasses + hi.npasses <= r.pp.npasses) {
         r.pp.npasses = lo.npasses + hi.npasses;
         for (int p = 0; p < lo.npasses; p++) { r.pp.shift[p] = lo.shift[p]; r.pp.bits[p] = lo.bits[p]; }
-        for (int p = 0; p < hi.npasses; p++) { r.pp.shift[lo.npasses + p] = hi.shift[p]; r.pp.bits[lo.npasses + p] = hi.bits[p]; }
+        for (int p = 0; p < hi.npasses; p++) {
+          r.pp.shift[lo.npasses + p] = r.kp.total_bits - 32 + hi.shift[p]; r.pp.bits[lo.npasses + p] = hi.bits[p];
+        }
         r.narrow_after = lo.npasses - 1;
       }
+    }
+    // Every pass but the last writes only the key bits later passes read (key >> (shift + bits)), in the narrowest
+    // of 1 / 2 / 4 / 8 bytes, and the next pass takes its digit from bit 0: C2's 20-bit keys move 2 + 1 instead of
+    // 4 + 4 bytes per row.  Not when the last pass writes the sorted keys.  The last pass of a count table needs the
+    // whole group key: it recovers the low bits the earlier passes consumed from the rows' slots, which takes one
+    // level of slot regions (at most 3 passes) and a table of 2^low_bits bases (at most 16 bits); beyond that the
+    // keys keep their full width.
+    const int np = r.pp.npasses;
+    const int low = gp.count_table && np > 1 ? r.pp.shift[np - 1] : 0;
+    const bool narrow = !r.want_sorted_keys && !(gp.count_table && (np > 3 || low > 16));
+    r.low_bits = narrow ? low : 0;
+    for (int p = 0; p < np; p++) {
+      const bool lastp = p == np - 1;
+      const int left = r.kp.total_bits - r.pp.shift[p] - r.pp.bits[p];      // key bits the later passes read
+      r.kdrop[p] = narrow && p > 0 ? r.pp.shift[p] : 0;
+      r.kin_bytes[p] = p == 0 ? r.key_bytes : r.kout_bytes[p - 1];
+      r.kout_bytes[p] = lastp ? (r.want_sorted_keys ? r.key_bytes : 0)
+                      : !narrow ? r.key_bytes : left <= 8 ? 1 : left <= 16 ? 2 : left <= 32 ? 4 : 8;
     }
     // single key column: the first pass takes its histogram from the statistics kernel (see stage_inputs)
     r.fold = nkeys == 1 && ri == 0 && gp.fused_raw && r.kp.k[0].cshift == 0 && r.kp.k[0].lshift == 0;
@@ -630,9 +654,13 @@ static void print_plan(const GroupPlan& gp, int64_t n, int nkeys, const ColStats
             (unsigned long long)st[c].nacount);
   for (int ri = 0; ri < nrounds; ri++) {
     const RoundPlan& r = gp.rounds[ri];
-    fprintf(stderr, "[dtb200]   round %d: keys=%d bits=%d group_shift=%d passes=%d narrow_after=%d fold=%d count_table=%d\n",
+    std::string kw;                                    // key bytes read:written by every pass
+    for (int p = 0; p < r.pp.npasses; p++)
+      kw += (p ? "," : "") + std::to_string(r.kin_bytes[p]) + ":" + std::to_string(r.kout_bytes[p]);
+    fprintf(stderr, "[dtb200]   round %d: keys=%d bits=%d group_shift=%d passes=%d narrow_after=%d fold=%d count_table=%d"
+            " key_bytes=%s low_bits=%d\n",
             ri, r.kp.nkeys, r.kp.total_bits, r.kp.group_shift, r.pp.npasses, r.narrow_after, (int)r.fold,
-            (int)(gp.count_table && ri == nrounds - 1));
+            (int)(gp.count_table && ri == nrounds - 1), kw.c_str(), r.low_bits);
   }
 }
 
@@ -668,6 +696,16 @@ static int sort_rounds(const GroupPlan& gp, int64_t n, int nfused, int32_t* orde
     // per-pass scratch: chunk x digit counts + digit totals/bases
     DevBuf work; DTB_TRY(work.alloc(radix_pass_work_bytes(n), s));
 
+    // the last pass of a count table recovers the consumed low key bits from the rows' slots: their bases are the
+    // first pass's digit bases (2 passes) or the scan of the rows per (second digit, first digit) (3 passes)
+    DevBuf lowbuf;
+    u32* low_base = nullptr; u32* regions = nullptr;
+    if (r.low_bits) {
+      DTB_TRY(lowbuf.alloc(sizeof(u32) * ((size_t)1 << 16) + sizeof(u32) * 256, s));
+      low_base = lowbuf.as<u32>(); regions = low_base + ((size_t)1 << 16);
+      if (pp.npasses == 3) DTB_CUDA_CHECK(cudaMemsetAsync(low_base, 0, sizeof(u32) * ((size_t)1 << r.low_bits), s));
+    }
+
     int32_t* round_out = ri == nrounds - 1 ? order : ((ri & 1) ? b.idxR1.as<int32_t>() : b.idxR0.as<int32_t>());
     void* kin = r.keep_composite ? b.bxk.p : b.keyA.p; void* kout = b.keyB.p;
     const int32_t* iin = idx_cur;
@@ -676,16 +714,21 @@ static int sort_rounds(const GroupPlan& gp, int64_t n, int nfused, int32_t* orde
       PassIO io;
       io.src_kind = (p == 0) ? src_kind : 0;
       io.keys_in = kin;
-      io.narrow_out = (p == r.narrow_after) ? (rk.total_bits - 32) : 0;
+      io.out_shift = last ? 0 : r.kdrop[p + 1] - r.kdrop[p];
+      io.out_bytes = r.kout_bytes[p];
       if (r.fold && p == 0 && pp.shift[0] == 0) {
         io.raw_hist = b.rawhist.as<unsigned short>(); io.raw_na = b.rawna.as<unsigned short>();
       }
-      const int kb = (r.narrow_after >= 0 && p > r.narrow_after) ? 4 : r.key_bytes;   // key width this pass reads
+      if (r.low_bits) {
+        if (p == 0) io.bases_out = pp.npasses == 2 ? low_base : regions;
+        if (p == 1 && !last) { io.regions = regions; io.region_bits = pp.bits[0]; io.low_hist = low_base; }
+        if (last) { io.low_base = low_base; io.low_bits = r.low_bits; }
+      }
       io.idx_in = iin;
       io.keys_out = (last && !r.want_sorted_keys) ? nullptr : kout;
       int32_t* iout = last ? round_out : ((p & 1) ? b.idxB.as<int32_t>() : b.idxA.as<int32_t>());
       io.idx_out = iout;
-      DTB_TRY(launch_radix_pass(io, rk, kb, n, pp.shift[p], pp.bits[p], work.as<u32>(), s,
+      DTB_TRY(launch_radix_pass(io, rk, r.kin_bytes[p], n, pp.shift[p] - r.kdrop[p], pp.bits[p], work.as<u32>(), s,
                                 (gp.count_table && last) ? b.gcount.as<u32>() : nullptr, rk.group_shift));
       if (last && r.want_sorted_keys) b.sorted_keys = kout;
       kin = kout;

@@ -96,13 +96,16 @@ __device__ __forceinline__ u64 norm_load_dynamic(const KeyNorm& k, int64_t i) {
 // load_raw / norm are split so that a kernel can issue all the loads of a tile before it touches any of
 // them (with load() alone ptxas reused one register for the raw element and serialised the 16 loads of
 // the scatter pass behind one another).
-template <typename KeyT>
+// Packed keys of InT (1, 2, 4 or 8 bytes: the radix passes store only the key bits later passes read, in the
+// narrowest word that holds them), widened to the pass's KeyT.
+template <typename InT, typename KeyT = InT>
 struct PackedSrc {
-  typedef KeyT raw_t;
-  const KeyT* p;
-  __device__ __forceinline__ KeyT load(int64_t i) const { return p[i]; }
+  typedef InT raw_t;
+  static constexpr bool packed = true;
+  const InT* p;
+  __device__ __forceinline__ KeyT load(int64_t i) const { return (KeyT)p[i]; }
   __device__ __forceinline__ raw_t load_raw(int64_t i) const { return p[i]; }
-  __device__ __forceinline__ KeyT norm(raw_t r) const { return r; }
+  __device__ __forceinline__ KeyT norm(raw_t r) const { return (KeyT)r; }
   __host__ KeyNorm key_norm() const { KeyNorm z; memset(&z, 0, sizeof(z)); return z; }   // packed keys carry no normalisation
 };
 
@@ -135,6 +138,7 @@ struct RawSrc {
     edge32 = (u32)kn.edge; na32 = (u32)kn.na_value; inc32 = (u32)kn.inc;
   }
   typedef typename RawKey<T>::load_t raw_t;
+  static constexpr bool packed = false;
   __host__ const KeyNorm& key_norm() const { return k; }
   __device__ __forceinline__ raw_t load_raw(int64_t i) const { return p[i]; }
   __device__ __forceinline__ KeyT norm(raw_t r) const {

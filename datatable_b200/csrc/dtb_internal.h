@@ -114,13 +114,28 @@ struct PassIO {
   // into its digit counts and does not run its count kernel
   const unsigned short* raw_hist = nullptr;
   const unsigned short* raw_na = nullptr;
-  int         narrow_out = 0;     // 64-bit keys, > 0: keys_out receives (key >> narrow_out) as uint32 (later passes run on 32-bit keys)
+  // keys_out receives (key >> out_shift) in words of out_bytes (1, 2, 4 or 8): only the bits later passes read
+  int         out_shift = 0;
+  int         out_bytes = 0;
+  // Recovering the low bits of the keys in the last pass of a count-table round (the passes before it dropped them;
+  // a row's consumed low bits v follow from its slot, the rows of v sit in slots [low_base[v], low_base[v+1])):
+  //   bases_out   : receives the pass's 256 digit bases (the 2-pass low_base, or the next pass's regions)
+  //   regions     : the previous pass's digit bases; the count kernel adds every row to low_hist[digit << region_bits
+  //                 | region of its slot], and the pass turns low_hist into its exclusive scan (the 3-pass low_base)
+  //   low_base    : last pass: key = (keys_in << low_bits) | v, v found from the row's slot
+  uint32_t*       bases_out = nullptr;
+  const uint32_t* regions = nullptr;
+  int             region_bits = 0;
+  uint32_t*       low_hist = nullptr;
+  const uint32_t* low_base = nullptr;
+  int             low_bits = 0;
 };
 
 // One stable pass = count + scan + scatter kernels.  work: radix_pass_work_bytes(n) of scratch.
 size_t radix_pass_work_bytes(int64_t n);
 // group_count (optional, last pass only): uint32 table indexed by (key >> group_shift), zeroed by the
 // caller; receives the number of rows of every group key (see launch_offsets_from_counts).
+// key_bytes: width of the packed keys_in words (1, 2, 4 or 8), or of the composite for a raw column (4 or 8).
 int launch_radix_pass(const PassIO& io, const KeyPlan& kp, int key_bytes, int64_t n,
                       int shift, int bits, uint32_t* work, cudaStream_t s,
                       uint32_t* group_count = nullptr, int group_shift = 0);

@@ -25,7 +25,8 @@
 // scatter): no separate `x` array is materialised for single-column keys.
 //
 // Bound: HBM.  Algorithmic bytes per row per pass = read (key + idx) + write (key + idx);
-// first pass reads the raw column only, last pass of a sort-only call writes idx only.
+// first pass reads the raw column only, last pass of a sort-only call writes idx only.  The keys between passes
+// hold only the bits later passes read, in 1 / 2 / 4 / 8 bytes (PassIO::out_shift / out_bytes, DESIGN 4.1).
 #include "dtb_common.cuh"
 
 namespace dtb {
@@ -109,24 +110,42 @@ int64_t radix_num_chunks(int64_t n) { return (n + CHUNK_ROWS - 1) / CHUNK_ROWS; 
 // ===========================================================================
 // count: tile_pre[tile][digit] (u16, rows of the digit in the earlier tiles of the chunk) and counts[chunk][digit]
 // ===========================================================================
+// The v in [lo, hi] whose rows occupy slot s: the last v with b[v] <= s (b = exclusive scan of the rows per v, so
+// b[lo] <= s; an empty v shares its b with the next one and is never the last).
+__device__ __forceinline__ u32 slot_owner(const u32* b, u32 lo, u32 hi, u32 s) {
+  while (lo < hi) { const u32 mid = (lo + hi + 1) >> 1; if (b[mid] <= s) lo = mid; else hi = mid - 1; }
+  return lo;
+}
+
+// regions (optional): the previous pass's digit bases.  A slot's region is the previous pass's digit of its row,
+// so low_hist[digit << region_bits | region] counts the rows by the low bits both passes consume.  A tile inside one
+// region adds its digit counts (summed over the chunk's consecutive tiles of that region); only the few tiles that
+// straddle a region boundary count row by row.
 template <typename KeyT, typename Src, int NBINS>
 __global__ void __launch_bounds__(PASS_THREADS)
 count_kernel(const __grid_constant__ Src src, int64_t n, int shift, u32 mask, u32* __restrict__ counts,
-             unsigned short* __restrict__ tile_pre)
+             unsigned short* __restrict__ tile_pre, const u32* __restrict__ regions, int region_bits,
+             u32* __restrict__ low_hist)
 {
   constexpr int BPT = NBINS / PASS_THREADS;
   __shared__ u32 h[NBINS];
+  __shared__ u32 rg[256];
   const int64_t cbase = (int64_t)blockIdx.x * CHUNK_ROWS;
   const int64_t cend = (cbase + CHUNK_ROWS < n) ? cbase + CHUNK_ROWS : n;
+  const u32 rmax = (1u << region_bits) - 1;
+  if (regions) { if (threadIdx.x <= rmax) rg[threadIdx.x] = regions[threadIdx.x]; }
   u32 total[BPT];                                          // rows of digit tid + j*THREADS in this chunk
+  u32 racc[BPT], rcur = ~0u;                               // rows of the digit in the current run of one-region tiles
 #pragma unroll
-  for (int j = 0; j < BPT; j++) total[j] = 0;
+  for (int j = 0; j < BPT; j++) { total[j] = 0; racc[j] = 0; }
   for (int64_t base = cbase; base < cend; base += PASS_TILE) {
 #pragma unroll
     for (int j = 0; j < BPT; j++) h[threadIdx.x + j * PASS_THREADS] = 0;
     __syncthreads();
     const int64_t end = (base + PASS_TILE < cend) ? base + PASS_TILE : cend;
-    if (end - base == PASS_TILE) {
+    u32 r0 = 0, r1 = 0;
+    if (regions) { r0 = slot_owner(rg, 0, rmax, (u32)base); r1 = slot_owner(rg, r0, rmax, (u32)(end - 1)); }
+    if (end - base == PASS_TILE && r0 == r1) {
       // coalesced: consecutive threads read consecutive rows; 16 independent loads in flight per thread
       KeyT k[PASS_IPT];
 #pragma unroll
@@ -134,11 +153,14 @@ count_kernel(const __grid_constant__ Src src, int64_t n, int shift, u32 mask, u3
 #pragma unroll
       for (int j = 0; j < PASS_IPT; j++) atomicAdd(&h[(u32)(k[j] >> shift) & mask], 1u);
     } else {
-      // the column's last, partial tile only: unrolling it costs registers in the whole kernel
+      // the column's last, partial tile and the tiles that straddle a region boundary: unrolling it costs
+      // registers in the whole kernel
 #pragma unroll 1
       for (int64_t i = base + threadIdx.x; i < end; i += PASS_THREADS) {
         const KeyT kk = src.load(i);
-        atomicAdd(&h[(u32)(kk >> shift) & mask], 1u);
+        const u32 d = (u32)(kk >> shift) & mask;
+        atomicAdd(&h[d], 1u);
+        if (r0 != r1) atomicAdd(&low_hist[(d << region_bits) | slot_owner(rg, r0, r1, (u32)i)], 1u);
       }
     }
     __syncthreads();
@@ -149,10 +171,19 @@ count_kernel(const __grid_constant__ Src src, int64_t n, int shift, u32 mask, u3
       // kernel adds it to the digit base and the chunk offset without walking the chunk's tiles
       tile_pre[(size_t)(base / PASS_TILE) * NBINS + threadIdx.x + j * PASS_THREADS] = (unsigned short)total[j];
       total[j] += c;
+      if (regions && r0 == r1) {
+        const u32 d = threadIdx.x + j * PASS_THREADS;
+        if (r0 != rcur && racc[j]) { atomicAdd(&low_hist[(d << region_bits) | rcur], racc[j]); racc[j] = 0; }
+        racc[j] += c;
+      }
     }
+    if (regions && r0 == r1) rcur = r0;
   }
 #pragma unroll
-  for (int j = 0; j < BPT; j++) counts[(size_t)blockIdx.x * NBINS + threadIdx.x + j * PASS_THREADS] = total[j];
+  for (int j = 0; j < BPT; j++) {
+    counts[(size_t)blockIdx.x * NBINS + threadIdx.x + j * PASS_THREADS] = total[j];
+    if (racc[j]) atomicAdd(&low_hist[((threadIdx.x + j * PASS_THREADS) << region_bits) | rcur], racc[j]);
+  }
 }
 
 // First pass over a raw column, counts from the statistics kernel's histogram of the low 8 bits of u
@@ -246,6 +277,38 @@ digit_base_kernel(const u32* __restrict__ total, u32* __restrict__ base)
   for (int j = 0; j < BPT; j++) { base[t * BPT + j] = e; e += v[j]; }
 }
 
+// In place: a[0..len) becomes its exclusive scan (len <= 2^16, the rows per consumed low-bit value).  One CTA, every
+// thread owns len / 1024 consecutive entries.
+__global__ void __launch_bounds__(1024)
+low_scan_kernel(u32* __restrict__ a, int len)
+{
+  __shared__ u32 wsum[32];
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int per = (len + 1023) / 1024, b0 = t * per;
+  u32 tsum = 0;
+  for (int j = 0; j < per; j++) if (b0 + j < len) tsum += a[b0 + j];
+  u32 incl = tsum;
+#pragma unroll
+  for (int k = 1; k < 32; k <<= 1) { const u32 o = __shfl_up_sync(0xffffffffu, incl, k); if (lane >= k) incl += o; }
+  if (lane == 31) wsum[warp] = incl;
+  __syncthreads();
+  u32 wpre = 0;
+  for (int w = 0; w < warp; w++) wpre += wsum[w];
+  u32 e = wpre + incl - tsum;
+  for (int j = 0; j < per; j++) if (b0 + j < len) { const u32 c = a[b0 + j]; a[b0 + j] = e; e += c; }
+}
+
+// The consumed low-bit values of every tile's first and last slot (equal for all but the tiles at a boundary).
+__global__ void __launch_bounds__(256)
+tile_low_kernel(const u32* __restrict__ low_base, u32 vmax, int64_t n, int64_t ntiles, uint2* __restrict__ tile_low)
+{
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= ntiles) return;
+  const int64_t first = t * PASS_TILE, last = (first + PASS_TILE < n ? first + PASS_TILE : n) - 1;
+  const u32 lo = slot_owner(low_base, 0, vmax, (u32)first);
+  tile_low[t] = make_uint2(lo, slot_owner(low_base, lo, vmax, (u32)last));
+}
+
 // ===========================================================================
 // scatter
 // ===========================================================================
@@ -263,7 +326,11 @@ struct PassArgs {
   const unsigned short* tile_pre;      // [ntiles][NBINS] rows of this digit in the earlier tiles of the chunk
   u32*           group_count;   // optional (last pass, small key domains): rows per group key
   int            group_shift;
-  int            narrow;        // 64-bit keys only, > 0: write (key >> narrow) as uint32 -- the low bits are consumed
+  int            out_shift;     // keys_out[dst] = key >> out_shift in words of out_bytes: the bits later passes read
+  int            out_bytes;
+  const u32*     low_base;      // 1-byte packed keys of a count-table last pass: key = (in << low_bits) | v(slot)
+  int            low_bits;
+  const uint2*   tile_low;      // [ntiles] v of the tile's first and last slot
 };
 
 // ---- TMA 1-D bulk copy (cp.async.bulk, SASS UBLKCP) completing on an mbarrier -----------------------
@@ -309,7 +376,7 @@ template <typename KeyT, int NBINS> struct PassCfg {
 template <typename KeyT, typename Src, int NBINS, bool FULL, int NB>
 __device__ __forceinline__ void scatter_tile(const PassArgs<KeyT, Src>& a, unsigned char* smem_raw, u32* s_wsum,
                                              uint64_t* s_bar, const int64_t base, const int tile_n,
-                                             const u32 (&bin_run)[NBINS / PASS_THREADS])
+                                             const u32 (&bin_run)[NBINS / PASS_THREADS], const uint2 tl)
 {
   constexpr int THREADS = PASS_THREADS, IPT = PASS_IPT, TILE = PASS_TILE;
   constexpr int WARPS = THREADS / 32;
@@ -355,6 +422,19 @@ __device__ __forceinline__ void scatter_tile(const PassArgs<KeyT, Src>& a, unsig
     for (int i = 0; i < IPT; i++) {                              // ... then normalised (identity for packed keys)
       const int lp = wbase + i * 32 + lane;
       key[i] = (FULL || lp < tile_n) ? a.src.norm(raw[i]) : (KeyT)0;
+    }
+    // a count-table last pass reads only the bits above those the earlier passes consumed: put them back from the
+    // row's slot (one value for the whole tile unless it straddles a boundary), so that the tile is staged with its
+    // full keys and the run heads below see the group keys
+    if constexpr (Src::packed && sizeof(typename Src::raw_t) == 1) {
+      if (a.low_base) {
+#pragma unroll
+        for (int i = 0; i < IPT; i++) {
+          const int lp = wbase + i * 32 + lane;
+          const u32 v = tl.x == tl.y ? tl.x : slot_owner(a.low_base, tl.x, tl.y, (u32)(base + lp));
+          key[i] = (key[i] << a.low_bits) | v;
+        }
+      }
     }
   }
   // first output slot of the thread's digits (loaded by the caller before the keys, parked here until
@@ -499,9 +579,11 @@ scatter_kernel(const __grid_constant__ PassArgs<KeyT, Src> a)
     const int b = tid * BPT + j;
     bin_run[j] = a.digit_base[b] + a.chunk_offs[(size_t)chunk * NBINS + b] + (u32)a.tile_pre[(size_t)tile * NBINS + b];
   }
+  uint2 tl = make_uint2(0, 0);
+  if constexpr (Src::packed && sizeof(typename Src::raw_t) == 1) { if (a.low_base) tl = a.tile_low[tile]; }
 
-  if (tile_n == TILE) scatter_tile<KeyT, Src, NBINS, true,  NB>(a, smem_raw, s_wsum, &s_bar, base, tile_n, bin_run);
-  else                scatter_tile<KeyT, Src, NBINS, false, NB>(a, smem_raw, s_wsum, &s_bar, base, tile_n, bin_run);
+  if (tile_n == TILE) scatter_tile<KeyT, Src, NBINS, true,  NB>(a, smem_raw, s_wsum, &s_bar, base, tile_n, bin_run, tl);
+  else                scatter_tile<KeyT, Src, NBINS, false, NB>(a, smem_raw, s_wsum, &s_bar, base, tile_n, bin_run, tl);
 
   // ---- coalesced scatter: consecutive threads write consecutive slots of a digit run ----
   const int lane = tid & 31;
@@ -542,10 +624,13 @@ scatter_kernel(const __grid_constant__ PassArgs<KeyT, Src> a)
       const u32 d = (u32)(k >> a.shift) & a.mask;
       const u32 dst = bin_dst[d] + (u32)p;
       if (a.keys_out) {
-        if constexpr (sizeof(KeyT) == 8) {
-          if (a.narrow) reinterpret_cast<u32*>(a.keys_out)[dst] = (u32)(k >> a.narrow);
-          else a.keys_out[dst] = k;
-        } else a.keys_out[dst] = k;
+        const KeyT ko = k >> a.out_shift;
+        switch (a.out_bytes) {
+          case 1:  reinterpret_cast<unsigned char*>(a.keys_out)[dst] = (unsigned char)ko; break;
+          case 2:  reinterpret_cast<unsigned short*>(a.keys_out)[dst] = (unsigned short)ko; break;
+          case 4:  reinterpret_cast<u32*>(a.keys_out)[dst] = (u32)ko; break;
+          default: a.keys_out[dst] = ko; break;
+        }
       }
       a.idx_out[dst] = rid;
     }
@@ -555,14 +640,15 @@ scatter_kernel(const __grid_constant__ PassArgs<KeyT, Src> a)
 template <typename KeyT, typename Src, int NBINS>
 static int run_scatter(Src src, const PassIO& io, int64_t n, int shift, u32 mask, int64_t ntiles,
                        const u32* counts, const u32* base, const unsigned short* tile_counts,
-                       u32* group_count, int group_shift, cudaStream_t s)
+                       u32* group_count, int group_shift, const uint2* tile_low, cudaStream_t s)
 {
   constexpr int MINB = PassCfg<KeyT, NBINS>::MINB;
   PassArgs<KeyT, Src> a;
   a.src = src; a.idx_in = io.idx_in; a.keys_out = (KeyT*)io.keys_out; a.idx_out = io.idx_out;
-  a.n = n; a.shift = shift; a.mask = mask; a.chunk_offs = counts; a.digit_base = base;
+  a.n = n; a.shift = shift + io.low_bits; a.mask = mask; a.chunk_offs = counts; a.digit_base = base;
   a.tile_pre = tile_counts; a.group_count = group_count; a.group_shift = group_shift;
-  a.narrow = io.narrow_out;
+  a.out_shift = io.out_shift; a.out_bytes = io.out_bytes ? io.out_bytes : (int)sizeof(KeyT);
+  a.low_base = io.low_base; a.low_bits = io.low_bits; a.tile_low = tile_low;
   constexpr size_t smem = PassCfg<KeyT, NBINS>::SMEM;
   // NB = ballots per row in the rank phase = digit width, rounded up to a built variant
   const int bits = __builtin_popcount(mask);
@@ -598,14 +684,26 @@ static int run_pass_nb(Src src, const PassIO& io, int64_t n, int shift, int bits
       fold_counts_kernel<<<(unsigned)nchunks, 256, 0, s>>>(io.raw_hist, io.raw_na, ntiles, (u32)k.edge & 255u, (u32)k.inc & 255u,
                                                          k.desc, (u32)k.na_value & mask, mask, counts, tile_counts);
     } else {
-      count_kernel<KeyT, Src, NBINS><<<(unsigned)nchunks, PASS_THREADS, 0, s>>>(src, n, shift, mask, counts, tile_counts);
+      count_kernel<KeyT, Src, NBINS><<<(unsigned)nchunks, PASS_THREADS, 0, s>>>(src, n, shift, mask, counts, tile_counts,
+                                                                                io.regions, io.region_bits, io.low_hist);
     }
   }
   chunk_scan_kernel<<<NBINS, 256, 0, s>>>(counts, nchunks, NBINS, total);
   digit_base_kernel<NBINS><<<1, 256, 0, s>>>(total, base);
   count_launch(3);
+  if (io.bases_out) DTB_CUDA_CHECK(cudaMemcpyAsync(io.bases_out, base, sizeof(u32) * NBINS, cudaMemcpyDeviceToDevice, s));
+  if (io.low_hist) {
+    low_scan_kernel<<<1, 1024, 0, s>>>(io.low_hist, 1 << (io.region_bits + bits));
+    count_launch();
+  }
+  uint2* tile_low = nullptr;
+  if (io.low_base) {
+    tile_low = reinterpret_cast<uint2*>(tile_counts + (size_t)(ntiles + CHUNK_TILES) * NBINS);
+    tile_low_kernel<<<(unsigned)((ntiles + 255) / 256), 256, 0, s>>>(io.low_base, (1u << io.low_bits) - 1, n, ntiles, tile_low);
+    count_launch();
+  }
   return run_scatter<KeyT, Src, NBINS>(src, io, n, shift, mask, ntiles, counts, base, tile_counts,
-                                       group_count, group_shift, s);
+                                       group_count, group_shift, tile_low, s);
 }
 
 template <typename KeyT, typename Src>
@@ -643,7 +741,7 @@ size_t radix_pass_work_bytes(int64_t n) {
   const size_t ntiles = (size_t)((n + PASS_TILE - 1) / PASS_TILE);
   const size_t nbins = 256;
   return sizeof(u32) * ((size_t)radix_num_chunks(n) * nbins + 2 * nbins)
-       + sizeof(unsigned short) * (ntiles + CHUNK_TILES) * nbins;
+       + sizeof(unsigned short) * (ntiles + CHUNK_TILES) * nbins + sizeof(uint2) * ntiles;
 }
 
 int launch_radix_pass(const PassIO& io, const KeyPlan& kp, int key_bytes, int64_t n,
@@ -651,11 +749,22 @@ int launch_radix_pass(const PassIO& io, const KeyPlan& kp, int key_bytes, int64_
                       uint32_t* group_count, int group_shift)
 {
   if (bits < 1 || bits > 8) { set_error("internal: digit width must be 1..8 bits"); return DTB_EINVAL; }
+  if ((io.low_base && (io.src_kind != 0 || key_bytes != 1 || io.low_bits < 1 || io.low_bits > 16)) ||
+      (io.regions && (io.raw_hist || !io.low_hist || io.region_bits < 1 || io.region_bits + bits > 16)) ||
+      io.out_bytes > (key_bytes == 8 ? 8 : 4)) {
+    set_error("internal: bad key widths for a radix pass"); return DTB_EINVAL;
+  }
   if (io.src_kind == 0) {
-    if (key_bytes == 4) { PackedSrc<u32> src{(const u32*)io.keys_in};
-      return run_pass<u32>(src, io, n, shift, bits, work, s, group_count, group_shift); }
-    else { PackedSrc<u64> src{(const u64*)io.keys_in};
-      return run_pass<u64>(src, io, n, shift, bits, work, s, group_count, group_shift); }
+    switch (key_bytes) {
+      case 1: { PackedSrc<unsigned char, u32> src{(const unsigned char*)io.keys_in};
+        return run_pass<u32>(src, io, n, shift, bits, work, s, group_count, group_shift); }
+      case 2: { PackedSrc<unsigned short, u32> src{(const unsigned short*)io.keys_in};
+        return run_pass<u32>(src, io, n, shift, bits, work, s, group_count, group_shift); }
+      case 4: { PackedSrc<u32> src{(const u32*)io.keys_in};
+        return run_pass<u32>(src, io, n, shift, bits, work, s, group_count, group_shift); }
+      default: { PackedSrc<u64> src{(const u64*)io.keys_in};
+        return run_pass<u64>(src, io, n, shift, bits, work, s, group_count, group_shift); }
+    }
   }
   return key_bytes == 4 ? run_pass_raw<u32>(io, kp, n, shift, bits, work, s, group_count, group_shift)
                         : run_pass_raw<u64>(io, kp, n, shift, bits, work, s, group_count, group_shift);
