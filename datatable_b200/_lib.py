@@ -18,6 +18,7 @@ NA_FIRST, NA_LAST, NA_REMOVE = 1, 2, 3
 OP_SUM, OP_MEAN, OP_MIN, OP_MAX, OP_COUNT, OP_COUNTNA, OP_NROWS = 1, 2, 3, 4, 5, 6, 7
 OP_FIRST, OP_LAST, OP_SD, OP_MEDIAN, OP_NUNIQUE = 8, 9, 10, 11, 12
 OP_PROD, OP_COV, OP_CORR = 13, 14, 15
+GROUP_CUMCOUNT, GROUP_NGROUP = 1, 2
 SET_UNION, SET_INTERSECT, SET_SETDIFF, SET_SYMDIFF = 0, 1, 2, 3
 OK, EINVAL, ENOTIMPL, ECUDA, ENOMEM, ENOSPACE = 0, -1, -2, -3, -4, -5
 
@@ -30,7 +31,8 @@ EXPORTS = [
     "dtb_gather", "dtb_memcpy", "dtb_set_option", "dtb_get_option", "dtb_last_call_stats",
     "dtb_profile_count", "dtb_profile_get", "dtb_profile_reset",
     "dtb_dense_scatter", "dtb_dense_compact",
-    "dtb_sort_grouped", "dtb_qcut", "dtb_cumulative_out_stype", "dtb_cumulative", "dtb_set_select", "dtb_largest_group", "dtb_join", "dtb_cache_begin", "dtb_cache_end", "dtb_lower_bound",
+    "dtb_sort_grouped", "dtb_qcut", "dtb_cumulative_out_stype", "dtb_cumulative", "dtb_shift", "dtb_fillna", "dtb_group_index",
+    "dtb_set_select", "dtb_largest_group", "dtb_join", "dtb_cache_begin", "dtb_cache_end", "dtb_lower_bound",
 ]
 
 
@@ -126,6 +128,11 @@ def _load():
     lib.dtb_cumulative_out_stype.argtypes = [c.c_int, c.c_int]
     lib.dtb_cumulative.argtypes = [c.c_int, c.c_int, dtb_col, c.c_int64, c.c_void_p, c.c_int, c.c_void_p, c.c_int64,
                                    c.c_void_p, c.c_void_p]
+    lib.dtb_shift.argtypes = [dtb_col, c.c_int64, c.c_void_p, c.c_int, c.c_void_p, c.c_int64, c.c_int64, c.c_void_p,
+                              c.c_void_p]
+    lib.dtb_fillna.argtypes = [c.c_int, dtb_col, c.c_int64, c.c_void_p, c.c_int, c.c_void_p, c.c_int64, c.c_void_p,
+                               c.c_void_p]
+    lib.dtb_group_index.argtypes = [c.c_int, c.c_int, c.c_void_p, c.c_int64, c.c_void_p, c.c_void_p]
     lib.dtb_set_select.argtypes = [c.c_int, c.c_void_p, c.c_void_p, c.c_int64, c.POINTER(c.c_int64), c.c_int,
                                    c.c_void_p, c.c_void_p, c.POINTER(c.c_int64)]
     lib.dtb_largest_group.argtypes = [c.c_void_p, c.c_int64, c.c_int64, c.c_void_p, c.POINTER(c.c_int64),

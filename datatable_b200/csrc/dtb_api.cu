@@ -1469,6 +1469,95 @@ int dtb_cumulative(int op, int reverse, dtb_col value, int64_t nrows_value, cons
   return DTB_OK;
 }
 
+// dtb_shift / dtb_fillna (fill: reverse; else shift): the argument checks and buffers of dtb_cumulative and an output
+// of the value's stype.
+static int value_row_fn(bool fill, int reverse, int64_t shift, dtb_col value, int64_t nrows_value, const void* order,
+                        int order_is64, const void* offsets, int64_t ngroups, dtb_stream stream, void* out)
+{
+  cudaStream_t s = (cudaStream_t)stream;
+  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
+  const char* fname = fill ? "fillna" : "shift";
+  const int esz = stype_bytes(value.stype);
+  if (!esz) {
+    set_error(std::string(fname) + " cannot be applied to columns of stype " + std::to_string(value.stype));
+    return DTB_ENOTIMPL;
+  }
+  if (ngroups < 0) { set_error("ngroups must be non-negative"); return DTB_EINVAL; }
+  if (!offsets) { set_error("offsets is NULL"); return DTB_EINVAL; }
+  if (nrows_value < 0) { set_error("nrows_value must be non-negative"); return DTB_EINVAL; }
+  if (!value.data && nrows_value > 0) { set_error("value column data is NULL"); return DTB_EINVAL; }
+  DTB_TRY(ensure_context());
+  if (ngroups == 0) return DTB_OK;
+  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
+  DevIn d_off;
+  int64_t n = 0;
+  DTB_TRY(bind_groupby(offsets, ngroups, true, s, d_off, n));
+  if (!out) { set_error("out is NULL"); return DTB_EINVAL; }
+  if (!order && n > nrows_value) { set_error("offsets cover more rows than the value column has"); return DTB_EINVAL; }
+  DevIn d_val, d_ord;
+  DTB_TRY(d_val.bind(value.data, (size_t)nrows_value * esz, s));
+  DTB_TRY(d_ord.bind(order, (size_t)n * (order_is64 ? 8 : 4), s));
+  const size_t out_bytes = (size_t)n * esz;
+  DevOut d_out; DTB_TRY(d_out.bind(out, out_bytes, s));
+  DevBuf scr;
+  if (fill) DTB_TRY(scr.alloc(cumulative_scratch_bytes(n), s));
+  {
+    ProfScope ps(fname, s);
+    if (fill)
+      DTB_TRY(launch_fillna(reverse, d_val.dptr, value.stype, nrows_value, d_ord.dptr, order_is64,
+                            (const int32_t*)d_off.dptr, ngroups, n, scr.p, d_out.dptr, s));
+    else
+      DTB_TRY(launch_shift(d_val.dptr, value.stype, nrows_value, d_ord.dptr, order_is64, (const int32_t*)d_off.dptr,
+                           ngroups, n, shift, d_out.dptr, s));
+  }
+  if (d_out.staged()) {
+    DTB_TRY(d_out.finish(out_bytes, s));
+    DTB_CUDA_CHECK(cudaStreamSynchronize(s));
+  }
+  return DTB_OK;
+}
+
+int dtb_shift(dtb_col value, int64_t nrows_value, const void* order, int order_is64, const void* offsets,
+              int64_t ngroups, int64_t n, dtb_stream stream, void* out)
+{
+  return value_row_fn(false, 0, n, value, nrows_value, order, order_is64, offsets, ngroups, stream, out);
+}
+
+int dtb_fillna(int reverse, dtb_col value, int64_t nrows_value, const void* order, int order_is64,
+               const void* offsets, int64_t ngroups, dtb_stream stream, void* out)
+{
+  return value_row_fn(true, reverse, 0, value, nrows_value, order, order_is64, offsets, ngroups, stream, out);
+}
+
+int dtb_group_index(int kind, int reverse, const void* offsets, int64_t ngroups, dtb_stream stream, void* out)
+{
+  cudaStream_t s = (cudaStream_t)stream;
+  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
+  if (kind != DTB_GROUP_CUMCOUNT && kind != DTB_GROUP_NGROUP) {
+    set_error("dtb_group_index takes DTB_GROUP_CUMCOUNT or DTB_GROUP_NGROUP"); return DTB_EINVAL;
+  }
+  if (ngroups < 0) { set_error("ngroups must be non-negative"); return DTB_EINVAL; }
+  if (!offsets) { set_error("offsets is NULL"); return DTB_EINVAL; }
+  DTB_TRY(ensure_context());
+  if (ngroups == 0) return DTB_OK;
+  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
+  DevIn d_off;
+  int64_t n = 0;
+  DTB_TRY(bind_groupby(offsets, ngroups, true, s, d_off, n));
+  if (!out) { set_error("out is NULL"); return DTB_EINVAL; }
+  const size_t out_bytes = (size_t)n * sizeof(int64_t);
+  DevOut d_out; DTB_TRY(d_out.bind(out, out_bytes, s));
+  {
+    ProfScope ps("group_index", s);
+    DTB_TRY(launch_group_index(kind, reverse, (const int32_t*)d_off.dptr, ngroups, n, (int64_t*)d_out.dptr, s));
+  }
+  if (d_out.staged()) {
+    DTB_TRY(d_out.finish(out_bytes, s));
+    DTB_CUDA_CHECK(cudaStreamSynchronize(s));
+  }
+  return DTB_OK;
+}
+
 int dtb_groupby_reduce_begin(dtb_groupby* g, int op, int value_stype, dtb_stream stream, dtb_reduce_state** out)
 {
   cudaStream_t s = (cudaStream_t)stream;

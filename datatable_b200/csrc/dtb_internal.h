@@ -305,6 +305,15 @@ int cumulative_out_stype(int op, int stype);
 size_t cumulative_scratch_bytes(int64_t n);
 int launch_cumulative(int op, int reverse, const void* v, int stype, int64_t nv, const void* order, int order_is64,
                       const int32_t* offsets, int64_t ng, int64_t n, void* scratch, void* out, cudaStream_t s);
+// shift / fillna / cumcount / ngroup inside every group (dtb_shift, dtb_fillna, dtb_group_index, dtb_reduce.cu):
+// out[p] for RowIndex position p, n elements of the value's stype (shift, fillna) or of int64 (group_index, kind
+// DTB_GROUP_CUMCOUNT / DTB_GROUP_NGROUP).  fillna's scratch: cumulative_scratch_bytes(n) of device memory.
+int launch_shift(const void* v, int stype, int64_t nv, const void* order, int order_is64, const int32_t* offsets,
+                 int64_t ng, int64_t n, int64_t shift, void* out, cudaStream_t s);
+int launch_fillna(int reverse, const void* v, int stype, int64_t nv, const void* order, int order_is64,
+                  const int32_t* offsets, int64_t ng, int64_t n, void* scratch, void* out, cudaStream_t s);
+int launch_group_index(int kind, int reverse, const int32_t* offsets, int64_t ng, int64_t n, int64_t* out,
+                       cudaStream_t s);
 int launch_set_select(const int32_t* order, const int32_t* offsets, int64_t ng, const int64_t* d_sizes, int K,
                       int mode, uint8_t* flags, cudaStream_t s);
 int launch_set_emit(const int32_t* pos, int64_t nsel, const int32_t* order, const int32_t* offsets, int32_t* out_rows,

@@ -702,9 +702,17 @@ int launch_nrows(const int32_t* offsets, int64_t ng, void* out, cudaStream_t s) 
 
 // One cumulative function over input type T: the scan state S, the element type O of out, the contribution of one
 // row (what the tile kernel writes into out), the fold, the merge (a = a then b) and the result of a state.
-enum { CUM_SUMI, CUM_SUMF, CUM_PRODI, CUM_PRODF, CUM_MIN, CUM_MAX };
+enum { CUM_SUMI, CUM_SUMF, CUM_PRODI, CUM_PRODF, CUM_MIN, CUM_MAX, CUM_FILL };
 
 template <typename T> struct CumMM { typename RawKey<T>::load_t b; };   // the latest extreme, or T's NA = none
+
+// T's NA as stored: the integer sentinel, or the quiet NaN dtb_gather writes
+template <typename T> __device__ __forceinline__ typename RawKey<T>::load_t raw_na() {
+  typedef typename RawKey<T>::load_t O;
+  if constexpr (std::is_same<T, float>::value) return (O)0x7FC00000u;
+  else if constexpr (std::is_same<T, double>::value) return (O)0x7FF8000000000000ull;
+  else return NaOf<T>::v();
+}
 
 template <int K, typename T> struct Cum;
 
@@ -774,14 +782,11 @@ template <typename T> struct Cum<CUM_PRODF, T> {
 // cummin / cummax: the state is the latest row holding the extreme so far, compared in T (prev < val ? prev : val
 // for min, > for max), so of equal values -- -0.0 and +0.0 included -- the later one wins.  "Latest among the
 // extremes" is associative.  An NA row leaves the state as it is; before the first valid row the state is NA.
+// CUM_FILL (fillna without a value) is the same state with every valid row winning: the latest valid value.
 template <int K, typename T> struct CumMinMax {
   typedef CumMM<T> S; typedef typename RawKey<T>::load_t O;
   static __device__ __forceinline__ O contrib(O raw, bool row_valid) { return row_valid ? raw : na(); }
-  static __device__ __forceinline__ O na() {
-    if constexpr (std::is_same<T, float>::value) return (O)0x7FC00000u;
-    else if constexpr (std::is_same<T, double>::value) return (O)0x7FF8000000000000ull;
-    else return NaOf<T>::v();
-  }
+  static __device__ __forceinline__ O na() { return raw_na<T>(); }
   static __device__ __forceinline__ bool valid(O b) { u64 u; return RawKey<T>::get(b, u); }
   static __device__ __forceinline__ T val(O b) {
     if constexpr (std::is_same<T, float>::value) return __uint_as_float((u32)b);
@@ -791,7 +796,7 @@ template <int K, typename T> struct CumMinMax {
   static __device__ __forceinline__ void init(S& a) { a.b = na(); }
   static __device__ __forceinline__ void add(S& a, O c) {
     if (!valid(c)) return;
-    if (valid(a.b) && (K == CUM_MIN ? val(a.b) < val(c) : val(a.b) > val(c))) return;
+    if (K != CUM_FILL && valid(a.b) && (K == CUM_MIN ? val(a.b) < val(c) : val(a.b) > val(c))) return;
     a.b = c;
   }
   static __device__ __forceinline__ void merge(S& a, const S& b) { add(a, b.b); }
@@ -800,6 +805,7 @@ template <int K, typename T> struct CumMinMax {
 };
 template <typename T> struct Cum<CUM_MIN, T> : CumMinMax<CUM_MIN, T> {};
 template <typename T> struct Cum<CUM_MAX, T> : CumMinMax<CUM_MAX, T> {};
+template <typename T> struct Cum<CUM_FILL, T> : CumMinMax<CUM_FILL, T> {};
 
 // (a, f) = (pa, pf) then (a, f): a segment state is the fold since the last head, f = a head was seen
 template <class C>
@@ -1058,6 +1064,168 @@ int launch_cumulative(int op, int reverse, const void* v, int stype, int64_t nv,
 #undef DTB_CUM_INT
 #undef DTB_CUM_ARGS
   set_error("internal: cumulative function / stype combination"); return DTB_EINVAL;
+}
+
+// ===========================================================================
+// Row functions per group: fillna, shift, cumcount, ngroup (dtb_fillna, dtb_shift, dtb_group_index)
+// ===========================================================================
+// fillna without a value replaces fill_rowindex (expr/fexpr_fillna.cc:66-118) and the apply_rowindex after it: it is
+// CUM_FILL of the cumulative scan above, the latest valid value of the group so far (REV: the earliest at or after).
+//
+// shift, cumcount and ngroup need no scan: a position's result depends only on its group's bounds.  One row-parallel
+// kernel over tiles of RTILE positions does them; the group of every position comes from the tile's head bitmap and
+// its popcount prefix, as in reduce_kernel.  Position q of the tile is t0 + i * RT + tid, so order is read and out
+// is written coalesced.
+//   ROW_SHIFT     out[p] = value[order[p - shift]] where p - shift lies in p's group [start, end), else NA: replaces
+//                 compute_lag_rowindex (expr/head_func_shift.cc:40-64) and the apply_rowindex after it in one pass;
+//                 no RowIndex of source positions is built.  Bound: the random value reads of a gather.
+//   ROW_CUMCOUNT  out[p] = p - start, reverse: end - 1 - p        (column/cumcountngroup.h:48-66)
+//   ROW_NGROUP    out[p] = g, reverse: ng - 1 - g                  Bound: the 8-byte write per row.
+enum { ROW_SHIFT, ROW_CUMCOUNT, ROW_NGROUP };
+
+template <int KIND, typename T, typename OrdT>
+__global__ void __launch_bounds__(RT, 1)
+group_row_kernel(const typename RawKey<T>::load_t* __restrict__ v, int64_t nv, const OrdT* __restrict__ order,
+                 const int32_t* __restrict__ offsets, int64_t ng, int64_t n, int64_t shift, int reverse,
+                 typename RawKey<T>::load_t* __restrict__ out)
+{
+  typedef typename RawKey<T>::load_t L;
+  __shared__ int64_t s_g[2];
+  __shared__ u32 s_bits[RTILE / 32];
+  __shared__ u32 s_wpre[RTILE / 32];
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int64_t t0 = (int64_t)blockIdx.x * RTILE;
+  const int64_t t1 = (t0 + RTILE < n) ? t0 + RTILE : n;
+  if (tid < RTILE / 32) s_bits[tid] = 0;
+  int64_t g_lo, g_hi;
+  tile_heads<false>(offsets, ng, n, t0, t1, tid, s_g, s_bits, g_lo, g_hi);
+  if (tid < 32) {
+    // exclusive prefix of popcounts over the RTILE/32 = 64 bitmap words (2 per lane)
+    const u32 a = __popc(s_bits[2 * lane]), b = __popc(s_bits[2 * lane + 1]);
+    u32 incl = a + b;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const u32 o = __shfl_up_sync(0xffffffffu, incl, d);
+      if (lane >= d) incl += o;
+    }
+    s_wpre[2 * lane] = incl - a - b;
+    s_wpre[2 * lane + 1] = incl - b;
+  }
+  __syncthreads();
+  // the group of tile position c is g_lo + heads(c), the number of heads at positions 1 .. c
+  auto heads = [&](int c) -> u32 { return s_wpre[c >> 5] + __popc(s_bits[c >> 5] & ((2u << (c & 31)) - 1u)); };
+
+  if constexpr (KIND == ROW_SHIFT) {
+    // all index loads first, then all value loads
+    int64_t row[RIPT];
+#pragma unroll
+    for (int i = 0; i < RIPT; i++) {
+      const int c = i * RT + tid;
+      const int64_t p = t0 + c, src = p - shift;               // |shift| <= 2^32: no overflow
+      row[i] = -1;
+      if (p < n) {
+        const int64_t g = g_lo + heads(c);
+        if (src >= (int64_t)offsets[g] && src < (int64_t)offsets[g + 1]) row[i] = order ? (int64_t)order[src] : src;
+      }
+    }
+    L val[RIPT];
+#pragma unroll
+    for (int i = 0; i < RIPT; i++) val[i] = (row[i] >= 0 && row[i] < nv) ? v[row[i]] : raw_na<T>();
+#pragma unroll
+    for (int i = 0; i < RIPT; i++) {
+      const int64_t p = t0 + i * RT + tid;
+      u64 u;
+      if (p < n) out[p] = RawKey<T>::get(val[i], u) ? val[i] : raw_na<T>();    // every NA as the stype's NA
+    }
+  } else if constexpr (KIND == ROW_CUMCOUNT) {
+#pragma unroll
+    for (int i = 0; i < RIPT; i++) {
+      const int c = i * RT + tid;
+      const int64_t p = t0 + c, g = g_lo + heads(c);
+      if (p < n) out[p] = reverse ? (int64_t)offsets[g + 1] - 1 - p : p - (int64_t)offsets[g];
+    }
+  } else {
+    const int64_t base = reverse ? ng - 1 - g_lo : g_lo;       // ngroup: base -+ heads(c)
+#pragma unroll
+    for (int i = 0; i < RIPT; i++) {
+      const int c = i * RT + tid;
+      const int64_t p = t0 + c, k = heads(c);
+      if (p < n) out[p] = reverse ? base - k : base + k;
+    }
+  }
+}
+
+template <typename T>
+static int run_shift(const void* v, int64_t nv, const void* order, int order_is64, const int32_t* offsets, int64_t ng,
+                     int64_t n, int64_t shift, void* out, cudaStream_t s)
+{
+  typedef typename RawKey<T>::load_t L;
+  const unsigned grid = (unsigned)((n + RTILE - 1) / RTILE);
+  if (order_is64)
+    group_row_kernel<ROW_SHIFT, T, int64_t><<<grid, RT, 0, s>>>((const L*)v, nv, (const int64_t*)order, offsets, ng, n,
+                                                                 shift, 0, (L*)out);
+  else
+    group_row_kernel<ROW_SHIFT, T, int32_t><<<grid, RT, 0, s>>>((const L*)v, nv, (const int32_t*)order, offsets, ng, n,
+                                                                 shift, 0, (L*)out);
+  count_launch(1);
+  DTB_CUDA_CHECK(cudaGetLastError());
+  return DTB_OK;
+}
+
+// out: n elements of the value's stype, out[p] for RowIndex position p.  The stype is checked by the caller.
+int launch_shift(const void* v, int stype, int64_t nv, const void* order, int order_is64, const int32_t* offsets,
+                 int64_t ng, int64_t n, int64_t shift, void* out, cudaStream_t s)
+{
+  if (n <= 0) return DTB_OK;
+  // positions are below 2^31, so every |shift| beyond that puts each source outside its group
+  const int64_t lim = (int64_t)1 << 32;
+  shift = shift > lim ? lim : (shift < -lim ? -lim : shift);
+#define DTB_SHIFT_ARGS v, nv, order, order_is64, offsets, ng, n, shift, out, s
+  switch (stype) {
+    case DTB_STYPE_BOOL: case DTB_STYPE_INT8: return run_shift<int8_t>(DTB_SHIFT_ARGS);
+    case DTB_STYPE_INT16: return run_shift<int16_t>(DTB_SHIFT_ARGS);
+    case DTB_STYPE_INT32: case DTB_STYPE_DATE32: return run_shift<int32_t>(DTB_SHIFT_ARGS);
+    case DTB_STYPE_INT64: case DTB_STYPE_TIME64: return run_shift<int64_t>(DTB_SHIFT_ARGS);
+    case DTB_STYPE_FLOAT32: return run_shift<float>(DTB_SHIFT_ARGS);
+    case DTB_STYPE_FLOAT64: return run_shift<double>(DTB_SHIFT_ARGS);
+  }
+#undef DTB_SHIFT_ARGS
+  set_error("internal: shift of stype " + std::to_string(stype)); return DTB_EINVAL;
+}
+
+// out: n elements of the value's stype; scratch: cumulative_scratch_bytes(n) of device memory.
+int launch_fillna(int reverse, const void* v, int stype, int64_t nv, const void* order, int order_is64,
+                  const int32_t* offsets, int64_t ng, int64_t n, void* scratch, void* out, cudaStream_t s)
+{
+  if (n <= 0) return DTB_OK;
+#define DTB_FILL_ARGS reverse, v, nv, order, order_is64, offsets, ng, n, scratch, out, s
+  switch (stype) {
+    case DTB_STYPE_BOOL: case DTB_STYPE_INT8: return run_cumulative_dir<CUM_FILL, int8_t>(DTB_FILL_ARGS);
+    case DTB_STYPE_INT16: return run_cumulative_dir<CUM_FILL, int16_t>(DTB_FILL_ARGS);
+    case DTB_STYPE_INT32: case DTB_STYPE_DATE32: return run_cumulative_dir<CUM_FILL, int32_t>(DTB_FILL_ARGS);
+    case DTB_STYPE_INT64: case DTB_STYPE_TIME64: return run_cumulative_dir<CUM_FILL, int64_t>(DTB_FILL_ARGS);
+    case DTB_STYPE_FLOAT32: return run_cumulative_dir<CUM_FILL, float>(DTB_FILL_ARGS);
+    case DTB_STYPE_FLOAT64: return run_cumulative_dir<CUM_FILL, double>(DTB_FILL_ARGS);
+  }
+#undef DTB_FILL_ARGS
+  set_error("internal: fillna of stype " + std::to_string(stype)); return DTB_EINVAL;
+}
+
+// kind: DTB_GROUP_CUMCOUNT or DTB_GROUP_NGROUP (checked by the caller); out: n int64 values.
+int launch_group_index(int kind, int reverse, const int32_t* offsets, int64_t ng, int64_t n, int64_t* out,
+                       cudaStream_t s)
+{
+  if (n <= 0) return DTB_OK;
+  const unsigned grid = (unsigned)((n + RTILE - 1) / RTILE);
+  if (kind == DTB_GROUP_CUMCOUNT)
+    group_row_kernel<ROW_CUMCOUNT, int64_t, int32_t><<<grid, RT, 0, s>>>(nullptr, 0, nullptr, offsets, ng, n, 0,
+                                                                          reverse, out);
+  else
+    group_row_kernel<ROW_NGROUP, int64_t, int32_t><<<grid, RT, 0, s>>>(nullptr, 0, nullptr, offsets, ng, n, 0,
+                                                                        reverse, out);
+  count_launch(1);
+  DTB_CUDA_CHECK(cudaGetLastError());
+  return DTB_OK;
 }
 
 // ===========================================================================

@@ -461,6 +461,58 @@ def cumulative(op, value, order, offsets, reverse=False, stype=None):
     return out
 
 
+def _row_fn_args(value, order, offsets, stype):
+    """(Col value, Col offsets, ngroups, Col order or None, positions, device) of a row function of (order, offsets)."""
+    v = Col(value, stype)
+    f = Col(offsets)
+    ngroups = f.nrows - 1
+    o = None if order is None else Col(order)
+    if o is not None and o.stype not in (INT32, INT64):
+        raise _lib.DtbValueError("order must be int32 or int64")
+    n = (int(offsets[-1].item()) if is_tensor(offsets) else int(offsets[-1])) if ngroups > 0 else 0
+    device = v.on_device and f.on_device and (o is None or o.on_device)
+    return v, f, ngroups, o, n, device
+
+
+def shift(value, order, offsets, n=1, stype=None):
+    """shift(value, n) inside every group of (order, offsets), as compute_lag_rowindex under by() (dtb_shift); one
+    group [0, nrows] is Shift_ColumnImpl without by().  Position p takes the value at position p - n of its group, NA
+    where that lies outside the group.  `order`: None = identity, int32 or int64.  Returns one value per position of
+    the RowIndex, of the value's stype; in HBM when the inputs are."""
+    v, f, ngroups, o, npos, device = _row_fn_args(value, order, offsets, stype)
+    out, optr = _alloc(npos, v.stype, device)
+    check(lib.dtb_shift(v.c(), v.nrows, ctypes.c_void_p(o.ptr) if o is not None else None,
+                        1 if o is not None and o.stype == INT64 else 0, ctypes.c_void_p(f.ptr), ngroups, int(n),
+                        _stream(), ctypes.c_void_p(optr)))
+    return out
+
+
+def fillna(value, order, offsets, reverse=False, stype=None):
+    """fillna(value) without a fill value inside every group of (order, offsets), as fill_rowindex (dtb_fillna): the
+    latest valid value at or before every position (reverse: the earliest at or after), NA before the first.  `order`:
+    None = identity, int32 or int64.  Returns one value per position of the RowIndex, of the value's stype; in HBM
+    when the inputs are."""
+    v, f, ngroups, o, npos, device = _row_fn_args(value, order, offsets, stype)
+    out, optr = _alloc(npos, v.stype, device)
+    check(lib.dtb_fillna(1 if reverse else 0, v.c(), v.nrows, ctypes.c_void_p(o.ptr) if o is not None else None,
+                         1 if o is not None and o.stype == INT64 else 0, ctypes.c_void_p(f.ptr), ngroups, _stream(),
+                         ctypes.c_void_p(optr)))
+    return out
+
+
+def group_index(kind, offsets, reverse=False):
+    """cumcount (GROUP_CUMCOUNT: the position inside the group) or ngroup (GROUP_NGROUP: the group's index) for every
+    position of the groups `offsets`, as CumcountNgroup_ColumnImpl (dtb_group_index); reverse counts from the other
+    end.  Returns int64[offsets[-1]]; in HBM when `offsets` is."""
+    f = Col(offsets)
+    ngroups = f.nrows - 1
+    n = (int(offsets[-1].item()) if is_tensor(offsets) else int(offsets[-1])) if ngroups > 0 else 0
+    out, optr = _alloc(n, INT64, f.on_device)
+    check(lib.dtb_group_index(kind, 1 if reverse else 0, ctypes.c_void_p(f.ptr), ngroups, _stream(),
+                              ctypes.c_void_p(optr)))
+    return out
+
+
 def set_select(mode, order, offsets, cum_sizes):
     """Group selection of union / intersect / setdiff / symdiff (set_funcs.cc:126-456): the first-row
     indices of the groups the operation keeps (int32, same memory kind as `order`)."""

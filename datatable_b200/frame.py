@@ -111,16 +111,17 @@ def count(x=None):
 
 class RowFn:
     """A function that returns one value per row and runs inside every group, the result in the grouped order (GtoALL):
-    qcut, cumsum, cumprod, cummin, cummax.  `cols` as given (a column, a list or tuple of columns, or f[:]); when the
-    query runs they are resolved and columns() makes one RowFnCol per column, with the function's checks of its other
-    arguments (evaluate_n of the reference's FExpr)."""
+    qcut, cumsum, cumprod, cummin, cummax, shift, fillna, cumcount, ngroup.  `cols` as given (a column, a list or tuple
+    of columns, or f[:]; None for a function of no column); when the query runs they are resolved and columns() makes
+    one RowFnCol per column, with the function's checks of its other arguments (evaluate_n of the reference's FExpr)."""
     def __init__(self, cols):
         self.cols = cols
 
 
 class RowFnCol:
     """One output column of a RowFn over column `name`: run(c, order, offsets) -> (values, stype), one value per
-    position of the RowIndex `order`, computed inside every group of `offsets`."""
+    position of the RowIndex `order`, computed inside every group of `offsets`.  name None: the function reads no
+    column (c is None) and its output is unnamed (C0, C1, ...)."""
     def __init__(self, name, run):
         self.name, self.run = name, run
 
@@ -194,6 +195,99 @@ def cummin(cols, reverse=False): return Cumulative(_lib.OP_MIN, "cummin", cols, 
 def cummax(cols, reverse=False): return Cumulative(_lib.OP_MAX, "cummax", cols, reverse)
 
 
+def _column_args_only(fname, cols):
+    """shift / fillna take column references; an expression or a reducer as the argument is not on the GPU path."""
+    for c in _flatten([cols]):
+        if not isinstance(c, (ColRef, str)):
+            raise NotImplementedError(f"{fname}() of an expression ({c!r}) is outside the GPU hot path")
+
+
+def _fixed_width(DT, name, fname):
+    st = DT._stypes[name]
+    if st not in _STYPE_NAMES:
+        raise NotImplementedError(f"{fname}() of a column of stype {st} is outside the GPU hot path")
+    return st
+
+
+class Shift(RowFn):
+    """dt.shift(cols, n=1) (expr/head_func_shift.cc:40-179): the value n rows earlier in the group (n < 0: -n rows
+    later), NA where that row is outside the group; without by() the selected rows are one group."""
+    def __init__(self, cols, n):
+        _column_args_only("shift", cols)
+        super().__init__(cols)
+        self.n = n
+
+    def columns(self, DT, refs):
+        return [RowFnCol(r.name, lambda c, order, offsets, st=_fixed_width(DT, r.name, "shift"):
+                         (engine.shift(c, order, offsets, self.n), st)) for r in refs]
+
+
+def shift(cols=None, n=1):
+    """pyfn_shift (expr/head_func_shift.cc:156-179): n is checked first, then cols; shift(frame, n) is
+    frame[:, shift(f[:], n)]."""
+    if n is None:
+        n = 1
+    if not isinstance(n, int) or isinstance(n, bool):
+        raise TypeError(f"Argument n in function datatable.shift() should be an integer, instead got {type(n)}")
+    if not -2**31 <= n < 2**31:
+        raise ValueError(f"Value is too large to fit in an int32: {n}")       # the reference's text on both sides
+    if cols is None:
+        raise TypeError("Function shift() requires 1 positional argument, but none were given")
+    if isinstance(cols, Frame):
+        return cols[:, Shift(f[:], n)]
+    if not isinstance(cols, (ColRef, Reducer, RowFn)):
+        raise TypeError(f"The first argument to shift() must be a column expression or a Frame, instead got "
+                        f"{type(cols)}")
+    return Shift(cols, n)
+
+
+class FillNA(RowFn):
+    """dt.fillna(cols, reverse=False) without a value (expr/fexpr_fillna.cc:66-118, 157-181): the latest valid value of
+    the group so far (reverse: the earliest at or after the row), NA before the first; without by() the selected
+    rows are one group."""
+    def __init__(self, cols, reverse):
+        _column_args_only("fillna", cols)
+        super().__init__(cols)
+        self.reverse = reverse
+
+    def columns(self, DT, refs):
+        return [RowFnCol(r.name, lambda c, order, offsets, st=_fixed_width(DT, r.name, "fillna"):
+                         (engine.fillna(c, order, offsets, self.reverse), st)) for r in refs]
+
+
+def fillna(cols, value=None, reverse=None):
+    """pyfn_fillna (expr/fexpr_fillna.cc:209-226).  fillna(cols, value=) is an elementwise if-else with the reference's
+    type promotion, which belongs to an expression engine: NotImplementedError."""
+    if value is not None and reverse is not None:
+        raise ValueError("Parameters value and reverse in function datatable.fillna() cannot be both set at the same "
+                         "time")
+    if reverse is not None and not isinstance(reverse, bool):
+        raise TypeError(f"Expected a boolean, instead got {type(reverse)}")
+    if value is not None:
+        raise NotImplementedError("fillna(cols, value=) is outside the GPU hot path")
+    return FillNA(cols, bool(reverse))
+
+
+class GroupIndex(RowFn):
+    """dt.cumcount(reverse=False) / dt.ngroup(reverse=False) (expr/fexpr_cumcountngroup.cc:40-116): int64, no input
+    column, an unnamed output (C0, C1, ...).  Without by() the selected rows are one group: 0 .. n-1 and 0."""
+    def __init__(self, kind, fname, reverse):
+        if reverse is None:
+            reverse = False
+        if not isinstance(reverse, bool):
+            raise TypeError(f"Argument reverse in function datatable.{fname}() should be a boolean, instead got "
+                            f"{type(reverse)}")
+        super().__init__(None)
+        self.kind, self.reverse = kind, reverse
+
+    def columns(self, DT, refs):
+        return [RowFnCol(None, lambda c, order, offsets: (engine.group_index(self.kind, offsets, self.reverse), INT64))]
+
+
+def cumcount(reverse=False): return GroupIndex(_lib.GROUP_CUMCOUNT, "cumcount", reverse)
+def ngroup(reverse=False): return GroupIndex(_lib.GROUP_NGROUP, "ngroup", reverse)
+
+
 def _cols_repr(cols):
     if isinstance(cols, (list, tuple)):
         return "[" + ", ".join(_cols_repr(c) for c in cols) + "]"
@@ -216,6 +310,8 @@ def _to_int32_strict(x):
 def _rowfn_cols(DT, e, bynames):
     """The columns of RowFn e (FExpr::evaluate_n of its argument): one RowFnCol per input column.  f[:] under by()
     leaves out the by() columns."""
+    if e.cols is None:
+        return e.columns(DT, [])
     refs = []
     for c in _flatten([e.cols]):
         if isinstance(c, ColRef) and isinstance(c.name, slice):
@@ -752,10 +848,10 @@ def _evaluate(DT, j, by_, sort_, isel=None):
         for name, e in zip(names, exprs):
             if e.name in bynames and j_is_all(j):
                 continue
-            c = dcol(e.name)
             if isinstance(e, RowFnCol):                    # inside every group, in the grouped order (GtoALL)
-                add(name, *e.run(c, order, offsets))
+                add(name, *e.run(None if e.name is None else dcol(e.name), order, offsets))
             else:
+                c = dcol(e.name)
                 add(name, engine.gather(c, order), c.stype)
         out._nrows = len(order)
         return out
@@ -776,7 +872,7 @@ def _evaluate(DT, j, by_, sort_, isel=None):
             # no Groupby (sort() alone, an `i` slice, or neither): one group of the selected rows in their order
             nsel = DT.nrows if order is None else len(order)
             offs = torch.tensor([0, nsel] if nsel else [0], dtype=torch.int32, device="cuda")
-            add(name, *e.run(dcol(e.name), order, offs))
+            add(name, *e.run(None if e.name is None else dcol(e.name), order, offs))
         elif order is None:
             c = DT._col(e.name)
             out._cols[name] = c.data; out._stypes[name] = c.stype
@@ -815,8 +911,8 @@ def _resolve_j(DT, j, bynames=()):
     names = []
     nbin = 0
     for e in es:
-        if isinstance(e, Reducer2):
-            names.append(f"C{nbin}")                                  # unnamed cov / corr columns: C0, C1, ...
+        if isinstance(e, Reducer2) or (isinstance(e, RowFnCol) and e.name is None):
+            names.append(f"C{nbin}")                                  # unnamed columns (cov, corr, cumcount, ngroup): C0, C1, ...
             nbin += 1
         elif isinstance(e, Reducer):
             names.append("count" if e.arg is None else e.arg.name)     # reducers keep the column's name

@@ -329,6 +329,40 @@ DTB_API int dtb_cumulative(int op, int reverse, dtb_col value, int64_t nrows_val
                            int order_is64, const void* offsets, int64_t ngroups, dtb_stream stream, void* out);
 
 /*
+ * dtb_shift, dtb_fillna, dtb_group_index -- the row functions that return one value per position inside every group
+ * (the GtoALL layout of the grouped frame).  Like dtb_cumulative, the value column is seen through `order` (NULL =
+ * identity; order_is64: int64 row ids) and cut by `offsets` (int32[ngroups+1], a Groupby, validated as dtb_reduce
+ * validates it; one group [0, n] for a call without by()), with host or device pointers; ngroups == 0 returns at once.
+ * Up to INT32_MAX positions.  out holds offsets[ngroups] elements, out[p] for position p of the RowIndex.  Results
+ * are deterministic: every output element is computed by one thread, so two calls give the same bytes.
+ * Errors: an stype without a fixed width gives DTB_ENOTIMPL; a bad kind, negative ngroups, NULL offsets, or offsets
+ * covering more rows than the column has without an order give DTB_EINVAL.
+ *
+ * dtb_shift: replaces compute_lag_rowindex (expr/head_func_shift.cc:40-64) and Shift_ColumnImpl (column/shift.h:37-88).
+ *   out[p] = value[order[p - n]] when p - n lies in p's group, else NA: n > 0 lags, n < 0 leads, n = 0 gathers the
+ *   column, and |n| >= the group's size gives a group of NA.  out has value.stype (every fixed-width stype).  The rule
+ *   holds for every int64 n, where the reference computes p - n in int32 and compares against nrows - |n| in size_t
+ *   (so its results for |n| beyond the positions come from overflow and are not followed).  NA: a source that is NA,
+ *   or outside the group, gives the stype's NA (a float NaN comes out as the quiet NaN 0x7FC00000 / 0x7FF8...);
+ *   every valid value keeps its bits, -0.0 included.  Bit-exact.
+ * dtb_fillna: replaces fill_rowindex (expr/fexpr_fillna.cc:66-118): fillna(cols) without a value.  out[p] = the
+ *   latest valid value of p's group at or before p (reverse != 0: the earliest at or after p), or NA where there is
+ *   none.  out has value.stype.  NA and bits as for dtb_shift; bit-exact.  fillna(cols, value=) is not this call.
+ * dtb_group_index: replaces CumcountNgroup_ColumnImpl (column/cumcountngroup.h:30-73).  Writes int64[offsets[ngroups]]:
+ *   DTB_GROUP_CUMCOUNT  p - start of p's group (reverse != 0: end - 1 - p);
+ *   DTB_GROUP_NGROUP    the index g of p's group (reverse != 0: ngroups - 1 - g).
+ *   Never NA.
+ */
+#define DTB_GROUP_CUMCOUNT 1
+#define DTB_GROUP_NGROUP   2
+DTB_API int dtb_shift(dtb_col value, int64_t nrows_value, const void* order, int order_is64,
+                      const void* offsets, int64_t ngroups, int64_t n, dtb_stream stream, void* out);
+DTB_API int dtb_fillna(int reverse, dtb_col value, int64_t nrows_value, const void* order, int order_is64,
+                       const void* offsets, int64_t ngroups, dtb_stream stream, void* out);
+DTB_API int dtb_group_index(int kind, int reverse, const void* offsets, int64_t ngroups,
+                            dtb_stream stream, void* out);
+
+/*
  * dtb_gather -- replaces materialisation of ArrayView_ColumnImpl<int32/int64>
  * (column/view.cc:88-155): out[i] = order[i] < 0 ? NA : src[order[i]].
  */
