@@ -1,10 +1,12 @@
 // dtb_api.cu -- the C-ABI (include/dtb200.h): call planning, HBM scratch,
 // host<->device staging and error reporting.  No compute happens on the host:
-// without a CUDA device every entry point fails with DTB_ECUDA.
+// without a CUDA device every entry point whose arguments pass the host checks
+// fails with DTB_ECUDA.
 #include <stdio.h>
 #include <chrono>
 #include <string.h>
 #include <mutex>
+#include <optional>
 #include <string>
 #include <vector>
 #include "dtb_common.cuh"
@@ -881,18 +883,17 @@ static int direct_reduce(const DirectGroups& dg, const DirectPlan& dp, int op, d
   return launch_direct_finalize(op, value.stype, acc0, acc1, dp, (const uint32_t*)dg.gkeys, ng, out, rows, s);
 }
 
-// A reducer over `value` seen through the RowIndex `order` (order_is64: int64 row ids); acc: 2 * ng u64 of scratch.
-static int reduce_rowindex(int op, dtb_col value, int64_t nrows_value, const void* order, int order_is64,
+// A reducer over the device column `value` seen through the RowIndex `order` (order_is64: int64 row ids); acc: 2 * ng
+// u64 of scratch.
+static int reduce_rowindex(int op, const void* value, int stype, int64_t nrows_value, const void* order, int order_is64,
                            const int32_t* offsets, int64_t ng, int64_t n, u64* acc, void* out, cudaStream_t s)
 {
-  DevIn dv;
-  if (op != DTB_OP_NROWS) DTB_TRY(dv.bind(value.data, (size_t)nrows_value * stype_bytes(value.stype), s));
   DevBuf extra;
-  const size_t xb = reduce_extra_bytes(op, value.stype, ng, n);
+  const size_t xb = reduce_extra_bytes(op, stype, ng, n);
   if (xb) DTB_TRY(extra.alloc(xb, s));
   ProfScope ps("reduce", s);
-  return launch_reduce_impl(op, dv.dptr, value.stype, nrows_value, order, order_is64, offsets, ng, n, acc, acc + ng,
-                            out, s, xb ? extra.p : nullptr);
+  return launch_reduce_impl(op, value, stype, nrows_value, order, order_is64, offsets, ng, n, acc, acc + ng, out, s,
+                            xb ? extra.p : nullptr);
 }
 
 // The fused reducers, once the groups are known.  When the group key domain is small they only need the key
@@ -934,7 +935,9 @@ static int fused_reduce(const GroupPlan& gp, int64_t n, const int32_t* order, co
       u64* acc = b.facc.as<u64>() + (size_t)gp.ftable * 2 * i;
       DTB_TRY(direct_reduce(res.direct, dp, sp.op, sp.value, order, offsets, n, ng, acc, acc + gp.ftable, true, ob.p, s));
     } else {
-      DTB_TRY(reduce_rowindex(sp.op, sp.value, n, order, 0, offsets, ng, n, gacc.as<u64>(), ob.p, s));
+      DevIn dv;
+      if (sp.op != DTB_OP_NROWS) DTB_TRY(dv.bind(sp.value.data, (size_t)n * stype_bytes(sp.value.stype), s));
+      DTB_TRY(reduce_rowindex(sp.op, dv.dptr, sp.value.stype, n, order, 0, offsets, ng, n, gacc.as<u64>(), ob.p, s));
     }
     fr.out[i] = ob.detach();
   }
@@ -1297,129 +1300,172 @@ static int bind_groupby(const void* offsets, int64_t ngroups, bool check_offsets
   return DTB_OK;
 }
 
-// check_offsets = false: the offsets come from group() (a handle's own), so they need no device check
-static int reduce_groups(int op, dtb_col value, int64_t nrows_value, const void* order, int order_is64,
-                         const void* offsets, int64_t ngroups, dtb_stream stream, void* out, bool check_offsets)
+// The arguments every per-group entry point shares (include/dtb200.h, "Per-group functions"): value columns of
+// nrows_value rows seen through the RowIndex `order` (NULL = identity), cut by the Groupby `offsets`, and one output.
+// An entry point constructs it first (which resets the call statistics), then checks its own argument and the stype;
+// enter() runs the shared checks on the host, then makes the context and opens the arena; bind() reads n and binds the
+// buffers; finish() copies a staged output back.
+struct Grouped {
+  cudaStream_t s;
+  dtb_col value[2] = {};
+  int nvalues;                  // value columns: 0 (dtb_group_index, DTB_OP_NROWS), 1, or 2 (dtb_reduce2)
+  int64_t nrows_value;
+  const void* order;
+  int order_is64;
+  const void* offsets;
+  int64_t ngroups;
+  void* out;
+  bool handle = false;          // a handle's own offsets: group() made them, so they need no device check
+  bool within_column = false;   // without an order, positions beyond the value column are an error (the row
+                                // functions); otherwise they read as NA (the reducers, dtb_sort_grouped)
+  bool per_position = false;    // out holds one element per position, else one per group
+  std::optional<ArenaScope> scope;
+  DevIn off, ord, val[2];
+  DevOut dout;
+  int64_t n = 0;                // positions: offsets[ngroups]
+
+  Grouped(dtb_stream stream, std::initializer_list<dtb_col> values, int64_t nrows_value_, const void* order_,
+          int order_is64_, const void* offsets_, int64_t ngroups_, void* out_)
+    : s((cudaStream_t)stream), nvalues((int)values.size()), nrows_value(nrows_value_), order(order_),
+      order_is64(order_is64_), offsets(offsets_), ngroups(ngroups_), out(out_)
+  {
+    int i = 0;
+    for (const dtb_col& v : values) value[i++] = v;
+    t_stats = dtb_call_stats{0, 0, 0, 0, 0};
+  }
+
+  // ngroups == 0 leaves nothing to do: the caller returns.
+  int enter() {
+    if (ngroups < 0) { set_error("ngroups must be non-negative"); return DTB_EINVAL; }
+    if (!offsets) { set_error("offsets is NULL"); return DTB_EINVAL; }
+    if (nrows_value < 0) { set_error("nrows_value must be non-negative"); return DTB_EINVAL; }
+    for (int i = 0; i < nvalues; i++)
+      if (!value[i].data && nrows_value > 0) { set_error("value column data is NULL"); return DTB_EINVAL; }
+    if (!out && ngroups > 0) { set_error("out is NULL"); return DTB_EINVAL; }
+    DTB_TRY(ensure_context());
+    if (ngroups == 0) return DTB_OK;
+    scope.emplace(s);
+    return scope->rc;
+  }
+
+  // out_esz: bytes per output element.
+  int bind(int out_esz) {
+    DTB_TRY(bind_groupby(offsets, ngroups, !handle, s, off, n));
+    if (within_column && !order && n > nrows_value) {
+      set_error("offsets cover more rows than the value column has"); return DTB_EINVAL;
+    }
+    for (int i = 0; i < nvalues; i++)
+      DTB_TRY(val[i].bind(value[i].data, (size_t)nrows_value * stype_bytes(value[i].stype), s));
+    DTB_TRY(ord.bind(order, (size_t)n * (order_is64 ? 8 : 4), s));
+    return dout.bind(out, (size_t)(per_position ? n : ngroups) * out_esz, s);
+  }
+
+  int open(int out_esz) {
+    DTB_TRY(enter());
+    return ngroups ? bind(out_esz) : DTB_OK;
+  }
+
+  // Waits for the stream when the output was staged, or always when sync.
+  int finish(bool sync = false) {
+    if (dout.staged()) DTB_TRY(dout.finish(dout.bytes, s));
+    if (sync || dout.staged()) DTB_CUDA_CHECK(cudaStreamSynchronize(s));
+    return DTB_OK;
+  }
+
+  const int32_t* offs() const { return (const int32_t*)off.dptr; }
+};
+
+// The stype check of the functions that take every fixed-width stype.
+static int fixed_width(int stype, const char* fname) {
+  if (stype_supported(stype)) return DTB_OK;
+  set_error(std::string(fname) + " cannot be applied to columns of stype " + std::to_string(stype));
+  return DTB_ENOTIMPL;
+}
+
+// dtb_reduce, and dtb_groupby_reduce with its handle g: where the handle's key domain is small, sum..countna over a
+// device column stream the key and value columns in storage order instead of reading through the RowIndex.
+static int reduce_groups(int op, Grouped& c, const dtb_groupby* g)
 {
-  cudaStream_t s = (cudaStream_t)stream;
-  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
-  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
-  if (ngroups < 0) { set_error("ngroups must be non-negative"); return DTB_EINVAL; }
-  if (!offsets) { set_error("offsets is NULL"); return DTB_EINVAL; }
-  if (!out && ngroups > 0) { set_error("out is NULL"); return DTB_EINVAL; }
+  const dtb_col value = c.value[0];
+  if (op < DTB_OP_SUM || op > DTB_OP_CORR) { set_error("unknown reducer " + std::to_string(op)); return DTB_EINVAL; }
   int out_st = 0;
   DTB_TRY(reducer_out_stype(op, value.stype, out_st));
-  if (op != DTB_OP_NROWS && !value.data && nrows_value > 0) { set_error("value column data is NULL"); return DTB_EINVAL; }
-  DTB_TRY(ensure_context());
-  if (ngroups == 0) return DTB_OK;
-
-  DevIn d_off;
-  int64_t n = 0;
-  DTB_TRY(bind_groupby(offsets, ngroups, check_offsets, s, d_off, n));
-  DevIn d_ord;
-  if (op != DTB_OP_NROWS) DTB_TRY(d_ord.bind(order, (size_t)n * (order_is64 ? 8 : 4), s));
-  DevOut d_out; DTB_TRY(d_out.bind(out, (size_t)ngroups * stype_bytes(out_st), s));
-  DevBuf acc; DTB_TRY(acc.alloc(sizeof(u64) * (size_t)ngroups * 2, s));
-  DTB_TRY(reduce_rowindex(op, value, nrows_value, d_ord.dptr, order_is64, (const int32_t*)d_off.dptr, ngroups, n,
-                          acc.as<u64>(), d_out.dptr, s));
-  if (d_out.staged()) {
-    DTB_TRY(d_out.finish((size_t)ngroups * stype_bytes(out_st), s));
-    DTB_CUDA_CHECK(cudaStreamSynchronize(s));
+  if (op == DTB_OP_NROWS) { c.nvalues = 0; c.order = nullptr; }   // reads neither the column nor the RowIndex
+  DTB_TRY(c.enter());
+  if (c.ngroups == 0) return DTB_OK;
+  if (g && g->direct.on && op < DTB_OP_NROWS && c.nrows_value == g->nrows && is_device_ptr(value.data)) {
+    const DirectGroups& dg = g->direct;
+    DTB_TRY(c.dout.bind(c.out, (size_t)c.ngroups * stype_bytes(out_st), c.s));
+    DevBuf acc; DTB_TRY(acc.alloc(sizeof(u64) * (size_t)dg.table * 2, c.s));
+    DevBuf dmap; DTB_TRY(dmap.alloc(direct_map_bytes(dg.table), c.s));
+    DirectPlan dp;
+    DTB_TRY(plan_direct(dg.table, (const uint32_t*)dg.gkeys, (const int32_t*)g->offsets, g->ngroups, g->nrows,
+                        dg.gmax, dmap.p, c.s, dp));
+    DTB_TRY(direct_reduce(dg, dp, op, value, (const int32_t*)g->order, (const int32_t*)g->offsets, g->nrows, g->ngroups,
+                          acc.as<u64>(), acc.as<u64>() + dg.table, true, c.dout.dptr, c.s));
+  } else {
+    DTB_TRY(c.bind(stype_bytes(out_st)));
+    DevBuf acc; DTB_TRY(acc.alloc(sizeof(u64) * (size_t)c.ngroups * 2, c.s));
+    DTB_TRY(reduce_rowindex(op, c.val[0].dptr, value.stype, c.nrows_value, c.ord.dptr, c.order_is64, c.offs(),
+                            c.ngroups, c.n, acc.as<u64>(), c.dout.dptr, c.s));
   }
-  return DTB_OK;
+  return c.finish();
 }
 
 int dtb_reduce(int op, dtb_col value, int64_t nrows_value, const void* order, int order_is64,
                const void* offsets, int64_t ngroups, dtb_stream stream, void* out)
 {
-  return reduce_groups(op, value, nrows_value, order, order_is64, offsets, ngroups, stream, out, true);
+  Grouped c(stream, {value}, nrows_value, order, order_is64, offsets, ngroups, out);
+  return reduce_groups(op, c, nullptr);
 }
 
 int dtb_groupby_reduce(dtb_groupby* g, int op, dtb_col value, int64_t nrows_value, dtb_stream stream, void* out)
 {
-  cudaStream_t s = (cudaStream_t)stream;
   if (!g) { set_error("groupby handle is NULL"); return DTB_EINVAL; }
   if (g->ngroups < 0) { set_error("the handle holds no Groupby (sort-only call)"); return DTB_EINVAL; }
-  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
-  const bool device_value = (op == DTB_OP_NROWS) || is_device_ptr(value.data);
-  if (!g->direct.on || op == DTB_OP_NROWS || op >= DTB_OP_FIRST || !device_value || nrows_value != g->nrows)
-    return reduce_groups(op, value, nrows_value, g->order, 0, g->offsets, g->ngroups, stream, out, false);
-  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
-  int out_st = 0;
-  DTB_TRY(reducer_out_stype(op, value.stype, out_st));
-  if (!out && g->ngroups > 0) { set_error("out is NULL"); return DTB_EINVAL; }
-  DTB_TRY(ensure_context());
-  if (g->ngroups == 0) return DTB_OK;
-  const DirectGroups& dg = g->direct;
-  DevOut d_out; DTB_TRY(d_out.bind(out, (size_t)g->ngroups * stype_bytes(out_st), s));
-  DevBuf acc; DTB_TRY(acc.alloc(sizeof(u64) * (size_t)dg.table * 2, s));
-  DevBuf dmap; DTB_TRY(dmap.alloc(direct_map_bytes(dg.table), s));
-  DirectPlan dp;
-  DTB_TRY(plan_direct(dg.table, (const uint32_t*)dg.gkeys, (const int32_t*)g->offsets, g->ngroups, g->nrows,
-                      dg.gmax, dmap.p, s, dp));
-  DTB_TRY(direct_reduce(dg, dp, op, value, (const int32_t*)g->order, (const int32_t*)g->offsets, g->nrows, g->ngroups,
-                        acc.as<u64>(), acc.as<u64>() + dg.table, true, d_out.dptr, s));
-  if (d_out.staged()) {
-    DTB_TRY(d_out.finish((size_t)g->ngroups * stype_bytes(out_st), s));
-    DTB_CUDA_CHECK(cudaStreamSynchronize(s));
-  }
-  return DTB_OK;
+  Grouped c(stream, {value}, nrows_value, g->order, 0, g->offsets, g->ngroups, out);
+  c.handle = true;
+  return reduce_groups(op, c, g);
 }
 
 int dtb_reduce2_out_stype(int op, int stype_x, int stype_y) { return reduce2_out_stype_host(op, stype_x, stype_y); }
 
-static int reduce2_groups(int op, dtb_col x, dtb_col y, int64_t nrows_value, const void* order, int order_is64,
-                          const void* offsets, int64_t ngroups, dtb_stream stream, void* out, bool check_offsets)
+// dtb_reduce2 and dtb_groupby_reduce2: c holds the columns x and y.
+static int reduce2_groups(int op, Grouped& c)
 {
-  cudaStream_t s = (cudaStream_t)stream;
-  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
-  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
+  const dtb_col x = c.value[0], y = c.value[1];
   if (op != DTB_OP_COV && op != DTB_OP_CORR) { set_error("dtb_reduce2 takes DTB_OP_COV or DTB_OP_CORR"); return DTB_EINVAL; }
-  if (ngroups < 0) { set_error("ngroups must be non-negative"); return DTB_EINVAL; }
-  if (!offsets) { set_error("offsets is NULL"); return DTB_EINVAL; }
-  if (!out && ngroups > 0) { set_error("out is NULL"); return DTB_EINVAL; }
   const int out_st = reduce2_out_stype_host(op, x.stype, y.stype);
   if (!out_st) {
     set_error("Invalid columns of stypes " + std::to_string(x.stype) + ", " + std::to_string(y.stype) + " in reducer " +
               std::to_string(op));
     return (stype_supported(x.stype) && stype_supported(y.stype)) ? DTB_EINVAL : DTB_ENOTIMPL;
   }
-  if (nrows_value < 0) { set_error("nrows_value must be non-negative"); return DTB_EINVAL; }
-  if ((!x.data || !y.data) && nrows_value > 0) { set_error("value column data is NULL"); return DTB_EINVAL; }
-  DTB_TRY(ensure_context());
-  if (ngroups == 0) return DTB_OK;
-  DevIn d_off;
-  int64_t n = 0;
-  DTB_TRY(bind_groupby(offsets, ngroups, check_offsets, s, d_off, n));
-  DevIn d_ord, dx, dy;
-  DTB_TRY(d_ord.bind(order, (size_t)n * (order_is64 ? 8 : 4), s));
-  DTB_TRY(dx.bind(x.data, (size_t)nrows_value * stype_bytes(x.stype), s));
-  DTB_TRY(dy.bind(y.data, (size_t)nrows_value * stype_bytes(y.stype), s));
-  DevOut d_out; DTB_TRY(d_out.bind(out, (size_t)ngroups * stype_bytes(out_st), s));
-  DevBuf scr; DTB_TRY(scr.alloc(reduce2_scratch_bytes(ngroups), s));
+  DTB_TRY(c.open(stype_bytes(out_st)));
+  if (c.ngroups == 0) return DTB_OK;
+  DevBuf scr; DTB_TRY(scr.alloc(reduce2_scratch_bytes(c.ngroups), c.s));
   {
-    ProfScope ps("reduce2", s);
-    DTB_TRY(launch_reduce2(op, dx.dptr, x.stype, dy.dptr, y.stype, nrows_value, d_ord.dptr, order_is64,
-                           (const int32_t*)d_off.dptr, ngroups, n, scr.as<u64>(), out_st == DTB_STYPE_FLOAT32, d_out.dptr, s));
+    ProfScope ps("reduce2", c.s);
+    DTB_TRY(launch_reduce2(op, c.val[0].dptr, x.stype, c.val[1].dptr, y.stype, c.nrows_value, c.ord.dptr, c.order_is64,
+                           c.offs(), c.ngroups, c.n, scr.as<u64>(), out_st == DTB_STYPE_FLOAT32, c.dout.dptr, c.s));
   }
-  if (d_out.staged()) {
-    DTB_TRY(d_out.finish((size_t)ngroups * stype_bytes(out_st), s));
-    DTB_CUDA_CHECK(cudaStreamSynchronize(s));
-  }
-  return DTB_OK;
+  return c.finish();
 }
 
 int dtb_reduce2(int op, dtb_col x, dtb_col y, int64_t nrows_value, const void* order, int order_is64,
                 const void* offsets, int64_t ngroups, dtb_stream stream, void* out)
 {
-  return reduce2_groups(op, x, y, nrows_value, order, order_is64, offsets, ngroups, stream, out, true);
+  Grouped c(stream, {x, y}, nrows_value, order, order_is64, offsets, ngroups, out);
+  return reduce2_groups(op, c);
 }
 
 int dtb_groupby_reduce2(dtb_groupby* g, int op, dtb_col x, dtb_col y, int64_t nrows_value, dtb_stream stream, void* out)
 {
   if (!g) { set_error("groupby handle is NULL"); return DTB_EINVAL; }
   if (g->ngroups < 0) { set_error("the handle holds no Groupby (sort-only call)"); return DTB_EINVAL; }
-  return reduce2_groups(op, x, y, nrows_value, g->order, 0, g->offsets, g->ngroups, stream, out, false);
+  Grouped c(stream, {x, y}, nrows_value, g->order, 0, g->offsets, g->ngroups, out);
+  c.handle = true;
+  return reduce2_groups(op, c);
 }
 
 int dtb_cumulative_out_stype(int op, int stype) { return cumulative_out_stype(op, stype); }
@@ -1427,135 +1473,75 @@ int dtb_cumulative_out_stype(int op, int stype) { return cumulative_out_stype(op
 int dtb_cumulative(int op, int reverse, dtb_col value, int64_t nrows_value, const void* order, int order_is64,
                    const void* offsets, int64_t ngroups, dtb_stream stream, void* out)
 {
-  cudaStream_t s = (cudaStream_t)stream;
-  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
+  Grouped c(stream, {value}, nrows_value, order, order_is64, offsets, ngroups, out);
   if (op != DTB_OP_SUM && op != DTB_OP_PROD && op != DTB_OP_MIN && op != DTB_OP_MAX) {
     set_error("dtb_cumulative takes DTB_OP_SUM, DTB_OP_PROD, DTB_OP_MIN or DTB_OP_MAX"); return DTB_EINVAL;
   }
-  const int esz = stype_bytes(value.stype);
-  if (!esz) { set_error("cumulative functions cannot be applied to columns of stype " + std::to_string(value.stype)); return DTB_ENOTIMPL; }
+  DTB_TRY(fixed_width(value.stype, "cumulative functions"));
   const int out_st = cumulative_out_stype(op, value.stype);
   if (!out_st) {
     set_error("Invalid column of stype " + std::to_string(value.stype) + " in cumulative function " + std::to_string(op));
     return DTB_EINVAL;
   }
-  if (ngroups < 0) { set_error("ngroups must be non-negative"); return DTB_EINVAL; }
-  if (!offsets) { set_error("offsets is NULL"); return DTB_EINVAL; }
-  if (nrows_value < 0) { set_error("nrows_value must be non-negative"); return DTB_EINVAL; }
-  if (!value.data && nrows_value > 0) { set_error("value column data is NULL"); return DTB_EINVAL; }
-  DTB_TRY(ensure_context());
-  if (ngroups == 0) return DTB_OK;
-  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
-  DevIn d_off;
-  int64_t n = 0;
-  DTB_TRY(bind_groupby(offsets, ngroups, true, s, d_off, n));
-  if (!out) { set_error("out is NULL"); return DTB_EINVAL; }
-  if (!order && n > nrows_value) { set_error("offsets cover more rows than the value column has"); return DTB_EINVAL; }
-  DevIn d_val, d_ord;
-  DTB_TRY(d_val.bind(value.data, (size_t)nrows_value * esz, s));
-  DTB_TRY(d_ord.bind(order, (size_t)n * (order_is64 ? 8 : 4), s));
-  const size_t out_bytes = (size_t)n * stype_bytes(out_st);
-  DevOut d_out; DTB_TRY(d_out.bind(out, out_bytes, s));
-  DevBuf scr; DTB_TRY(scr.alloc(cumulative_scratch_bytes(n), s));
+  c.within_column = c.per_position = true;
+  DTB_TRY(c.open(stype_bytes(out_st)));
+  if (c.ngroups == 0) return DTB_OK;
+  DevBuf scr; DTB_TRY(scr.alloc(cumulative_scratch_bytes(c.n), c.s));
   {
-    ProfScope ps("cumulative", s);
-    DTB_TRY(launch_cumulative(op, reverse, d_val.dptr, value.stype, nrows_value, d_ord.dptr, order_is64,
-                              (const int32_t*)d_off.dptr, ngroups, n, scr.p, d_out.dptr, s));
+    ProfScope ps("cumulative", c.s);
+    DTB_TRY(launch_cumulative(op, reverse, c.val[0].dptr, value.stype, nrows_value, c.ord.dptr, order_is64, c.offs(),
+                              ngroups, c.n, scr.p, c.dout.dptr, c.s));
   }
-  if (d_out.staged()) {
-    DTB_TRY(d_out.finish(out_bytes, s));
-    DTB_CUDA_CHECK(cudaStreamSynchronize(s));
-  }
-  return DTB_OK;
-}
-
-// dtb_shift / dtb_fillna (fill: reverse; else shift): the argument checks and buffers of dtb_cumulative and an output
-// of the value's stype.
-static int value_row_fn(bool fill, int reverse, int64_t shift, dtb_col value, int64_t nrows_value, const void* order,
-                        int order_is64, const void* offsets, int64_t ngroups, dtb_stream stream, void* out)
-{
-  cudaStream_t s = (cudaStream_t)stream;
-  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
-  const char* fname = fill ? "fillna" : "shift";
-  const int esz = stype_bytes(value.stype);
-  if (!esz) {
-    set_error(std::string(fname) + " cannot be applied to columns of stype " + std::to_string(value.stype));
-    return DTB_ENOTIMPL;
-  }
-  if (ngroups < 0) { set_error("ngroups must be non-negative"); return DTB_EINVAL; }
-  if (!offsets) { set_error("offsets is NULL"); return DTB_EINVAL; }
-  if (nrows_value < 0) { set_error("nrows_value must be non-negative"); return DTB_EINVAL; }
-  if (!value.data && nrows_value > 0) { set_error("value column data is NULL"); return DTB_EINVAL; }
-  DTB_TRY(ensure_context());
-  if (ngroups == 0) return DTB_OK;
-  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
-  DevIn d_off;
-  int64_t n = 0;
-  DTB_TRY(bind_groupby(offsets, ngroups, true, s, d_off, n));
-  if (!out) { set_error("out is NULL"); return DTB_EINVAL; }
-  if (!order && n > nrows_value) { set_error("offsets cover more rows than the value column has"); return DTB_EINVAL; }
-  DevIn d_val, d_ord;
-  DTB_TRY(d_val.bind(value.data, (size_t)nrows_value * esz, s));
-  DTB_TRY(d_ord.bind(order, (size_t)n * (order_is64 ? 8 : 4), s));
-  const size_t out_bytes = (size_t)n * esz;
-  DevOut d_out; DTB_TRY(d_out.bind(out, out_bytes, s));
-  DevBuf scr;
-  if (fill) DTB_TRY(scr.alloc(cumulative_scratch_bytes(n), s));
-  {
-    ProfScope ps(fname, s);
-    if (fill)
-      DTB_TRY(launch_fillna(reverse, d_val.dptr, value.stype, nrows_value, d_ord.dptr, order_is64,
-                            (const int32_t*)d_off.dptr, ngroups, n, scr.p, d_out.dptr, s));
-    else
-      DTB_TRY(launch_shift(d_val.dptr, value.stype, nrows_value, d_ord.dptr, order_is64, (const int32_t*)d_off.dptr,
-                           ngroups, n, shift, d_out.dptr, s));
-  }
-  if (d_out.staged()) {
-    DTB_TRY(d_out.finish(out_bytes, s));
-    DTB_CUDA_CHECK(cudaStreamSynchronize(s));
-  }
-  return DTB_OK;
+  return c.finish();
 }
 
 int dtb_shift(dtb_col value, int64_t nrows_value, const void* order, int order_is64, const void* offsets,
               int64_t ngroups, int64_t n, dtb_stream stream, void* out)
 {
-  return value_row_fn(false, 0, n, value, nrows_value, order, order_is64, offsets, ngroups, stream, out);
+  Grouped c(stream, {value}, nrows_value, order, order_is64, offsets, ngroups, out);
+  DTB_TRY(fixed_width(value.stype, "shift"));
+  c.within_column = c.per_position = true;
+  DTB_TRY(c.open(stype_bytes(value.stype)));
+  if (c.ngroups == 0) return DTB_OK;
+  {
+    ProfScope ps("shift", c.s);
+    DTB_TRY(launch_shift(c.val[0].dptr, value.stype, nrows_value, c.ord.dptr, order_is64, c.offs(), ngroups, c.n, n,
+                         c.dout.dptr, c.s));
+  }
+  return c.finish();
 }
 
 int dtb_fillna(int reverse, dtb_col value, int64_t nrows_value, const void* order, int order_is64,
                const void* offsets, int64_t ngroups, dtb_stream stream, void* out)
 {
-  return value_row_fn(true, reverse, 0, value, nrows_value, order, order_is64, offsets, ngroups, stream, out);
+  Grouped c(stream, {value}, nrows_value, order, order_is64, offsets, ngroups, out);
+  DTB_TRY(fixed_width(value.stype, "fillna"));
+  c.within_column = c.per_position = true;
+  DTB_TRY(c.open(stype_bytes(value.stype)));
+  if (c.ngroups == 0) return DTB_OK;
+  DevBuf scr; DTB_TRY(scr.alloc(cumulative_scratch_bytes(c.n), c.s));
+  {
+    ProfScope ps("fillna", c.s);
+    DTB_TRY(launch_fillna(reverse, c.val[0].dptr, value.stype, nrows_value, c.ord.dptr, order_is64, c.offs(), ngroups,
+                          c.n, scr.p, c.dout.dptr, c.s));
+  }
+  return c.finish();
 }
 
 int dtb_group_index(int kind, int reverse, const void* offsets, int64_t ngroups, dtb_stream stream, void* out)
 {
-  cudaStream_t s = (cudaStream_t)stream;
-  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
+  Grouped c(stream, {}, 0, nullptr, 0, offsets, ngroups, out);
   if (kind != DTB_GROUP_CUMCOUNT && kind != DTB_GROUP_NGROUP) {
     set_error("dtb_group_index takes DTB_GROUP_CUMCOUNT or DTB_GROUP_NGROUP"); return DTB_EINVAL;
   }
-  if (ngroups < 0) { set_error("ngroups must be non-negative"); return DTB_EINVAL; }
-  if (!offsets) { set_error("offsets is NULL"); return DTB_EINVAL; }
-  DTB_TRY(ensure_context());
-  if (ngroups == 0) return DTB_OK;
-  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
-  DevIn d_off;
-  int64_t n = 0;
-  DTB_TRY(bind_groupby(offsets, ngroups, true, s, d_off, n));
-  if (!out) { set_error("out is NULL"); return DTB_EINVAL; }
-  const size_t out_bytes = (size_t)n * sizeof(int64_t);
-  DevOut d_out; DTB_TRY(d_out.bind(out, out_bytes, s));
+  c.per_position = true;
+  DTB_TRY(c.open(sizeof(int64_t)));
+  if (c.ngroups == 0) return DTB_OK;
   {
-    ProfScope ps("group_index", s);
-    DTB_TRY(launch_group_index(kind, reverse, (const int32_t*)d_off.dptr, ngroups, n, (int64_t*)d_out.dptr, s));
+    ProfScope ps("group_index", c.s);
+    DTB_TRY(launch_group_index(kind, reverse, c.offs(), ngroups, c.n, (int64_t*)c.dout.dptr, c.s));
   }
-  if (d_out.staged()) {
-    DTB_TRY(d_out.finish(out_bytes, s));
-    DTB_CUDA_CHECK(cudaStreamSynchronize(s));
-  }
-  return DTB_OK;
+  return c.finish();
 }
 
 int dtb_groupby_reduce_begin(dtb_groupby* g, int op, int value_stype, dtb_stream stream, dtb_reduce_state** out)
@@ -1656,7 +1642,6 @@ int dtb_gather(dtb_col src, int64_t nrows_src, const void* order, int order_is64
                dtb_stream stream, void* out)
 {
   cudaStream_t s = (cudaStream_t)stream;
-  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
   t_stats = dtb_call_stats{0, 0, 0, 0, 0};
   const int esz = stype_bytes(src.stype);
   if (!esz) { set_error("Unable to gather Column of stype " + std::to_string(src.stype)); return DTB_ENOTIMPL; }
@@ -1664,6 +1649,7 @@ int dtb_gather(dtb_col src, int64_t nrows_src, const void* order, int order_is64
   if (n > 0 && (!order || !out)) { set_error("order/out is NULL"); return DTB_EINVAL; }
   DTB_TRY(ensure_context());
   if (n == 0) return DTB_OK;
+  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
   DevIn d_src, d_ord;
   DTB_TRY(d_src.bind(src.data, (size_t)nrows_src * esz, s));
   DTB_TRY(d_ord.bind(order, (size_t)n * (order_is64 ? 8 : 4), s));
@@ -1751,70 +1737,38 @@ static int group_by_value(dtb_col value, int64_t nrows_value, const void* order,
 int dtb_sort_grouped(dtb_col value, int64_t nrows_value, const void* order, const void* offsets, int64_t ngroups,
                      dtb_stream stream, void* order_out)
 {
-  cudaStream_t s = (cudaStream_t)stream;
-  const int esz = stype_bytes(value.stype);
-  if (!esz) { set_error("Unable to sort Column of stype " + std::to_string(value.stype)); return DTB_ENOTIMPL; }
-  if (ngroups < 0 || !offsets) { set_error("bad dtb_sort_grouped arguments"); return DTB_EINVAL; }
-  DTB_TRY(ensure_context());
-  if (ngroups == 0) return DTB_OK;
-  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
-  DevIn d_off; DTB_TRY(d_off.bind(offsets, sizeof(int32_t) * (size_t)(ngroups + 1), s));
-  int32_t n32 = 0;
-  DTB_CUDA_CHECK(cudaMemcpyAsync(&n32, (const int32_t*)d_off.dptr + ngroups, sizeof(int32_t), cudaMemcpyDefault, s));
-  DTB_CUDA_CHECK(cudaStreamSynchronize(s));
-  const int64_t n = n32;
-  if (n == 0) return DTB_OK;
-  if (!order_out) { set_error("order_out is NULL"); return DTB_EINVAL; }
-  DevIn d_val, d_ord;
-  DTB_TRY(d_val.bind(value.data, (size_t)nrows_value * esz, s));
-  DTB_TRY(d_ord.bind(order, (size_t)n * 4, s));
-  DevOut d_out; DTB_TRY(d_out.bind(order_out, (size_t)n * 4, s));
+  Grouped c(stream, {value}, nrows_value, order, 0, offsets, ngroups, order_out);
+  if (!stype_supported(value.stype)) { set_error("Unable to sort Column of stype " + std::to_string(value.stype)); return DTB_ENOTIMPL; }
+  c.per_position = true;
+  DTB_TRY(c.open(sizeof(int32_t)));
+  if (c.ngroups == 0) return DTB_OK;
   GroupedByValue gv;
-  DTB_TRY(group_by_value(dtb_col{d_val.dptr, value.stype, 0}, nrows_value, d_ord.dptr, (const int32_t*)d_off.dptr,
-                         ngroups, n, DTB_FLAG_SORT_ONLY, s, gv));
+  DTB_TRY(group_by_value(dtb_col{c.val[0].dptr, value.stype, 0}, nrows_value, c.ord.dptr, c.offs(), ngroups, c.n,
+                         DTB_FLAG_SORT_ONLY, c.s, gv));
   // positions -> rows
-  DTB_TRY(launch_gather(gv.ord, DTB_STYPE_INT32, n, gv.res.order.p, 0, n, d_out.dptr, s));
-  if (d_out.staged()) DTB_TRY(d_out.finish((size_t)n * 4, s));
-  DTB_CUDA_CHECK(cudaStreamSynchronize(s));
-  return DTB_OK;
+  DTB_TRY(launch_gather(gv.ord, DTB_STYPE_INT32, c.n, gv.res.order.p, 0, c.n, c.dout.dptr, c.s));
+  return c.finish(true);
 }
 
 int dtb_qcut(dtb_col value, int64_t nrows_value, const void* order, const void* offsets, int64_t ngroups,
              int nquantiles, dtb_stream stream, void* out)
 {
-  cudaStream_t s = (cudaStream_t)stream;
-  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
-  const int esz = stype_bytes(value.stype);
-  if (!esz) { set_error("qcut() cannot be applied to columns of stype " + std::to_string(value.stype)); return DTB_ENOTIMPL; }
+  Grouped c(stream, {value}, nrows_value, order, 0, offsets, ngroups, out);
   if (nquantiles <= 0) {
     set_error("Number of quantiles must be positive, instead got: " + std::to_string(nquantiles)); return DTB_EINVAL;
   }
-  if (ngroups < 0) { set_error("ngroups must be non-negative"); return DTB_EINVAL; }
-  if (!offsets) { set_error("offsets is NULL"); return DTB_EINVAL; }
-  if (nrows_value < 0) { set_error("nrows_value must be non-negative"); return DTB_EINVAL; }
-  if (!value.data && nrows_value > 0) { set_error("value column data is NULL"); return DTB_EINVAL; }
-  DTB_TRY(ensure_context());
-  if (ngroups == 0) return DTB_OK;
-  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
-  DevIn d_off;
-  int64_t n = 0;
-  DTB_TRY(bind_groupby(offsets, ngroups, true, s, d_off, n));
-  if (!out) { set_error("out is NULL"); return DTB_EINVAL; }
-  if (!order && n > nrows_value) { set_error("offsets cover more rows than the value column has"); return DTB_EINVAL; }
-  DevIn d_val, d_ord;
-  DTB_TRY(d_val.bind(value.data, (size_t)nrows_value * esz, s));
-  DTB_TRY(d_ord.bind(order, (size_t)n * 4, s));
-  DevOut d_out; DTB_TRY(d_out.bind(out, (size_t)n * 4, s));
+  DTB_TRY(fixed_width(value.stype, "qcut()"));
+  c.within_column = c.per_position = true;
+  DTB_TRY(c.open(sizeof(int32_t)));
+  if (c.ngroups == 0) return DTB_OK;
   GroupedByValue gv;
-  DTB_TRY(group_by_value(dtb_col{d_val.dptr, value.stype, 0}, nrows_value, d_ord.dptr, (const int32_t*)d_off.dptr,
-                         ngroups, n, 0, s, gv));
+  DTB_TRY(group_by_value(dtb_col{c.val[0].dptr, value.stype, 0}, nrows_value, c.ord.dptr, c.offs(), ngroups, c.n, 0,
+                         c.s, gv));
   const int64_t nc = gv.res.ngroups;
-  DevBuf scr; DTB_TRY(scr.alloc(qcut_scratch_bytes(nc, ngroups), s));
+  DevBuf scr; DTB_TRY(scr.alloc(qcut_scratch_bytes(nc, ngroups), c.s));
   DTB_TRY(launch_qcut(gv.vg.p, value.stype, gv.res.order.as<int32_t>(), gv.res.offsets.as<int32_t>(), nc,
-                      gv.gid.as<int32_t>(), ngroups, n, nquantiles, scr.p, (int32_t*)d_out.dptr, s));
-  if (d_out.staged()) DTB_TRY(d_out.finish((size_t)n * 4, s));
-  DTB_CUDA_CHECK(cudaStreamSynchronize(s));
-  return DTB_OK;
+                      gv.gid.as<int32_t>(), ngroups, c.n, nquantiles, scr.p, (int32_t*)c.dout.dptr, c.s));
+  return c.finish(true);
 }
 
 int dtb_set_select(int mode, const void* order, const void* offsets, int64_t ngroups, const int64_t* cum_sizes,

@@ -93,6 +93,44 @@ def _alloc(n, st, device):
     return a, a.ctypes.data
 
 
+def _out_stype(query, op, *stypes, fn="reducer"):
+    """query(op, *stypes): the output stype of function `fn` op over columns of `stypes`; DtbValueError when the
+    library refuses them (0)."""
+    out_st = query(op, *stypes)
+    if not out_st:
+        cols = (f"column of stype {stypes[0]}" if len(stypes) == 1
+                else "columns of stypes " + ", ".join(str(s) for s in stypes))
+        raise _lib.DtbValueError(f"Invalid {cols} in {fn} {op}")
+    return out_st
+
+
+class _Grouped:
+    """The arguments of a per-group function: value columns seen through the RowIndex `order` (None = identity; int32,
+    or also int64 when wide_order) and cut by the Groupby `offsets`.  device: every input is in HBM.  The object owns
+    the contiguous copies that Col makes of strided or list inputs: keep it alive until the library call returns."""
+
+    def __init__(self, values, order, offsets, wide_order=True):
+        self._offsets = offsets
+        self._f = f = Col(offsets)
+        self.ngroups = f.nrows - 1
+        self.offsets = ctypes.c_void_p(f.ptr)
+        self.offsets_on_device = f.on_device
+        self._o = o = None if order is None else Col(order)
+        if o is not None and o.stype not in ((INT32, INT64) if wide_order else (INT32,)):
+            raise _lib.DtbValueError("order must be int32 or int64" if wide_order else "order must be int32")
+        self.order = None if o is None else ctypes.c_void_p(o.ptr)
+        self.order_is64 = 1 if o is not None and o.stype == INT64 else 0
+        self.device = all(c.on_device for c in values) and f.on_device and (o is None or o.on_device)
+
+    @property
+    def n(self):
+        """Positions of the RowIndex, offsets[-1]: read from HBM when the offsets are there, so only when needed."""
+        if self.ngroups <= 0:
+            return 0
+        last = self._offsets[-1]
+        return int(last.item() if is_tensor(last) else last)
+
+
 def _keys(cols, flags):
     """Key columns and flags as the C-ABI takes them: (cols, nrows, flags, ckeys, cflags).  The library reads
     nrows rows of every key column, so they must all have that many."""
@@ -185,9 +223,7 @@ class Groupby:
                     self._red.append((_lib.OP_NROWS, INT64, None))
                 else:
                     v = Col(val)
-                    out_st = lib.dtb_reduce_out_stype(op, v.stype)
-                    if not out_st:
-                        raise _lib.DtbValueError(f"Invalid column of stype {v.stype} in reducer {op}")
+                    out_st = _out_stype(lib.dtb_reduce_out_stype, op, v.stype)
                     specs[i] = _lib.dtb_reduce_spec(op, 0, v.c())
                     self._red.append((op, out_st, v))
             check(lib.dtb_groupby_create_reduce(ckeys, nk, cflags, na_pos, n, _stream(), specs, len(reducers),
@@ -207,9 +243,7 @@ class Groupby:
             out_st = INT64
         else:
             v = Col(value)
-            out_st = lib.dtb_reduce_out_stype(op, v.stype)
-        if not out_st:
-            raise _lib.DtbValueError(f"Invalid column of stype {v.stype} in reducer {op}")
+            out_st = _out_stype(lib.dtb_reduce_out_stype, op, v.stype)
         if out is None:
             out, optr = _alloc(self.ngroups, out_st, v.on_device)
         else:
@@ -221,9 +255,7 @@ class Groupby:
         """The reducer fed piecewise (dtb_groupby_reduce_begin / _add / _end).  pieces: [(CUDA tensor with rows
         [row0, row0 + len), row0, CUDA event to wait for or None), ...] covering every row once.  Returns the result
         (CUDA tensor) or None when the handle has no streaming path for this reducer (use reduce())."""
-        out_st = lib.dtb_reduce_out_stype(op, stype)
-        if not out_st:
-            raise _lib.DtbValueError(f"Invalid column of stype {stype} in reducer {op}")
+        out_st = _out_stype(lib.dtb_reduce_out_stype, op, stype)
         st = ctypes.c_void_p(0)
         rc = lib.dtb_groupby_reduce_begin(self._h, op, stype, _stream(), ctypes.byref(st))
         if rc == _lib.ENOTIMPL:
@@ -255,9 +287,7 @@ class Groupby:
         cx, cy = Col(x), Col(y)
         if cx.nrows != cy.nrows:
             raise _lib.DtbValueError("cov / corr need two columns of the same length")
-        out_st = reduce2_out_stype(op, cx.stype, cy.stype)
-        if not out_st:
-            raise _lib.DtbValueError(f"Invalid columns of stypes {cx.stype}, {cy.stype} in reducer {op}")
+        out_st = _out_stype(lib.dtb_reduce2_out_stype, op, cx.stype, cy.stype)
         if out is None:
             out, optr = _alloc(self.ngroups, out_st, cx.on_device and cy.on_device)
         else:
@@ -277,9 +307,7 @@ class Groupby:
     def reduce_ordered(self, op, value, order):
         """Reducer over the handle's groups but another RowIndex (the output of sort_grouped)."""
         v = Col(value)
-        out_st = lib.dtb_reduce_out_stype(op, v.stype)
-        if not out_st:
-            raise _lib.DtbValueError(f"Invalid column of stype {v.stype} in reducer {op}")
+        out_st = _out_stype(lib.dtb_reduce_out_stype, op, v.stype)
         out, optr = _alloc(self.ngroups, out_st, True)
         check(lib.dtb_reduce(op, v.c(), v.nrows, ctypes.c_void_p(order.data_ptr()), 0, ctypes.c_void_p(self.offsets_ptr),
                              self.ngroups, _stream(), ctypes.c_void_p(optr)))
@@ -330,29 +358,14 @@ def reduce_out_stype(op, stype):
 
 
 def reduce(op, value, order, offsets, stype=None):
-    """Per-group reducer over `value` viewed through RowIndex `order` (None = identity)."""
-    ngroups = int(offsets.shape[0]) - 1
-    if op == _lib.OP_NROWS:
-        v = None
-        vst, vptr, vn, vdev = INT8, 0, 0, is_tensor(offsets) and offsets.is_cuda
-    else:
-        v = Col(value, stype)
-        vst, vptr, vn, vdev = v.stype, v.ptr, v.nrows, v.on_device
-    out_st = lib.dtb_reduce_out_stype(op, vst)
-    if not out_st:
-        raise _lib.DtbValueError(f"Invalid column of stype {vst} in reducer {op}")
-    out, optr = _alloc(ngroups, out_st, vdev)
-    o = None if order is None else Col(order)
-    f = Col(offsets)
-    is64 = 0
-    if o is not None:
-        if o.stype == INT64:
-            is64 = 1
-        elif o.stype != INT32:
-            raise _lib.DtbValueError("order must be int32 or int64")
-    check(lib.dtb_reduce(op, dtb_col(ctypes.c_void_p(vptr), vst, 0), vn,
-                         ctypes.c_void_p(o.ptr) if o is not None else None, is64,
-                         ctypes.c_void_p(f.ptr), ngroups, _stream(), ctypes.c_void_p(optr)))
+    """Per-group reducer over `value` viewed through RowIndex `order` (None = identity); the result is in HBM when
+    `value` is (with OP_NROWS, when `offsets` is)."""
+    v = Col.from_ptr(0, INT8, 0, on_device=False) if op == _lib.OP_NROWS else Col(value, stype)
+    out_st = _out_stype(lib.dtb_reduce_out_stype, op, v.stype)
+    g = _Grouped([v], order, offsets)
+    out, optr = _alloc(g.ngroups, out_st, g.offsets_on_device if op == _lib.OP_NROWS else v.on_device)
+    check(lib.dtb_reduce(op, v.c(), v.nrows, g.order, g.order_is64, g.offsets, g.ngroups, _stream(),
+                         ctypes.c_void_p(optr)))
     return out
 
 
@@ -362,21 +375,14 @@ def reduce2_out_stype(op, stype_x, stype_y):
 
 def reduce2(op, x, y, order, offsets, stype_x=None, stype_y=None):
     """cov / corr (OP_COV / OP_CORR) per group of the columns x and y viewed through RowIndex `order` (None =
-    identity; int32 or int64), segmented by `offsets` (dtb_reduce2)."""
-    ngroups = int(offsets.shape[0]) - 1
+    identity; int32 or int64), segmented by `offsets` (dtb_reduce2); in HBM when x and y are."""
     cx, cy = Col(x, stype_x), Col(y, stype_y)
     if cx.nrows != cy.nrows:
         raise _lib.DtbValueError("cov / corr need two columns of the same length")
-    out_st = reduce2_out_stype(op, cx.stype, cy.stype)
-    if not out_st:
-        raise _lib.DtbValueError(f"Invalid columns of stypes {cx.stype}, {cy.stype} in reducer {op}")
-    out, optr = _alloc(ngroups, out_st, cx.on_device and cy.on_device)
-    o = None if order is None else Col(order)
-    if o is not None and o.stype not in (INT32, INT64):
-        raise _lib.DtbValueError("order must be int32 or int64")
-    f = Col(offsets)
-    check(lib.dtb_reduce2(op, cx.c(), cy.c(), cx.nrows, ctypes.c_void_p(o.ptr) if o is not None else None,
-                          1 if o is not None and o.stype == INT64 else 0, ctypes.c_void_p(f.ptr), ngroups, _stream(),
+    out_st = _out_stype(lib.dtb_reduce2_out_stype, op, cx.stype, cy.stype)
+    g = _Grouped([cx, cy], order, offsets)
+    out, optr = _alloc(g.ngroups, out_st, cx.on_device and cy.on_device)
+    check(lib.dtb_reduce2(op, cx.c(), cy.c(), cx.nrows, g.order, g.order_is64, g.offsets, g.ngroups, _stream(),
                           ctypes.c_void_p(optr)))
     return out
 
@@ -401,16 +407,9 @@ def sort_grouped(value, order, offsets, stype=None):
     """Column::sort_grouped (sort.cc:1499-1530): reorder the rows inside every group of (order, offsets)
     by `value` ascending, NA first, stable.  Returns the new int32 RowIndex (median / nunique read it)."""
     v = Col(value, stype)
-    f = Col(offsets)
-    ngroups = f.nrows - 1
-    o = None if order is None else Col(order)
-    if o is not None and o.stype != INT32:
-        raise _lib.DtbValueError("order must be int32")
-    n = int(offsets[-1].item()) if is_tensor(offsets) else int(offsets[-1])
-    device = v.on_device and f.on_device and (o is None or o.on_device)
-    out, optr = _alloc(n, INT32, device)
-    check(lib.dtb_sort_grouped(v.c(), v.nrows, ctypes.c_void_p(o.ptr) if o is not None else None,
-                               ctypes.c_void_p(f.ptr), ngroups, _stream(), ctypes.c_void_p(optr)))
+    g = _Grouped([v], order, offsets, wide_order=False)
+    out, optr = _alloc(g.n, INT32, g.device)
+    check(lib.dtb_sort_grouped(v.c(), v.nrows, g.order, g.offsets, g.ngroups, _stream(), ctypes.c_void_p(optr)))
     return out
 
 
@@ -419,18 +418,11 @@ def qcut(value, order, offsets, nquantiles=10, stype=None):
     (expr/fexpr_qcut.cc:118-146); one group [0, n] without by().  Returns the int32 bins, one per position of the
     RowIndex (order None = identity), NA as INT32_MIN; in HBM when the inputs are."""
     v = Col(value, stype)
-    f = Col(offsets)
-    ngroups = f.nrows - 1
-    o = None if order is None else Col(order)
-    if o is not None and o.stype != INT32:
-        raise _lib.DtbValueError("order must be int32")
+    g = _Grouped([v], order, offsets, wide_order=False)
     if not -2**31 <= int(nquantiles) < 2**31:
         raise _lib.DtbValueError(f"nquantiles does not fit in an int32: {nquantiles}")
-    n = (int(offsets[-1].item()) if is_tensor(offsets) else int(offsets[-1])) if ngroups > 0 else 0
-    device = v.on_device and f.on_device and (o is None or o.on_device)
-    out, optr = _alloc(n, INT32, device)
-    check(lib.dtb_qcut(v.c(), v.nrows, ctypes.c_void_p(o.ptr) if o is not None else None, ctypes.c_void_p(f.ptr),
-                       ngroups, int(nquantiles), _stream(), ctypes.c_void_p(optr)))
+    out, optr = _alloc(g.n, INT32, g.device)
+    check(lib.dtb_qcut(v.c(), v.nrows, g.order, g.offsets, g.ngroups, int(nquantiles), _stream(), ctypes.c_void_p(optr)))
     return out
 
 
@@ -444,34 +436,12 @@ def cumulative(op, value, order, offsets, reverse=False, stype=None):
     `order`: None = identity, int32 or int64.  Returns one value per position of the RowIndex, of stype
     cumulative_out_stype(op, stype); in HBM when the inputs are."""
     v = Col(value, stype)
-    f = Col(offsets)
-    ngroups = f.nrows - 1
-    out_st = cumulative_out_stype(op, v.stype)
-    if not out_st:
-        raise _lib.DtbValueError(f"Invalid column of stype {v.stype} in cumulative function {op}")
-    o = None if order is None else Col(order)
-    if o is not None and o.stype not in (INT32, INT64):
-        raise _lib.DtbValueError("order must be int32 or int64")
-    n = (int(offsets[-1].item()) if is_tensor(offsets) else int(offsets[-1])) if ngroups > 0 else 0
-    device = v.on_device and f.on_device and (o is None or o.on_device)
-    out, optr = _alloc(n, out_st, device)
-    check(lib.dtb_cumulative(op, 1 if reverse else 0, v.c(), v.nrows, ctypes.c_void_p(o.ptr) if o is not None else None,
-                             1 if o is not None and o.stype == INT64 else 0, ctypes.c_void_p(f.ptr), ngroups, _stream(),
-                             ctypes.c_void_p(optr)))
+    out_st = _out_stype(lib.dtb_cumulative_out_stype, op, v.stype, fn="cumulative function")
+    g = _Grouped([v], order, offsets)
+    out, optr = _alloc(g.n, out_st, g.device)
+    check(lib.dtb_cumulative(op, 1 if reverse else 0, v.c(), v.nrows, g.order, g.order_is64, g.offsets, g.ngroups,
+                             _stream(), ctypes.c_void_p(optr)))
     return out
-
-
-def _row_fn_args(value, order, offsets, stype):
-    """(Col value, Col offsets, ngroups, Col order or None, positions, device) of a row function of (order, offsets)."""
-    v = Col(value, stype)
-    f = Col(offsets)
-    ngroups = f.nrows - 1
-    o = None if order is None else Col(order)
-    if o is not None and o.stype not in (INT32, INT64):
-        raise _lib.DtbValueError("order must be int32 or int64")
-    n = (int(offsets[-1].item()) if is_tensor(offsets) else int(offsets[-1])) if ngroups > 0 else 0
-    device = v.on_device and f.on_device and (o is None or o.on_device)
-    return v, f, ngroups, o, n, device
 
 
 def shift(value, order, offsets, n=1, stype=None):
@@ -479,11 +449,11 @@ def shift(value, order, offsets, n=1, stype=None):
     group [0, nrows] is Shift_ColumnImpl without by().  Position p takes the value at position p - n of its group, NA
     where that lies outside the group.  `order`: None = identity, int32 or int64.  Returns one value per position of
     the RowIndex, of the value's stype; in HBM when the inputs are."""
-    v, f, ngroups, o, npos, device = _row_fn_args(value, order, offsets, stype)
-    out, optr = _alloc(npos, v.stype, device)
-    check(lib.dtb_shift(v.c(), v.nrows, ctypes.c_void_p(o.ptr) if o is not None else None,
-                        1 if o is not None and o.stype == INT64 else 0, ctypes.c_void_p(f.ptr), ngroups, int(n),
-                        _stream(), ctypes.c_void_p(optr)))
+    v = Col(value, stype)
+    g = _Grouped([v], order, offsets)
+    out, optr = _alloc(g.n, v.stype, g.device)
+    check(lib.dtb_shift(v.c(), v.nrows, g.order, g.order_is64, g.offsets, g.ngroups, int(n), _stream(),
+                        ctypes.c_void_p(optr)))
     return out
 
 
@@ -492,10 +462,10 @@ def fillna(value, order, offsets, reverse=False, stype=None):
     latest valid value at or before every position (reverse: the earliest at or after), NA before the first.  `order`:
     None = identity, int32 or int64.  Returns one value per position of the RowIndex, of the value's stype; in HBM
     when the inputs are."""
-    v, f, ngroups, o, npos, device = _row_fn_args(value, order, offsets, stype)
-    out, optr = _alloc(npos, v.stype, device)
-    check(lib.dtb_fillna(1 if reverse else 0, v.c(), v.nrows, ctypes.c_void_p(o.ptr) if o is not None else None,
-                         1 if o is not None and o.stype == INT64 else 0, ctypes.c_void_p(f.ptr), ngroups, _stream(),
+    v = Col(value, stype)
+    g = _Grouped([v], order, offsets)
+    out, optr = _alloc(g.n, v.stype, g.device)
+    check(lib.dtb_fillna(1 if reverse else 0, v.c(), v.nrows, g.order, g.order_is64, g.offsets, g.ngroups, _stream(),
                          ctypes.c_void_p(optr)))
     return out
 
@@ -504,12 +474,9 @@ def group_index(kind, offsets, reverse=False):
     """cumcount (GROUP_CUMCOUNT: the position inside the group) or ngroup (GROUP_NGROUP: the group's index) for every
     position of the groups `offsets`, as CumcountNgroup_ColumnImpl (dtb_group_index); reverse counts from the other
     end.  Returns int64[offsets[-1]]; in HBM when `offsets` is."""
-    f = Col(offsets)
-    ngroups = f.nrows - 1
-    n = (int(offsets[-1].item()) if is_tensor(offsets) else int(offsets[-1])) if ngroups > 0 else 0
-    out, optr = _alloc(n, INT64, f.on_device)
-    check(lib.dtb_group_index(kind, 1 if reverse else 0, ctypes.c_void_p(f.ptr), ngroups, _stream(),
-                              ctypes.c_void_p(optr)))
+    g = _Grouped([], None, offsets)
+    out, optr = _alloc(g.n, INT64, g.offsets_on_device)
+    check(lib.dtb_group_index(kind, 1 if reverse else 0, g.offsets, g.ngroups, _stream(), ctypes.c_void_p(optr)))
     return out
 
 

@@ -21,7 +21,8 @@
  *     thread-local message (the reference throws dt::Error subclasses,
  *     utils/exceptions.h:43; a C ABI must not throw).
  *   - there is NO CPU fallback: without a usable CUDA device every compute
- *     call fails with DTB_ECUDA.
+ *     call fails with DTB_ECUDA once its arguments pass the checks that need
+ *     no device.
  */
 #ifndef DTB200_H
 #define DTB200_H
@@ -202,10 +203,30 @@ DTB_API const void* dtb_groupby_offsets(const dtb_groupby* g);   /* device int32
 DTB_API int         dtb_groupby_destroy(dtb_groupby* g, dtb_stream stream);
 
 /*
+ * Per-group functions: dtb_reduce, dtb_reduce2, dtb_cumulative, dtb_shift, dtb_fillna, dtb_group_index, dtb_qcut,
+ * dtb_sort_grouped, and the handle variants dtb_groupby_reduce / dtb_groupby_reduce2, share one argument contract.
+ * The value columns hold nrows_value rows each and are seen through the RowIndex `order` (NULL = identity;
+ * order_is64: int64 row ids, where the function takes them, else int32).  `offsets` (int32[ngroups+1]) cuts the
+ * n = offsets[ngroups] positions of the RowIndex into groups; a call without by() passes one group [0, n].  Every
+ * pointer may be host or device memory.  The arguments are checked in this order, all on the host before any CUDA
+ * call, so that without a device an argument error still returns its own code:
+ *   1. the function's own argument (op, kind, nquantiles): DTB_EINVAL;
+ *   2. the stype: one without a fixed width gives DTB_ENOTIMPL, one the op refuses DTB_EINVAL;
+ *   3. ngroups < 0;  4. offsets NULL;  5. nrows_value < 0;  6. value data NULL while nrows_value > 0;
+ *   7. out NULL while ngroups > 0: DTB_EINVAL.
+ * ngroups == 0 then returns at once.  Caller offsets must be a Groupby (groupby.h:41-47): offsets[0] = 0 and
+ * strictly increasing, so no group is empty; otherwise DTB_EINVAL (device offsets are checked on the device; a
+ * handle's own offsets are not checked).  Positions beyond the value column: without an order, n > nrows_value is
+ * DTB_EINVAL for the row functions (dtb_cumulative, dtb_shift, dtb_fillna, dtb_qcut); the reducers and
+ * dtb_sort_grouped read those positions as NA (nrows_value bounds the gather).
+ */
+
+/*
  * dtb_reduce -- replaces ColumnImpl::materialize() of the per-group reducer
  * columns (column/reduce_unary.h:30-68 driven by column/latent.cc:103-135 and
  * column/column_impl.cc:78-103): value column viewed through the RowIndex
- * `order` (NULL = identity), segmented by `offsets`.
+ * `order` (NULL = identity), segmented by `offsets`; arguments as in
+ * "Per-group functions" above.
  *
  *   out : ngroups elements of stype dtb_reduce_out_stype(op, value.stype);
  *         NA results are written as the stype's NA sentinel.
@@ -276,8 +297,8 @@ DTB_API int dtb_groupby_reduce_end(dtb_reduce_state* st, dtb_stream stream, void
 
 /*
  * dtb_reduce2 -- cov / corr per group (expr/head_reduce_binary.cc:114-221): the columns x and y, both viewed
- * through the RowIndex `order` (NULL = identity; order_is64: int64 row ids), segmented by `offsets`.  Host or device
- * pointers, offsets validated as dtb_reduce does.  nrows_value: rows in each of x and y (bounds the gather).
+ * through the RowIndex `order` (NULL = identity; order_is64: int64 row ids), segmented by `offsets`; arguments as in
+ * "Per-group functions".  nrows_value: rows in each of x and y (bounds the gather).
  *   out : ngroups elements of stype dtb_reduce2_out_stype(op, x.stype, y.stype): FLOAT32 when both columns are
  *         FLOAT32, FLOAT64 otherwise (bool and integer columns included); 0 = invalid combination.
  * Only rows where both values are valid count; m = their number.  COV is NA when m <= 1, else
@@ -300,9 +321,8 @@ DTB_API int dtb_groupby_reduce2(dtb_groupby* g, int op, dtb_col x, dtb_col y, in
  * dtb_cumulative -- cumsum / cumprod / cummin / cummax inside every group: replaces CumSumProd_ColumnImpl
  * (column/cumsumprod.h) and CumMinMax_ColumnImpl (column/cumminmax.h) as FExpr_CumSumProd / FExpr_CumMinMax run
  * them (expr/fexpr_cumsumprod.cc, expr/fexpr_cumminmax.cc).  op: DTB_OP_SUM, DTB_OP_PROD, DTB_OP_MIN or DTB_OP_MAX.
- * The value column is seen through `order` (NULL = identity; order_is64: int64 row ids) and cut by `offsets`
- * (int32[ngroups+1], a Groupby, validated as dtb_reduce validates it; one group [0, n] for a call without by()).
- * reverse != 0 scans every group from its last position to its first.  Host or device pointers.
+ * The value column is seen through `order` (NULL = identity; order_is64: int64 row ids) and cut by `offsets`;
+ * arguments as in "Per-group functions".  reverse != 0 scans every group from its last position to its first.
  *   out : offsets[ngroups] elements of stype dtb_cumulative_out_stype(op, value.stype), out[p] for position p of
  *         the RowIndex (the GtoALL layout of the grouped frame): SUM / PROD give INT64 for bool and int8-64 and keep FLOAT32 /
  *         FLOAT64; MIN / MAX keep the column's stype (bool, int8-64, float32/64, date32, time64).  0 = refused.
@@ -331,12 +351,9 @@ DTB_API int dtb_cumulative(int op, int reverse, dtb_col value, int64_t nrows_val
 /*
  * dtb_shift, dtb_fillna, dtb_group_index -- the row functions that return one value per position inside every group
  * (the GtoALL layout of the grouped frame).  Like dtb_cumulative, the value column is seen through `order` (NULL =
- * identity; order_is64: int64 row ids) and cut by `offsets` (int32[ngroups+1], a Groupby, validated as dtb_reduce
- * validates it; one group [0, n] for a call without by()), with host or device pointers; ngroups == 0 returns at once.
+ * identity; order_is64: int64 row ids) and cut by `offsets`; arguments as in "Per-group functions".
  * Up to INT32_MAX positions.  out holds offsets[ngroups] elements, out[p] for position p of the RowIndex.  Results
  * are deterministic: every output element is computed by one thread, so two calls give the same bytes.
- * Errors: an stype without a fixed width gives DTB_ENOTIMPL; a bad kind, negative ngroups, NULL offsets, or offsets
- * covering more rows than the column has without an order give DTB_EINVAL.
  *
  * dtb_shift: replaces compute_lag_rowindex (expr/head_func_shift.cc:40-64) and Shift_ColumnImpl (column/shift.h:37-88).
  *   out[p] = value[order[p - n]] when p - n lies in p's group, else NA: n > 0 lags, n < 0 leads, n = 0 gathers the
@@ -390,7 +407,8 @@ DTB_API int dtb_slice_groups(const void* offsets, int64_t ngroups, int64_t start
 /*
  * dtb_sort_grouped -- replaces Column::sort_grouped (sort.cc:1499-1530): reorders the rows INSIDE every
  * group of (order, offsets) by `value` ascending, NA first, stable; the groups themselves stay where
- * they are.  order_out: int32[offsets[ngroups]].  DTB_OP_MEDIAN / DTB_OP_NUNIQUE expect this order
+ * they are.  order: int32 RowIndex; arguments as in "Per-group functions", order_out is its `out`.
+ * order_out: int32[offsets[ngroups]].  DTB_OP_MEDIAN / DTB_OP_NUNIQUE expect this order
  * (the reference's Median_ColumnImpl calls sort_grouped in its pre_materialize_hook).
  */
 DTB_API int dtb_sort_grouped(dtb_col value, int64_t nrows_value, const void* order, const void* offsets,
@@ -399,8 +417,8 @@ DTB_API int dtb_sort_grouped(dtb_col value, int64_t nrows_value, const void* ord
 /*
  * dtb_qcut -- replaces Qcut_ColumnImpl::materialize (column/qcut.h:78-155) run on every group, as
  * FExpr_Qcut::evaluate_n does under by() (expr/fexpr_qcut.cc:64-158).  The value column is seen through `order`
- * (int32 RowIndex; NULL = identity) and cut by `offsets` (int32[ngroups+1], a Groupby: offsets[0] = 0, strictly
- * increasing; one group [0, n] for a call without by()).  Inside every group the distinct values are numbered
+ * (int32 RowIndex; NULL = identity) and cut by `offsets`; arguments as in "Per-group functions".  Inside every
+ * group the distinct values are numbered
  * i = 0 .. G-1 in group()'s order, NA first; has_na = the first one is NA, V = G - has_na, q = nquantiles:
  *   V <= 1:  a = 0, b = (q - 1) / 2 (integer division)
  *   else:    a = q * (1 - FLT_EPSILON) / (V - 1), b = -a * has_na
@@ -409,8 +427,7 @@ DTB_API int dtb_sort_grouped(dtb_col value, int64_t nrows_value, const void* ord
  *   - a * i + b is a multiply and an add, each rounded to nearest (no fused multiply-add), as the reference
  *     computes it.
  * out: int32[offsets[ngroups]], out[p] = the bin of the row at position p of the RowIndex (the GtoALL layout of
- * the grouped frame).  Host or device pointers.  nquantiles <= 0: DTB_EINVAL; an stype without a fixed width:
- * DTB_ENOTIMPL.  Up to INT32_MAX rows.
+ * the grouped frame).  nquantiles <= 0: DTB_EINVAL.  Up to INT32_MAX rows.
  */
 DTB_API int dtb_qcut(dtb_col value, int64_t nrows_value, const void* order, const void* offsets, int64_t ngroups,
                      int nquantiles, dtb_stream stream, void* out);
