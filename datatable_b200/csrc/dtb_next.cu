@@ -793,9 +793,9 @@ __global__ void join_kernel(JoinPlan jp, int64_t nx, int64_t nj, int32_t* __rest
       long long iv = 0; double dv = 0; bool isf = false;
       xvalid[c] = load_any(jp.c[c].x, jp.c[c].xst, r, iv, dv, isf);
       const bool jf = jp.c[c].jst == DTB_STYPE_FLOAT32 || jp.c[c].jst == DTB_STYPE_FLOAT64;
-      if (jf) {
-        xd[c] = isf ? dv : (double)iv;
-        if (jp.c[c].jst == DTB_STYPE_FLOAT32) xd[c] = (double)(float)xd[c];    // static_cast<TJ>(newval)
+      if (jf) {                                        // static_cast<TJ>(newval): one rounding, from X's own type
+        if (jp.c[c].jst == DTB_STYPE_FLOAT32) xd[c] = isf ? (double)(float)dv : (double)(float)iv;
+        else                                  xd[c] = isf ? dv : (double)iv;
       } else if (xvalid[c]) {
         long long lo, hi; int_range(jp.c[c].jst, lo, hi);
         if (isf) {

@@ -221,10 +221,8 @@ def join_index(xcols, xst, jcols, jst):
                 elif not (int_range[jst[c]][0] <= int(x) <= int_range[jst[c]][1]):
                     bad = True
                 x = int(x) if not bad else x
-            elif jst[c] == FLOAT32:
-                x = float(np.float32(x))
-            else:
-                x = float(x)
+            else:                                                 # static_cast<TJ>(newval): one rounding, from X's type
+                x = float(xcols[c][r:r + 1].astype(np.float32 if jst[c] == FLOAT32 else np.float64)[0])
             xv.append(x)
         if bad:
             continue
