@@ -1670,6 +1670,9 @@ int dtb_dense_scatter(const void* keys, int key_stype, const void* vals, int64_t
   const int kb = (key_stype == DTB_STYPE_INT32) ? 4 : (key_stype == DTB_STYPE_INT64 ? 8 : 0);
   if (!kb) { set_error("dense merge: group keys must be int32 or int64"); return DTB_ENOTIMPL; }
   if (n < 0 || table_size < 1 || (n > 0 && (!keys || !vals)) || !table || !present) { set_error("bad dtb_dense_scatter arguments"); return DTB_EINVAL; }
+  if (table_size % 1024 || table_size > ((int64_t)1 << 22)) {
+    set_error("dense merge: table size must be a multiple of 1024 and at most 2^22"); return DTB_EINVAL;
+  }
   if (!is_device_ptr(table) || !is_device_ptr(present) || (n > 0 && (!is_device_ptr(keys) || !is_device_ptr(vals)))) {
     set_error("dense merge works on device buffers (they are NCCL all-reduced in place)"); return DTB_EINVAL;
   }

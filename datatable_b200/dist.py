@@ -34,6 +34,19 @@ _MERGE_OP = {_lib.OP_SUM: _lib.OP_SUM, _lib.OP_MIN: _lib.OP_MIN, _lib.OP_MAX: _l
              _lib.OP_COUNT: _lib.OP_SUM, _lib.OP_NROWS: _lib.OP_SUM, _lib.OP_COUNTNA: _lib.OP_SUM}
 
 
+def _merge_op(op):
+    """The reducer that merges partials of `op`; refused before any work when the partials of `op` do not merge."""
+    if op not in _MERGE_OP:
+        raise _lib.DtbNotImplError(f"reducer {op} has no merge rule across ranks (sum, count, countna, nrows, min, max)")
+    return _MERGE_OP[op]
+
+
+def _bytes(x):
+    """The raw bytes of a 1-d tensor.  All-gathers and all-to-alls only move data; moving it as bytes lets every key
+    dtype travel on every backend (neither NCCL nor gloo has an int16 type)."""
+    return x.contiguous().view(torch.uint8)
+
+
 def local_groupby(k, v, op):
     """(group keys, partials) of this rank's partition; k, v are CUDA tensors."""
     order, offsets, ng = engine.group([k], [0], _lib.NA_FIRST)
@@ -43,15 +56,22 @@ def local_groupby(k, v, op):
     return gkeys, part
 
 
+def _dense_key_stype(dtype):
+    st = {torch.int32: _lib.INT32, torch.int64: _lib.INT64}.get(dtype)
+    if st is None:
+        raise _lib.DtbNotImplError(f"dense merge: group keys must be int32 or int64, not {dtype}")
+    return st
+
+
 def _dense_scatter(gkeys, part, kmin, table, present):
-    st = _lib.INT64 if gkeys.dtype == torch.int64 else _lib.INT32
+    st = _dense_key_stype(gkeys.dtype)
     _lib.check(_lib.lib.dtb_dense_scatter(ctypes.c_void_p(gkeys.data_ptr()), st, ctypes.c_void_p(part.data_ptr()),
                                           gkeys.numel(), int(kmin), table.numel(), ctypes.c_void_p(table.data_ptr()),
                                           ctypes.c_void_p(present.data_ptr()), engine._stream()))
 
 
 def _dense_compact(table, present, kmin, key_dtype):
-    st = _lib.INT64 if key_dtype == torch.int64 else _lib.INT32
+    st = _dense_key_stype(key_dtype)
     size = table.numel()
     out_k = torch.empty(size, dtype=key_dtype, device=table.device)
     out_v = torch.empty(size, dtype=table.dtype, device=table.device)
@@ -75,6 +95,7 @@ class _EngineKernels:
 
 def merge_partials(gkeys, part, op, group=None, kernels=_EngineKernels):
     """All-gather every rank's (key, partial) list and merge equal keys with the engine's kernels."""
+    mop = _merge_op(op)
     world = dist.get_world_size(group)
     if world == 1:
         return gkeys, part
@@ -87,13 +108,13 @@ def merge_partials(gkeys, part, op, group=None, kernels=_EngineKernels):
     ppad = torch.zeros(cap, dtype=part.dtype, device=part.device); ppad[:part.numel()] = part
     kall = torch.empty(world * cap, dtype=gkeys.dtype, device=gkeys.device)
     pall = torch.empty(world * cap, dtype=part.dtype, device=part.device)
-    dist.all_gather_into_tensor(kall, kpad, group=group)
-    dist.all_gather_into_tensor(pall, ppad, group=group)
+    dist.all_gather_into_tensor(_bytes(kall), _bytes(kpad), group=group)
+    dist.all_gather_into_tensor(_bytes(pall), _bytes(ppad), group=group)
     if any(sz != cap for sz in sizes_h):
         keep = torch.cat([torch.arange(r * cap, r * cap + sizes_h[r], device=gkeys.device) for r in range(world)])
         kall, pall = kall[keep].contiguous(), pall[keep].contiguous()
     order, offsets, ng = kernels.group(kall)
-    merged = kernels.reduce(_MERGE_OP[op], pall, order, offsets)
+    merged = kernels.reduce(mop, pall, order, offsets)
     first = kernels.take(order, offsets[:-1])
     return kernels.take(kall, first), merged
 
@@ -111,50 +132,70 @@ def merge_partials_dense(gkeys, part, op, group=None, kernels=_EngineKernels, ke
     column); without it one small all-reduce learns the global range (two scalars: the only extra host
     round trip).  The partial table and the presence table travel in ONE all-reduce (presence as 0/1 in
     the partials' dtype).  Falls back to `merge_partials` for MIN/MAX partials (NA partials do not
-    all-reduce) and for key ranges beyond DENSE_MAX."""
+    all-reduce), for float keys and for key ranges beyond DENSE_MAX.  int8 / int16 / bool keys go through the
+    tables as int32.  An empty or inverted key_range, or a key outside it, raises DtbValueError on every rank."""
     global LAST_MERGE_LAUNCHES
+    _merge_op(op)
+    if key_range is not None and int(key_range[1]) < int(key_range[0]):
+        raise _lib.DtbValueError(f"key_range {tuple(key_range)} is empty")
     world = dist.get_world_size(group)
     if world == 1:
         LAST_MERGE_LAUNCHES = 0
         return gkeys, part
     dev = gkeys.device
+    if gkeys.dtype.is_floating_point or op not in _SUM_LIKE or part.element_size() != 8:
+        LAST_MERGE_LAUNCHES = 8      # decided from what every rank shares: no range collective
+        return merge_partials(gkeys, part, op, group, kernels)
+    keys = gkeys if gkeys.dtype in (torch.int32, torch.int64) else gkeys.to(torch.int32)
     if key_range is not None:
         kmin, hi = int(key_range[0]), int(key_range[1])
     else:
         big = torch.iinfo(torch.int64).max
-        if gkeys.numel():
-            rng = torch.stack([-gkeys[0].to(torch.int64), gkeys[-1].to(torch.int64)])
+        if keys.numel():
+            # -(-2^63) wraps: clamp the int64 NA key first, so that it makes the span too large for a table
+            rng = torch.stack([-keys[0].to(torch.int64).clamp_min(-big), keys[-1].to(torch.int64)])
         else:
             rng = torch.tensor([-big, -big], dtype=torch.int64, device=dev)
         dist.all_reduce(rng, op=dist.ReduceOp.MAX, group=group)
         neg_lo, hi = rng.tolist()
         kmin = -neg_lo
     span = hi - kmin + 1
-    if op not in _SUM_LIKE or part.element_size() != 8 or span > DENSE_MAX or span <= 0:
+    if span > DENSE_MAX or span <= 0:
         LAST_MERGE_LAUNCHES = 8
         return merge_partials(gkeys, part, op, group, kernels) if span > 0 else (gkeys, part)
     size = (span + 1023) // 1024 * 1024
-    both = torch.zeros(2 * size, dtype=part.dtype, device=dev)        # [partials | presence], one collective
+    both = torch.zeros(2 * size + 1, dtype=part.dtype, device=dev)    # [partials | presence | keys out of range]
     table = both[:size]
     present = torch.zeros(size, dtype=torch.int32, device=dev)
-    kernels.dense_scatter(gkeys, part, kmin, table, present)
-    both[size:] = present                                             # 0 / 1 in the partials' dtype
+    kernels.dense_scatter(keys, part, kmin, table, present)
+    both[size:2 * size] = present                                     # 0 / 1 in the partials' dtype
+    if key_range is not None:                                         # the scatter drops them: count them instead
+        info = torch.iinfo(keys.dtype)
+        if kmin > info.max or hi < info.min:
+            both[2 * size] = keys.numel()
+        else:
+            both[2 * size] = ((keys < max(kmin, info.min)) | (keys > min(hi, info.max))).sum()
     dist.all_reduce(both, op=dist.ReduceOp.SUM, group=group)
-    present = (both[size:] != 0).to(torch.int32)
+    present = (both[size:2 * size] != 0).to(torch.int32)
     LAST_MERGE_LAUNCHES = 5          # scatter + block sums + scan + compact + emit
-    return kernels.dense_compact(table, present, kmin, gkeys.dtype)
+    mk, mv = kernels.dense_compact(table, present, kmin, keys.dtype)
+    if key_range is not None and both[2 * size].item() != 0:          # dtb_dense_compact has synchronised
+        raise _lib.DtbValueError(f"{int(both[2 * size].item())} group keys lie outside key_range {tuple(key_range)}")
+    return (mk if mk.dtype == gkeys.dtype else mk.to(gkeys.dtype)), mv
 
 
-def groupby_partitioned(k, v, op=_lib.OP_SUM, group=None, exchange="allgather"):
+def groupby_partitioned(k, v, op=_lib.OP_SUM, group=None, exchange="allgather", key_range=None):
     """DT[:, op(f.v), by(f.k)] over a frame row-partitioned across the ranks of `group`.
     exchange="allreduce": dense per-key tables all-reduced in place (every rank gets all groups);
-    "allgather": every rank gets all groups; "alltoall": rank r gets the r-th key range."""
+    "allgather": every rank gets all groups; "alltoall": rank r gets the r-th key range.
+    key_range: the caller's bound on the keys of all ranks, for exchange="allreduce" (see merge_partials_dense)."""
+    _merge_op(op)
     gkeys, part = local_groupby(k, v, op)
     if dist.is_available() and dist.is_initialized():
         if exchange == "alltoall":
             return merge_partials_alltoall(gkeys, part, op, group)
         if exchange == "allreduce":
-            return merge_partials_dense(gkeys, part, op, group)
+            return merge_partials_dense(gkeys, part, op, group, key_range=key_range)
         return merge_partials(gkeys, part, op, group)
     return gkeys, part
 
@@ -183,7 +224,7 @@ def _splitters(sorted_keys, world, group=None):
     have = torch.tensor([1 if n > 0 else 0], dtype=torch.int64, device=sorted_keys.device)
     allsamp = torch.empty(world * nsamp, dtype=sorted_keys.dtype, device=sorted_keys.device)
     allhave = torch.empty(world, dtype=torch.int64, device=sorted_keys.device)
-    dist.all_gather_into_tensor(allsamp, samp, group=group)
+    dist.all_gather_into_tensor(_bytes(allsamp), _bytes(samp), group=group)
     dist.all_gather_into_tensor(allhave, have, group=group)
     samp_h, have_h = allsamp.cpu().numpy(), allhave.cpu().numpy()
     pool = sorted(samp_h.reshape(world, nsamp)[have_h.astype(bool)].reshape(-1).tolist())
@@ -216,7 +257,9 @@ def _exchange(sorted_keys, payloads, world, group=None, kernels=None):
 
     def a2a(x):
         out = torch.empty(nrecv, dtype=x.dtype, device=x.device)
-        dist.all_to_all_single(out, x.contiguous(), output_split_sizes=recv_l, input_split_sizes=send_l, group=group)
+        esz = x.element_size()
+        dist.all_to_all_single(_bytes(out), _bytes(x), output_split_sizes=[c * esz for c in recv_l],
+                               input_split_sizes=[c * esz for c in send_l], group=group)
         return out
     timed = sorted_keys.is_cuda
     if timed:
@@ -231,15 +274,21 @@ def _exchange(sorted_keys, payloads, world, group=None, kernels=None):
 
 def merge_partials_alltoall(gkeys, part, op, group=None, kernels=_EngineKernels):
     """Key-range all-to-all of per-group partials; `gkeys` must be ascending (as group() returns them).
-    Rank r ends with the groups whose keys fall into the r-th global key range."""
+    Rank r ends with the groups whose keys fall into the r-th global key range.  Float keys travel as their
+    order-preserving integer images: a bisection by `<` is not monotone over a NaN-first run, so the NaN group
+    could otherwise be cut to different sides on different ranks."""
+    mop = _merge_op(op)
     world = dist.get_world_size(group)
     if world == 1:
         return gkeys, part
+    if gkeys.dtype.is_floating_point:
+        ik, mv = merge_partials_alltoall(_float_image(gkeys), part, op, group, kernels)
+        return _float_unimage(ik, gkeys.dtype), mv
     rk, (rp,) = _exchange(gkeys, [part], world, group, kernels)
     if rk.numel() == 0:
         return rk, rp
     order, offsets, ng = kernels.group(rk)
-    merged = kernels.reduce(_MERGE_OP[op], rp, order, offsets)
+    merged = kernels.reduce(mop, rp, order, offsets)
     first = kernels.take(order, offsets[:-1])
     return kernels.take(rk, first), merged
 

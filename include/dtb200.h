@@ -469,7 +469,9 @@ DTB_API int dtb_join(const dtb_col* xkeys, const dtb_col* jkeys, int nkeys, int6
  * key - kmin; the caller all-reduces `table` (SUM, typed as the partials are) and `present` (uint32
  * SUM) in place with NCCL; dtb_dense_compact then lists the keys that occur on any rank, ascending,
  * with their merged partials.  Device buffers only.  table/present must be zeroed before the scatter;
- * table_size: multiple of 1024, at most 2^22.  key_stype: DTB_STYPE_INT32 or DTB_STYPE_INT64.
+ * table_size: multiple of 1024, at most 2^22 (both functions refuse any other with DTB_EINVAL).  key_stype:
+ * DTB_STYPE_INT32 or DTB_STYPE_INT64.  The scatter skips a key outside [kmin, kmin + table_size): the caller
+ * chooses kmin and the size so that every key fits, or counts the keys that do not.
  */
 DTB_API int dtb_dense_scatter(const void* keys, int key_stype, const void* vals, int64_t n, int64_t kmin,
                       int64_t table_size, void* table, void* present, dtb_stream stream);

@@ -34,14 +34,28 @@ class OracleKernels:
 
     @staticmethod
     def lower_bound(sorted_keys, values):
-        return torch.from_numpy(np.searchsorted(sorted_keys.numpy(), values.numpy(), side="left").astype(np.int64))
+        # lower_bound_kernel's own bisection (dtb_next.cu), not np.searchsorted: on a run that is not ascending under
+        # `<` (NaN first) the two differ, and the exchange must not depend on which one runs
+        s = sorted_keys.tolist()
+        out = []
+        for x in values.tolist():
+            lo, hi = 0, len(s)
+            while lo < hi:
+                mid = (lo + hi) >> 1
+                if s[mid] < x:
+                    lo = mid + 1
+                else:
+                    hi = mid
+            out.append(lo)
+        return torch.tensor(out, dtype=torch.int64)
 
     # numpy stand-ins of dtb_dense_scatter / dtb_dense_compact (include/dtb200.h)
     @staticmethod
     def dense_scatter(gkeys, part, kmin, table, present):
         x = gkeys.long() - kmin
-        table[x] = part
-        present[x] = 1
+        keep = (x >= 0) & (x < table.numel())          # the kernel skips a key outside the table
+        table[x[keep]] = part[keep]
+        present[x[keep]] = 1
 
     @staticmethod
     def dense_compact(table, present, kmin, key_dtype):
@@ -88,18 +102,98 @@ def _worker(rank, world, port, q):
         dist.destroy_process_group()
 
 
-def test_merge_partials_world2():
+def _run_world2(worker):
     s = socket.socket(); s.bind(("127.0.0.1", 0)); port = s.getsockname()[1]; s.close()
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, q)) for r in range(2)]
-    for p in procs:
-        p.start()
-    res = [q.get(timeout=120) for _ in range(2)]
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    res.sort(key=lambda t: t[0])
+    procs = [ctx.Process(target=worker, args=(r, 2, port, q)) for r in range(2)]
+    try:
+        for p in procs:
+            p.start()
+        res = [q.get(timeout=120) for _ in range(2)]
+        for p in procs:
+            p.join(timeout=60)
+            assert p.exitcode == 0
+    finally:
+        for p in procs:
+            if p.is_alive():
+                p.terminate()
+            p.join(timeout=10)
+    return sorted(res, key=lambda t: t[0])
+
+
+I64_NA = np.iinfo(np.int64).min
+
+
+def _na_worker(rank, world, port, q):
+    """Group keys that hold the int64 NA or NaN, through the dense and the all-to-all merge."""
+    os.environ["MASTER_ADDR"] = "127.0.0.1"
+    os.environ["MASTER_PORT"] = str(port)
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    try:
+        from datatable_b200 import dist as ddist, _lib
+        out = {}
+
+        def t(a, dt):
+            return torch.tensor(a, dtype=dt)
+        # int64 NA on rank 0 only, then on every rank
+        k = [[I64_NA, 0, 1, 2], [5, 6, 7]][rank]
+        p = [[1.0, 2.0, 3.0, 4.0], [10.0, 20.0, 30.0]][rank]
+        out["na_one"] = ddist.merge_partials_dense(t(k, torch.int64), t(p, torch.float64), _lib.OP_SUM,
+                                                   kernels=OracleKernels)
+        k = [[I64_NA, 0, 1], [I64_NA, 1, 9]][rank]
+        p = [[1.0, 2.0, 3.0], [10.0, 20.0, 30.0]][rank]
+        out["na_all"] = ddist.merge_partials_dense(t(k, torch.int64), t(p, torch.float64), _lib.OP_SUM,
+                                                   kernels=OracleKernels)
+        # float keys with NaN through the all-to-all: the NaN group must come out once, first
+        k = [[np.nan, 1.0, 2.0, 3.0], [np.nan, 0.1, 0.2, 0.3, 1.0]][rank]
+        p = [[1.0, 2.0, 3.0, 4.0], [10.0, 20.0, 30.0, 40.0, 50.0]][rank]
+        out["nan_a2a"] = ddist.merge_partials_alltoall(t(k, torch.float64), t(p, torch.float64), _lib.OP_SUM,
+                                                       kernels=OracleKernels)
+        # a key outside the caller's key_range is refused on every rank rather than dropped
+        k = [[0, 1, 2], [3, 4, 12]][rank]
+        try:
+            ddist.merge_partials_dense(t(k, torch.int32), t([1.0, 2.0, 3.0], torch.float64), _lib.OP_SUM,
+                                       kernels=OracleKernels, key_range=(0, 9))
+            out["outside"] = None
+        except _lib.DtbValueError as e:
+            out["outside"] = str(e)
+        out = {name: v if isinstance(v, (str, type(None))) else (v[0].numpy(), v[1].numpy()) for name, v in out.items()}
+        q.put((rank, out))
+    finally:
+        dist.destroy_process_group()
+
+
+def test_merge_partials_na_keys_world2():
+    res = _run_world2(_na_worker)
+    want_one = (np.array([I64_NA, 0, 1, 2, 5, 6, 7]), np.array([1.0, 2, 3, 4, 10, 20, 30]))
+    want_all = (np.array([I64_NA, 0, 1, 9]), np.array([11.0, 2, 23, 30]))
+    for rank, out in res:                            # every rank holds every group, NA included
+        for name, (wk, wv) in (("na_one", want_one), ("na_all", want_all)):
+            gk, gv = out[name]
+            assert np.array_equal(gk, wk) and np.array_equal(gv, wv), (rank, name, gk, gv)
+        assert out["outside"] is not None and "outside key_range" in out["outside"], (rank, out["outside"])
+    gk = np.concatenate([out["nan_a2a"][0] for _, out in res])
+    gv = np.concatenate([out["nan_a2a"][1] for _, out in res])
+    assert np.isnan(gk[0]) and not np.isnan(gk[1:]).any(), gk
+    assert np.array_equal(gk[1:], [0.1, 0.2, 0.3, 1.0, 2.0, 3.0]) and np.array_equal(gv, [11.0, 20, 30, 40, 52, 3, 4])
+
+
+def test_merge_refusals_without_collectives():
+    """An op without a merge rule and an empty key_range are refused before any local work or collective."""
+    from datatable_b200 import dist as ddist, _lib
+    k, p = torch.tensor([1, 2], dtype=torch.int32), torch.tensor([1.0, 2.0], dtype=torch.float64)
+    for fn in (ddist.merge_partials, ddist.merge_partials_dense, ddist.merge_partials_alltoall):
+        with pytest.raises(_lib.DtbNotImplError, match="no merge rule"):
+            fn(k, p, _lib.OP_MEAN, kernels=OracleKernels)
+    with pytest.raises(_lib.DtbNotImplError, match="no merge rule"):
+        ddist.groupby_partitioned(k, p, _lib.OP_MEAN)
+    with pytest.raises(_lib.DtbValueError, match="empty"):
+        ddist.merge_partials_dense(k, p, _lib.OP_SUM, kernels=OracleKernels, key_range=(5, 4))
+
+
+def test_merge_partials_world2():
+    res = _run_world2(_worker)
     kall = np.concatenate([r[1] for r in res]); vall = np.concatenate([r[2] for r in res])
     uk = np.unique(kall)
     want = np.array([vall[kall == x].sum() for x in uk])
