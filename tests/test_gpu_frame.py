@@ -139,6 +139,15 @@ def test_reducers_without_by():              # tests/test-reduce.py:84-93
     assert R.to_list() == [[16], [2.0], [3], [4]]
 
 
+def test_repeated_column_names_deduplicated():   # frame/names.cc: _deduplicate gives x, x.0, x.1, ...
+    dt = dtmod(); f = dt.f
+    DT = dt.Frame(x=[1, None, 3])
+    for fr in (DT, DT.to_device()):
+        R = fr[:, [f.x, f.x]]
+        assert R.names == ("x", "x.0")
+        assert R.to_list() == [[1, None, 3], [1, None, 3]]
+
+
 def test_device_frame_stays_on_device():
     import torch
     dt = dtmod(); f, by = dt.f, dt.by
