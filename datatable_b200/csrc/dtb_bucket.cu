@@ -34,11 +34,6 @@ constexpr int BK_IPT = 8;                         // (16 rows x 256 threads ran 
 constexpr int BK_TILE = BK_THREADS * BK_IPT;      //  state per thread) 4096 rows per tile
 constexpr int64_t BK_CHUNK = 262144;              // rows per aggregate CTA
 
-static inline int bk_grid(int64_t n, int threads) {
-  const int64_t want = (n + threads - 1) / threads;
-  return (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : (want < 1 ? 1 : want));
-}
-
 // ---- rows per (slab, bucket) -> start[slab][bucket] ------------------------------------------------
 // A slab is a contiguous range of tiles.  Every slab gets its own output range inside every bucket
 // (buckets stay contiguous: slab 0's rows, then slab 1's, ...), so that the scatter tiles of one slab
@@ -414,18 +409,13 @@ int launch_bucketed_reduce(const u32* xkeys, int gshift, int dbits, int ncols, c
     for (int w = 0; w < BK_NWORDS; w++) acc.w[w] = acc_w[c][w];
     ProfScope ps("bucket_aggregate", s);
     const size_t smem = (size_t)cols.esz[c] * BK_ATILE + sizeof(u32) * BK_KEYS;
-#define DTB_AGG(T) { DTB_CUDA_CHECK(cudaFuncSetAttribute(bucket_aggregate_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-                     bucket_aggregate_kernel<T><<<chunks, BK_THREADS, smem, s>>>(xlow, (const typename RawKey<T>::load_t*)cols.out[c], start, nb, n, acc); }
-    switch (stypes[c]) {
-      case DTB_STYPE_BOOL: case DTB_STYPE_INT8:    DTB_AGG(int8_t)  break;
-      case DTB_STYPE_INT16:                        DTB_AGG(int16_t) break;
-      case DTB_STYPE_INT32: case DTB_STYPE_DATE32: DTB_AGG(int32_t) break;
-      case DTB_STYPE_INT64: case DTB_STYPE_TIME64: DTB_AGG(int64_t) break;
-      case DTB_STYPE_FLOAT32:                      DTB_AGG(float)   break;
-      case DTB_STYPE_FLOAT64:                      DTB_AGG(double)  break;
-      default: set_error("unsupported stype"); return DTB_ENOTIMPL;
-    }
-#undef DTB_AGG
+    DTB_TRY(with_stype(stypes[c], "unsupported stype ", [&](auto t) {
+      typedef typename decltype(t)::type T;
+      DTB_CUDA_CHECK(cudaFuncSetAttribute(bucket_aggregate_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      bucket_aggregate_kernel<T><<<chunks, BK_THREADS, smem, s>>>(xlow, (const typename RawKey<T>::load_t*)cols.out[c], start,
+                                                                  nb, n, acc);
+      return DTB_OK;
+    }));
     count_launch();
     DTB_CUDA_CHECK(cudaGetLastError());
   }

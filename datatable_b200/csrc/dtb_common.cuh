@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
+#include <type_traits>
 #include "dtb_internal.h"
 
 namespace dtb {
@@ -64,6 +65,19 @@ template <> struct RawKey<double> {
   typedef u64 load_t;
   static __device__ __forceinline__ bool get(u64 t, u64& u) { return f64_image(t, u); }
 };
+
+// T's NA as stored: the integer sentinel, or the quiet NaN every kernel writes for a float NA
+template <typename T> __host__ __device__ __forceinline__ typename RawKey<T>::load_t raw_na() {
+  typedef typename RawKey<T>::load_t O;
+  if constexpr (std::is_same<T, float>::value) return (O)0x7FC00000u;
+  else if constexpr (std::is_same<T, double>::value) return (O)0x7FF8000000000000ull;
+  else return NaOf<T>::v();
+}
+
+// The unsigned word of T's width: kernels that only move elements (gather, first / last) run one instance per width
+template <typename T>
+using bits_t = typename std::conditional<sizeof(T) == 1, uint8_t, typename std::conditional<sizeof(T) == 2, uint16_t,
+               typename std::conditional<sizeof(T) == 4, u32, u64>::type>::type>::type;
 
 // x = NA ? na_value : (((desc ? edge - u : u - edge) >> cshift) + inc)
 __device__ __forceinline__ u64 norm_apply(bool valid, u64 u, const KeyNorm& k) {
@@ -174,6 +188,37 @@ static inline int stype_bytes(int st) {
     case DTB_STYPE_INT64: case DTB_STYPE_FLOAT64: case DTB_STYPE_TIME64: return 8;
     default: return 0;
   }
+}
+
+// ---- host-side launch helpers --------------------------------------------------
+// CTAs of a grid-stride loop that wants `blocks` of them: at least 1, at most per_sm per SM
+static inline int grid_for(int64_t blocks, int per_sm) {
+  return (int)(blocks > NUM_SMS * per_sm ? NUM_SMS * per_sm : (blocks < 1 ? 1 : blocks));
+}
+
+template <typename T> struct TypeTag { typedef T type; };
+
+// f(TypeTag<T>()) with T the C++ type of an element of stype st: BOOL runs as INT8, DATE32 as INT32 and TIME64 as
+// INT64.  Any other stype fails with DTB_ENOTIMPL and the error `what` followed by the stype's number.
+template <typename F>
+static inline int with_stype(int st, const char* what, F&& f) {
+  switch (st) {
+    case DTB_STYPE_BOOL: case DTB_STYPE_INT8:    return f(TypeTag<int8_t>());
+    case DTB_STYPE_INT16:                        return f(TypeTag<int16_t>());
+    case DTB_STYPE_INT32: case DTB_STYPE_DATE32: return f(TypeTag<int32_t>());
+    case DTB_STYPE_INT64: case DTB_STYPE_TIME64: return f(TypeTag<int64_t>());
+    case DTB_STYPE_FLOAT32:                      return f(TypeTag<float>());
+    case DTB_STYPE_FLOAT64:                      return f(TypeTag<double>());
+  }
+  set_error(what + std::to_string(st));
+  return DTB_ENOTIMPL;
+}
+
+// f(order) with the RowIndex typed by its width: const int32_t* or const int64_t*
+template <typename F>
+static inline void with_order(const void* order, int order_is64, F&& f) {
+  if (order_is64) f((const int64_t*)order);
+  else            f((const int32_t*)order);
 }
 
 }  // namespace dtb

@@ -21,11 +21,6 @@
 
 namespace dtb {
 
-static inline int grid_for(int64_t n, int threads = 256) {
-  const int64_t want = (n + threads - 1) / threads;
-  return (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : (want < 1 ? 1 : want));
-}
-
 // raw element -> (valid, double) / (valid, order-preserving u64 image) ------------------------
 template <typename T> __device__ __forceinline__ bool elem_valid(const void* v, int64_t i) {
   typedef typename RawKey<T>::load_t L;
@@ -36,17 +31,6 @@ template <typename T> __device__ __forceinline__ double elem_double(const void* 
   else if constexpr (std::is_same<T, double>::value) return ((const double*)v)[i];
   else return (double)((const T*)v)[i];
 }
-
-#define DTB_DISPATCH_STYPE(st, CALL)                                   \
-  switch (st) {                                                        \
-    case DTB_STYPE_BOOL: case DTB_STYPE_INT8:    { CALL(int8_t);  break; }   \
-    case DTB_STYPE_INT16:                        { CALL(int16_t); break; }   \
-    case DTB_STYPE_INT32: case DTB_STYPE_DATE32: { CALL(int32_t); break; }   \
-    case DTB_STYPE_INT64: case DTB_STYPE_TIME64: { CALL(int64_t); break; }   \
-    case DTB_STYPE_FLOAT32:                      { CALL(float);   break; }   \
-    case DTB_STYPE_FLOAT64:                      { CALL(double);  break; }   \
-    default: set_error("unsupported stype"); return DTB_ENOTIMPL;      \
-  }
 
 // ===========================================================================
 // first / last: out[g] = v[order[offsets[g]]] or v[order[offsets[g+1]-1]] (NA stays NA)
@@ -67,19 +51,15 @@ int launch_firstlast(const void* v, int stype, int64_t nv, const int32_t* order,
                      int64_t ng, int last, void* out, cudaStream_t s)
 {
   if (ng == 0) return DTB_OK;
-  const int grid = grid_for(ng);
-  switch (stype_bytes(stype)) {
-    case 1: firstlast_kernel<uint8_t><<<grid, 256, 0, s>>>((const uint8_t*)v, nv, order, offsets, ng, last, (uint8_t)0x80, (uint8_t*)out); break;
-    case 2: firstlast_kernel<uint16_t><<<grid, 256, 0, s>>>((const uint16_t*)v, nv, order, offsets, ng, last, (uint16_t)0x8000, (uint16_t*)out); break;
-    case 4: firstlast_kernel<u32><<<grid, 256, 0, s>>>((const u32*)v, nv, order, offsets, ng, last,
-                                                       stype == DTB_STYPE_FLOAT32 ? 0x7FC00000u : 0x80000000u, (u32*)out); break;
-    case 8: firstlast_kernel<u64><<<grid, 256, 0, s>>>((const u64*)v, nv, order, offsets, ng, last,
-                                                       stype == DTB_STYPE_FLOAT64 ? 0x7FF8000000000000ull : 0x8000000000000000ull, (u64*)out); break;
-    default: set_error("unsupported stype"); return DTB_ENOTIMPL;
-  }
-  count_launch();
-  DTB_CUDA_CHECK(cudaGetLastError());
-  return DTB_OK;
+  return with_stype(stype, "unsupported stype ", [&](auto t) {
+    typedef typename decltype(t)::type T;
+    typedef bits_t<T> E;
+    firstlast_kernel<E><<<grid_for((ng + 255) / 256, 16), 256, 0, s>>>((const E*)v, nv, order, offsets, ng, last,
+                                                                       (E)raw_na<T>(), (E*)out);
+    count_launch();
+    DTB_CUDA_CHECK(cudaGetLastError());
+    return DTB_OK;
+  });
 }
 
 // ===========================================================================
@@ -105,7 +85,7 @@ __global__ void expand_gid_kernel(const int32_t* __restrict__ offsets, int64_t n
 
 int launch_expand_gid(const int32_t* offsets, int64_t ng, int64_t n, int32_t* gid, cudaStream_t s) {
   if (n == 0) return DTB_OK;
-  expand_gid_kernel<<<grid_for((n + 7) / 8), 256, 0, s>>>(offsets, ng, n, gid);
+  expand_gid_kernel<<<grid_for(((n + 7) / 8 + 255) / 256, 16), 256, 0, s>>>(offsets, ng, n, gid);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;
@@ -154,17 +134,16 @@ int launch_first_valid_pos(const void* v, int stype, int64_t nv, const void* ord
                            int64_t ng, int64_t n, int zero_only, const u64* gate, u64* pos, cudaStream_t s)
 {
   if (ng == 0 || n == 0) return DTB_OK;
-  const int grid = grid_for((n + 7) / 8);
-#define CALL(T) { typedef typename RawKey<T>::load_t L;                                                             \
-                  if (order_is64) first_valid_pos_kernel<T, int64_t><<<grid, 256, 0, s>>>((const L*)v, nv,          \
-                                    (const int64_t*)order, offsets, ng, n, zero_only, gate, pos);                    \
-                  else            first_valid_pos_kernel<T, int32_t><<<grid, 256, 0, s>>>((const L*)v, nv,          \
-                                    (const int32_t*)order, offsets, ng, n, zero_only, gate, pos); }
-  DTB_DISPATCH_STYPE(stype, CALL)
-#undef CALL
-  count_launch();
-  DTB_CUDA_CHECK(cudaGetLastError());
-  return DTB_OK;
+  return with_stype(stype, "unsupported stype ", [&](auto t) {
+    typedef typename decltype(t)::type T;
+    with_order(order, order_is64, [&](auto o) {
+      first_valid_pos_kernel<T><<<grid_for(((n + 7) / 8 + 255) / 256, 16), 256, 0, s>>>(
+          (const typename RawKey<T>::load_t*)v, nv, o, offsets, ng, n, zero_only, gate, pos);
+    });
+    count_launch();
+    DTB_CUDA_CHECK(cudaGetLastError());
+    return DTB_OK;
+  });
 }
 
 // ===========================================================================
@@ -242,8 +221,8 @@ __global__ void sd_finalize_kernel(const double* __restrict__ m2, const u64* __r
     const double q = m2[g];
     const bool valid = c > 1 && !isnan(q);                     // head_reduce_unary.cc:213
     const double sd = q >= 0 ? sqrt(q / (double)(c - 1)) : 0.0;
-    if (out_f32) ((u32*)out)[g] = valid ? __float_as_uint((float)sd) : 0x7FC00000u;
-    else         ((u64*)out)[g] = valid ? (u64)__double_as_longlong(sd) : 0x7FF8000000000000ull;
+    if (out_f32) ((u32*)out)[g] = valid ? __float_as_uint((float)sd) : raw_na<float>();
+    else         ((u64*)out)[g] = valid ? (u64)__double_as_longlong(sd) : raw_na<double>();
   }
 }
 
@@ -253,17 +232,19 @@ int launch_sd(const void* v, int stype, int64_t nv, const int32_t* order, const 
   if (ng == 0) return DTB_OK;
   if (n > 0) {
     double* pivot = m2 + ng;
-    const int grid = grid_for((n + 7) / 8);
+    const int grid = grid_for(((n + 7) / 8 + 255) / 256, 16);
     fill_u64((u64*)pivot, ng, ~0ull, s);
     DTB_TRY(launch_first_valid_pos(v, stype, nv, order, 0, offsets, ng, n, 0, nullptr, (u64*)pivot, s));
-#define CALL(T) sd_pivot_kernel<T><<<grid_for(ng), 256, 0, s>>>(v, order, ng, pivot); \
-                sd_pass_kernel<T, false><<<grid, 256, 0, s>>>(v, nv, order, offsets, ng, n, pivot, sum, cnt, m2); \
-                sd_pass_kernel<T, true><<<grid, 256, 0, s>>>(v, nv, order, offsets, ng, n, pivot, sum, cnt, m2)
-    DTB_DISPATCH_STYPE(stype, CALL)
-#undef CALL
+    DTB_TRY(with_stype(stype, "unsupported stype ", [&](auto t) {
+      typedef typename decltype(t)::type T;
+      sd_pivot_kernel<T><<<grid_for((ng + 255) / 256, 16), 256, 0, s>>>(v, order, ng, pivot);
+      sd_pass_kernel<T, false><<<grid, 256, 0, s>>>(v, nv, order, offsets, ng, n, pivot, sum, cnt, m2);
+      sd_pass_kernel<T, true><<<grid, 256, 0, s>>>(v, nv, order, offsets, ng, n, pivot, sum, cnt, m2);
+      return DTB_OK;
+    }));
     count_launch(3);
   }
-  sd_finalize_kernel<<<grid_for(ng), 256, 0, s>>>(m2, cnt, ng, stype == DTB_STYPE_FLOAT32, out);
+  sd_finalize_kernel<<<grid_for((ng + 255) / 256, 16), 256, 0, s>>>(m2, cnt, ng, stype == DTB_STYPE_FLOAT32, out);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;
@@ -404,8 +385,8 @@ __global__ void pair_finalize_kernel(int corr, const u64* __restrict__ acc, int6
     bool valid; double r;
     if (corr) { valid = c > 1 && vv > 0; r = sxy / sqrt(vv); }
     else      { valid = c > 1; r = sxy / (double)(c - 1); }
-    if (out_f32) ((u32*)out)[g] = valid ? __float_as_uint((float)r) : 0x7FC00000u;
-    else         ((u64*)out)[g] = valid ? (u64)__double_as_longlong(r) : 0x7FF8000000000000ull;
+    if (out_f32) ((u32*)out)[g] = valid ? __float_as_uint((float)r) : raw_na<float>();
+    else         ((u64*)out)[g] = valid ? (u64)__double_as_longlong(r) : raw_na<double>();
   }
 }
 
@@ -424,9 +405,9 @@ static void run_pairs(const PairCols& pc, const OrdT* order, const int32_t* offs
 {
   double* px = reinterpret_cast<double*>(acc + 6 * ng);
   double* py = px + ng;
-  const int grid = grid_for((n + 7) / 8);
+  const int grid = grid_for(((n + 7) / 8 + 255) / 256, 16);
   pair_first_pos_kernel<OrdT><<<grid, 256, 0, s>>>(pc, order, offsets, ng, n, (u64*)px);
-  pair_pivot_kernel<OrdT><<<grid_for(ng), 256, 0, s>>>(pc, order, ng, px, py);
+  pair_pivot_kernel<OrdT><<<grid_for((ng + 255) / 256, 16), 256, 0, s>>>(pc, order, ng, px, py);
   pair_pass_kernel<OrdT, false><<<grid, 256, 0, s>>>(pc, order, offsets, ng, n, px, py, acc, corr);
   pair_pass_kernel<OrdT, true><<<grid, 256, 0, s>>>(pc, order, offsets, ng, n, px, py, acc, corr);
   count_launch(4);
@@ -441,10 +422,9 @@ int launch_reduce2(int op, const void* x, int sx, const void* y, int sy, int64_t
   const int corr = op == DTB_OP_CORR;
   if (n > 0) {
     const PairCols pc = {x, y, sx, sy, nv};
-    if (order_is64) run_pairs(pc, (const int64_t*)order, offsets, ng, n, scratch, corr, s);
-    else            run_pairs(pc, (const int32_t*)order, offsets, ng, n, scratch, corr, s);
+    with_order(order, order_is64, [&](auto o) { run_pairs(pc, o, offsets, ng, n, scratch, corr, s); });
   }
-  pair_finalize_kernel<<<grid_for(ng), 256, 0, s>>>(corr, scratch, ng, out_f32, out);
+  pair_finalize_kernel<<<grid_for((ng + 255) / 256, 16), 256, 0, s>>>(corr, scratch, ng, out_f32, out);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;
@@ -482,8 +462,8 @@ __global__ void median_kernel(const void* __restrict__ v, int64_t nv, const int3
         else m = (elem_double<T>(v, r1) + elem_double<T>(v, r2)) / 2;
       }
     }
-    if (F32) ((u32*)out)[g] = valid ? __float_as_uint((float)m) : 0x7FC00000u;
-    else     ((u64*)out)[g] = valid ? (u64)__double_as_longlong(m) : 0x7FF8000000000000ull;
+    if (F32) ((u32*)out)[g] = valid ? __float_as_uint((float)m) : raw_na<float>();
+    else     ((u64*)out)[g] = valid ? (u64)__double_as_longlong(m) : raw_na<double>();
   }
 }
 
@@ -491,13 +471,12 @@ int launch_median(const void* v, int stype, int64_t nv, const int32_t* order, co
                   int64_t ng, void* out, cudaStream_t s)
 {
   if (ng == 0) return DTB_OK;
-  const int grid = grid_for(ng);
-#define CALL(T) median_kernel<T><<<grid, 256, 0, s>>>(v, nv, order, offsets, ng, out)
-  DTB_DISPATCH_STYPE(stype, CALL)
-#undef CALL
-  count_launch();
-  DTB_CUDA_CHECK(cudaGetLastError());
-  return DTB_OK;
+  return with_stype(stype, "unsupported stype ", [&](auto t) {
+    median_kernel<typename decltype(t)::type><<<grid_for((ng + 255) / 256, 16), 256, 0, s>>>(v, nv, order, offsets, ng, out);
+    count_launch();
+    DTB_CUDA_CHECK(cudaGetLastError());
+    return DTB_OK;
+  });
 }
 
 // ===========================================================================
@@ -547,13 +526,14 @@ int launch_distinct_flags(const void* v, int stype, int64_t nv, const int32_t* o
                           int64_t ng, int64_t n, int8_t* flag, cudaStream_t s)
 {
   if (n == 0) return DTB_OK;
-#define CALL(T) { distinct_flags_kernel<T><<<grid_for(n), 256, 0, s>>>(v, nv, order, n, flag); \
-                  distinct_starts_kernel<T><<<grid_for(ng), 256, 0, s>>>(v, nv, order, offsets, ng, flag); }
-  DTB_DISPATCH_STYPE(stype, CALL)
-#undef CALL
-  count_launch(2);
-  DTB_CUDA_CHECK(cudaGetLastError());
-  return DTB_OK;
+  return with_stype(stype, "unsupported stype ", [&](auto t) {
+    typedef typename decltype(t)::type T;
+    distinct_flags_kernel<T><<<grid_for((n + 255) / 256, 16), 256, 0, s>>>(v, nv, order, n, flag);
+    distinct_starts_kernel<T><<<grid_for((ng + 255) / 256, 16), 256, 0, s>>>(v, nv, order, offsets, ng, flag);
+    count_launch(2);
+    DTB_CUDA_CHECK(cudaGetLastError());
+    return DTB_OK;
+  });
 }
 
 // ===========================================================================
@@ -646,15 +626,17 @@ int launch_qcut(const void* vg, int stype, const int32_t* cord, const int32_t* c
   uint8_t* has_na = (uint8_t*)(cog + nc);
   {
     ProfScope ps("qcut_coef", s);
-    qcut_starts_kernel<<<grid_for(nc), 256, 0, s>>>(cord, coff, nc, gid, ng, cog, cstart);
-#define CALL(T) qcut_coef_kernel<T><<<grid_for(ng), 256, 0, s>>>(vg, cord, coff, cstart, ng, q, coef, has_na)
-    DTB_DISPATCH_STYPE(stype, CALL)
-#undef CALL
+    qcut_starts_kernel<<<grid_for((nc + 255) / 256, 16), 256, 0, s>>>(cord, coff, nc, gid, ng, cog, cstart);
+    DTB_TRY(with_stype(stype, "unsupported stype ", [&](auto t) {
+      qcut_coef_kernel<typename decltype(t)::type><<<grid_for((ng + 255) / 256, 16), 256, 0, s>>>(vg, cord, coff, cstart,
+                                                                                                 ng, q, coef, has_na);
+      return DTB_OK;
+    }));
     count_launch(2);
     DTB_CUDA_CHECK(cudaGetLastError());
   }
   ProfScope ps("qcut_emit", s);
-  qcut_emit_kernel<<<grid_for((n + 7) / 8), 256, 0, s>>>(cord, coff, nc, n, cog, cstart, coef, has_na, out);
+  qcut_emit_kernel<<<grid_for(((n + 7) / 8 + 255) / 256, 16), 256, 0, s>>>(cord, coff, nc, n, cog, cstart, coef, has_na, out);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;
@@ -710,7 +692,7 @@ __global__ void set_emit_kernel(const int32_t* __restrict__ pos, int64_t nsel, c
 int launch_set_select(const int32_t* order, const int32_t* offsets, int64_t ng, const int64_t* d_sizes, int K,
                       int mode, uint8_t* flags, cudaStream_t s)
 {
-  set_select_kernel<<<grid_for(ng), 256, 0, s>>>(order, offsets, ng, d_sizes, K, mode, flags);
+  set_select_kernel<<<grid_for((ng + 255) / 256, 16), 256, 0, s>>>(order, offsets, ng, d_sizes, K, mode, flags);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;
@@ -720,7 +702,7 @@ int launch_set_emit(const int32_t* pos, int64_t nsel, const int32_t* order, cons
                     cudaStream_t s)
 {
   if (nsel == 0) return DTB_OK;
-  set_emit_kernel<<<grid_for(nsel), 256, 0, s>>>(pos, nsel, order, offsets, out_rows);
+  set_emit_kernel<<<grid_for((nsel + 255) / 256, 16), 256, 0, s>>>(pos, nsel, order, offsets, out_rows);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;
@@ -747,7 +729,7 @@ __global__ void largest_group_kernel(const int32_t* __restrict__ offsets, int64_
 int launch_largest_group(const int32_t* offsets, int64_t ng, int64_t skip, unsigned long long* d_result, cudaStream_t s)
 {
   if (ng <= skip) return DTB_OK;
-  largest_group_kernel<<<grid_for(ng - skip), 256, 0, s>>>(offsets, ng, skip, d_result);
+  largest_group_kernel<<<grid_for((ng - skip + 255) / 256, 16), 256, 0, s>>>(offsets, ng, skip, d_result);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;
@@ -840,7 +822,7 @@ int launch_join(int nkeys, const void* const* xcols, const int* xst, const void*
   if (nx == 0) return DTB_OK;
   JoinPlan jp; jp.nkeys = nkeys;
   for (int c = 0; c < nkeys; c++) { jp.c[c].x = xcols[c]; jp.c[c].j = jcols[c]; jp.c[c].xst = xst[c]; jp.c[c].jst = jst[c]; }
-  join_kernel<<<grid_for(nx), 256, 0, s>>>(jp, nx, nj, out);
+  join_kernel<<<grid_for((nx + 255) / 256, 16), 256, 0, s>>>(jp, nx, nj, out);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;
@@ -865,13 +847,13 @@ __global__ void lower_bound_kernel(const T* __restrict__ sorted, int64_t n, cons
 int launch_lower_bound(const void* sorted, int stype, int64_t n, const void* values, int64_t m, int64_t* out, cudaStream_t s)
 {
   if (m == 0) return DTB_OK;
-  const int grid = grid_for(m);
-#define CALL(T) lower_bound_kernel<T><<<grid, 256, 0, s>>>((const T*)sorted, n, (const T*)values, m, out)
-  DTB_DISPATCH_STYPE(stype, CALL)
-#undef CALL
-  count_launch();
-  DTB_CUDA_CHECK(cudaGetLastError());
-  return DTB_OK;
+  return with_stype(stype, "unsupported stype ", [&](auto t) {
+    typedef typename decltype(t)::type T;
+    lower_bound_kernel<T><<<grid_for((m + 255) / 256, 16), 256, 0, s>>>((const T*)sorted, n, (const T*)values, m, out);
+    count_launch();
+    DTB_CUDA_CHECK(cudaGetLastError());
+    return DTB_OK;
+  });
 }
 
 // ===========================================================================
@@ -1047,7 +1029,7 @@ int launch_slice_groups_emit(const int32_t* offsets, const SliceParams& p, const
 {
   if (nout == 0) return DTB_OK;
   DTB_TRY(launch_expand_gid(offsets_out, ng_out, nout, gid, s));
-  slice_emit_kernel<<<grid_for(nout), 256, 0, s>>>(offsets, p, offsets_out, gsel, gid, nout, rows_out);
+  slice_emit_kernel<<<grid_for((nout + 255) / 256, 16), 256, 0, s>>>(offsets, p, offsets_out, gsel, gid, nout, rows_out);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;

@@ -87,8 +87,7 @@ int launch_compose_keys(const KeyPlan& kp, int64_t n, const int32_t* idx, void* 
     return DTB_EINVAL;
   }
   if (n == 0) return DTB_OK;
-  int64_t want = (n + 1023) / 1024;
-  int grid = (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : want);
+  const int grid = grid_for((n + 1023) / 1024, 16);
   if (key_bytes == 4) compose_keys_kernel<u32><<<grid, 256, 0, s>>>(kp, n, idx, (u32*)keys_out, out_shift);
   else                compose_keys_kernel<u64><<<grid, 256, 0, s>>>(kp, n, idx, (u64*)keys_out, out_shift);
   count_launch();
@@ -721,20 +720,10 @@ template <typename KeyT>
 static int run_pass_raw(const PassIO& io, const KeyPlan& kp, int64_t n, int shift, int bits,
                         u32* work, cudaStream_t s, u32* group_count, int group_shift)
 {
-  const KeyNorm& k = kp.k[0];
-#define DTB_CASE(T)                                                                          \
-  { RawSrc<T, KeyT> src; src.init(k);                                                        \
-    return run_pass<KeyT>(src, io, n, shift, bits, work, s, group_count, group_shift); }
-  switch (k.stype) {
-    case DTB_STYPE_BOOL: case DTB_STYPE_INT8:    DTB_CASE(int8_t)
-    case DTB_STYPE_INT16:                        DTB_CASE(int16_t)
-    case DTB_STYPE_INT32: case DTB_STYPE_DATE32: DTB_CASE(int32_t)
-    case DTB_STYPE_INT64: case DTB_STYPE_TIME64: DTB_CASE(int64_t)
-    case DTB_STYPE_FLOAT32:                      DTB_CASE(float)
-    case DTB_STYPE_FLOAT64:                      DTB_CASE(double)
-  }
-#undef DTB_CASE
-  set_error("internal: bad stype in radix pass"); return DTB_EINVAL;
+  return with_stype(kp.k[0].stype, "internal: radix pass over a key of stype ", [&](auto t) {
+    RawSrc<typename decltype(t)::type, KeyT> src; src.init(kp.k[0]);
+    return run_pass<KeyT>(src, io, n, shift, bits, work, s, group_count, group_shift);
+  });
 }
 
 size_t radix_pass_work_bytes(int64_t n) {
@@ -777,8 +766,7 @@ __global__ void widen_u32_kernel(const u32* __restrict__ in, int64_t n, int64_t*
 
 int launch_widen_u32(const uint32_t* in, int64_t n, int64_t* out, cudaStream_t s) {
   if (n == 0) return DTB_OK;
-  int64_t want = (n + 255) / 256;
-  int grid = (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : want);
+  const int grid = grid_for((n + 255) / 256, 16);
   widen_u32_kernel<<<grid, 256, 0, s>>>(in, n, out);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
@@ -792,8 +780,7 @@ __global__ void iota32_kernel(int32_t* out, int64_t n) {
 
 int launch_iota32(int32_t* out, int64_t n, cudaStream_t s) {
   if (n == 0) return DTB_OK;
-  int64_t want = (n + 255) / 256;
-  int grid = (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : want);
+  const int grid = grid_for((n + 255) / 256, 16);
   iota32_kernel<<<grid, 256, 0, s>>>(out, n);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());

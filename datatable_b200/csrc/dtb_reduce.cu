@@ -302,8 +302,7 @@ __global__ void fill_u64_kernel(u64* p, int64_t n, u64 v) {
 
 void fill_u64(unsigned long long* p, int64_t n, unsigned long long v, cudaStream_t s) {
   if (n <= 0) return;
-  const int g = (int)((n + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (n + 255) / 256);
-  fill_u64_kernel<<<g, 256, 0, s>>>(p, n, v);
+  fill_u64_kernel<<<grid_for((n + 255) / 256, 8), 256, 0, s>>>(p, n, v);
   count_launch();
 }
 
@@ -323,8 +322,8 @@ __device__ __forceinline__ void store_result(void* out, int out_stype, int64_t g
       ((int32_t*)out)[g] = valid ? (int32_t)bits : INT32_MIN; break;
     case DTB_STYPE_INT64: case DTB_STYPE_TIME64:
       ((int64_t*)out)[g] = valid ? (int64_t)bits : INT64_MIN; break;
-    case DTB_STYPE_FLOAT32: ((u32*)out)[g] = valid ? (u32)bits : 0x7FC00000u; break;
-    case DTB_STYPE_FLOAT64: ((u64*)out)[g] = valid ? bits : 0x7FF8000000000000ull; break;
+    case DTB_STYPE_FLOAT32: ((u32*)out)[g] = valid ? (u32)bits : raw_na<float>(); break;
+    case DTB_STYPE_FLOAT64: ((u64*)out)[g] = valid ? bits : raw_na<double>(); break;
   }
 }
 
@@ -381,31 +380,32 @@ static int zero_fix_end(int op, int stype, const GroupRows& gr, int64_t ng, void
   if (!wants_zero_fix(op, stype, gr) || ng == 0) return DTB_OK;
   DTB_TRY(launch_first_valid_pos(gr.v, stype, gr.nv, gr.order, gr.order_is64, gr.offsets, ng, gr.n, 1,
                                  gr.zpos + ng, gr.zpos, s));
-  const int fgrid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
-  zero_fix_kernel<<<fgrid, 256, 0, s>>>(stype, gr, ng, out);
+  zero_fix_kernel<<<grid_for((ng + 255) / 256, 8), 256, 0, s>>>(stype, gr, ng, out);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;
 }
 
+// out[g] = the result of the accumulators of group key gkeys[g] (direct-address reducers), or of group g (gkeys NULL)
 __global__ void finalize_kernel(int op, int in_stype, int out_stype, const u64* __restrict__ acc0,
-                                const u64* __restrict__ acc1, int64_t ng, void* out, const GroupRows gr)
+                                const u64* __restrict__ acc1, const u32* __restrict__ gkeys,
+                                int64_t ng, void* out, const GroupRows gr)
 {
   const bool in_float = (in_stype == DTB_STYPE_FLOAT32 || in_stype == DTB_STYPE_FLOAT64);
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += stride) {
-    const u64 a = acc0[g];
+    const u32 x = gkeys ? gkeys[g] : (u32)g;
+    const u64 a = acc0[x];
     bool valid = true; u64 bits = a;
     switch (op) {
       case DTB_OP_SUM:
         if (out_stype == DTB_STYPE_FLOAT32) bits = __float_as_uint((float)__longlong_as_double((long long)a));
         break;                                            // int64 / float64: accumulator bits are the result
       case DTB_OP_MEAN: {
-        const u64 c = acc1[g];
+        const u64 c = acc1[x];
         valid = c != 0;
         const double m = __longlong_as_double((long long)a) / (double)c;
-        bits = (out_stype == DTB_STYPE_FLOAT32) ? (u64)__float_as_uint((float)m)
-                                                : (u64)__double_as_longlong(m);
+        bits = (out_stype == DTB_STYPE_FLOAT32) ? (u64)__float_as_uint((float)m) : (u64)__double_as_longlong(m);
         break; }
       case DTB_OP_MIN: case DTB_OP_MAX: {
         const bool is_min = (op == DTB_OP_MIN);
@@ -440,6 +440,20 @@ static int reduce_out_stype(int op, int st) {
   return 0;
 }
 
+// out[g] = finalize_kernel's result for every group, with the sign lookup of a zero float min / max (gr.zpos)
+static int finalize(int op, int stype, const u64* acc0, const u64* acc1, const u32* gkeys, int64_t ng, void* out,
+                    const GroupRows& gr, cudaStream_t s)
+{
+  const int out_st = reduce_out_stype(op, stype);
+  if (!out_st) { set_error("Invalid column type in reducer"); return DTB_EINVAL; }
+  if (ng == 0) return DTB_OK;
+  DTB_TRY(zero_fix_begin(op, stype, gr, ng, s));
+  finalize_kernel<<<grid_for((ng + 255) / 256, 8), 256, 0, s>>>(op, stype, out_st, acc0, acc1, gkeys, ng, out, gr);
+  count_launch();
+  DTB_CUDA_CHECK(cudaGetLastError());
+  return zero_fix_end(op, stype, gr, ng, out, s);
+}
+
 size_t reduce_extra_bytes(int op, int stype, int64_t ng, int64_t n) {
   if (op == DTB_OP_SD) return 2 * sizeof(double) * (size_t)(ng > 0 ? ng : 1);      // m2, pivots
   if (op == DTB_OP_PROD)                                                          // acc1, then the tiles' slots
@@ -456,42 +470,12 @@ static int run_reduce(const void* v, int64_t nv, const void* order, int order_is
 {
   typedef typename RawKey<T>::load_t L;
   const unsigned grid = (unsigned)((n + RTILE - 1) / RTILE);
-  if (order_is64)
-    reduce_kernel<T, CAT, int64_t><<<grid, RT, 0, s>>>((const L*)v, nv, (const int64_t*)order, offsets, ng, n, acc0, acc1, flag);
-  else
-    reduce_kernel<T, CAT, int32_t><<<grid, RT, 0, s>>>((const L*)v, nv, (const int32_t*)order, offsets, ng, n, acc0, acc1, flag);
+  with_order(order, order_is64, [&](auto o) {
+    reduce_kernel<T, CAT><<<grid, RT, 0, s>>>((const L*)v, nv, o, offsets, ng, n, acc0, acc1, flag);
+  });
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;
-}
-
-template <int CAT>
-static int dispatch_T(int st, const void* v, int64_t nv, const void* order, int order_is64,
-                      const int32_t* offsets, int64_t ng, int64_t n, u64* acc0, u64* acc1,
-                      int flag, cudaStream_t s)
-{
-  constexpr bool INTS = CAT != CAT_SUMF && CAT != CAT_PRODF, FLOATS = CAT != CAT_SUMI && CAT != CAT_PRODI;
-  switch (st) {
-    case DTB_STYPE_BOOL: case DTB_STYPE_INT8:
-      if constexpr (INTS) return run_reduce<int8_t, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
-      break;
-    case DTB_STYPE_INT16:
-      if constexpr (INTS) return run_reduce<int16_t, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
-      break;
-    case DTB_STYPE_INT32:
-      if constexpr (INTS) return run_reduce<int32_t, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
-      break;
-    case DTB_STYPE_INT64:
-      if constexpr (INTS) return run_reduce<int64_t, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
-      break;
-    case DTB_STYPE_FLOAT32:
-      if constexpr (FLOATS) return run_reduce<float, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
-      break;
-    case DTB_STYPE_FLOAT64:
-      if constexpr (FLOATS) return run_reduce<double, CAT>(v, nv, order, order_is64, offsets, ng, n, acc0, acc1, flag, s);
-      break;
-  }
-  set_error("internal: reducer/stype combination"); return DTB_EINVAL;
 }
 
 template <int CAT>
@@ -557,8 +541,8 @@ __global__ void prod_finalize_kernel(const int32_t* __restrict__ offsets, int64_
       bool valid;
       const double r = prodf_value(p, valid);
       // float32: the float64 r is exact wherever a float32 result is not 0, so this rounds once
-      if (out_stype == DTB_STYPE_FLOAT32) ((u32*)out)[g] = valid ? __float_as_uint((float)r) : 0x7FC00000u;
-      else ((u64*)out)[g] = valid ? (u64)__double_as_longlong(r) : 0x7FF8000000000000ull;
+      if (out_stype == DTB_STYPE_FLOAT32) ((u32*)out)[g] = valid ? __float_as_uint((float)r) : raw_na<float>();
+      else ((u64*)out)[g] = valid ? (u64)__double_as_longlong(r) : raw_na<double>();
     }
   }
 }
@@ -569,20 +553,20 @@ static int launch_prod(const void* value, int stype, int64_t nv, const void* ord
                        const int32_t* offsets, int64_t ng, int64_t n, u64* acc0, u64* acc1, int out_st, void* out,
                        cudaStream_t s)
 {
-  const bool isflt = (stype == DTB_STYPE_FLOAT32 || stype == DTB_STYPE_FLOAT64);
-  const int64_t ntiles = (n + RTILE - 1) / RTILE;            // every tile writes both its slots
-  fill_u64(acc0, ng, isflt ? 0ull : 1ull, s);
-  fill_u64(acc1, ng, 0ull, s);
-  DTB_CUDA_CHECK(cudaGetLastError());
-  if (n > 0)
-    DTB_TRY(isflt ? dispatch_T<CAT_PRODF>(stype, value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 0, s)
-                  : dispatch_T<CAT_PRODI>(stype, value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 0, s));
-  const int fgrid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
-  if (isflt) prod_finalize_kernel<CAT_PRODF><<<fgrid, 256, 0, s>>>(offsets, ng, n, acc0, acc1, ntiles, out_st, out);
-  else       prod_finalize_kernel<CAT_PRODI><<<fgrid, 256, 0, s>>>(offsets, ng, n, acc0, acc1, ntiles, out_st, out);
-  count_launch();
-  DTB_CUDA_CHECK(cudaGetLastError());
-  return DTB_OK;
+  return with_stype(stype, "internal: product of stype ", [&](auto t) {
+    typedef typename decltype(t)::type T;
+    constexpr bool ISF = std::is_floating_point<T>::value;
+    constexpr int CAT = ISF ? CAT_PRODF : CAT_PRODI;
+    const int64_t ntiles = (n + RTILE - 1) / RTILE;          // every tile writes both its slots
+    fill_u64(acc0, ng, ISF ? 0ull : 1ull, s);
+    fill_u64(acc1, ng, 0ull, s);
+    DTB_CUDA_CHECK(cudaGetLastError());
+    if (n > 0) DTB_TRY((run_reduce<T, CAT>(value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 0, s)));
+    prod_finalize_kernel<CAT><<<grid_for((ng + 255) / 256, 8), 256, 0, s>>>(offsets, ng, n, acc0, acc1, ntiles, out_st, out);
+    count_launch();
+    DTB_CUDA_CHECK(cudaGetLastError());
+    return DTB_OK;
+  });
 }
 
 // acc0/acc1: device scratch of ng u64 each (allocated by the caller in dtb_api.cu)
@@ -593,7 +577,7 @@ int launch_reduce_impl(int op, const void* value, int stype, int64_t nv, const v
   const int out_st = reduce_out_stype(op, stype);
   if (!out_st) { set_error("Invalid column type in reducer"); return DTB_EINVAL; }
   if (ng == 0) return DTB_OK;
-  const int fgrid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
+  const int fgrid = grid_for((ng + 255) / 256, 8);
   if (op >= DTB_OP_FIRST && op <= DTB_OP_NUNIQUE) {
     // within-group ordered reducers (dtb_next.cu): they walk the ARR32 RowIndex
     if (order_is64) { set_error("first/last/sd/median/nunique take an int32 RowIndex"); return DTB_ENOTIMPL; }
@@ -613,47 +597,38 @@ int launch_reduce_impl(int op, const void* value, int stype, int64_t nv, const v
     DTB_TRY(launch_distinct_flags(value, stype, nv, o32, offsets, ng, n, flag, s));
     fill_u64_kernel<<<fgrid, 256, 0, s>>>(acc0, ng, 0ull);
     count_launch();
-    if (n > 0) DTB_TRY(dispatch_T<CAT_COUNT>(DTB_STYPE_INT8, flag, n, nullptr, 0, offsets, ng, n, acc0, acc1, 0, s));
-    finalize_kernel<<<fgrid, 256, 0, s>>>(DTB_OP_COUNT, DTB_STYPE_INT8, DTB_STYPE_INT64, acc0, acc1, ng, out, GroupRows());
-    count_launch();
-    DTB_CUDA_CHECK(cudaGetLastError());
-    return DTB_OK;
+    if (n > 0) DTB_TRY((run_reduce<int8_t, CAT_COUNT>(flag, n, nullptr, 0, offsets, ng, n, acc0, acc1, 0, s)));
+    return finalize(DTB_OP_COUNT, DTB_STYPE_INT8, acc0, acc1, nullptr, ng, out, GroupRows(), s);
   }
   if (op == DTB_OP_NROWS) return launch_nrows(offsets, ng, out, s);
   if (op == DTB_OP_PROD) {
     if (!extra) { set_error("internal: reducer scratch missing"); return DTB_EINVAL; }
     return launch_prod(value, stype, nv, order, order_is64, offsets, ng, n, acc0, (u64*)extra, out_st, out, s);
   }
-  const bool isflt = (stype == DTB_STYPE_FLOAT32 || stype == DTB_STYPE_FLOAT64);
   u64 init0 = (op == DTB_OP_MIN) ? ~0ull : 0ull;          // 0.0 == 0 bits for float sums
   fill_u64_kernel<<<fgrid, 256, 0, s>>>(acc0, ng, init0);
   count_launch();
   if (op == DTB_OP_MEAN) { fill_u64_kernel<<<fgrid, 256, 0, s>>>(acc1, ng, 0ull); count_launch(); }
   DTB_CUDA_CHECK(cudaGetLastError());
   if (n > 0) {
-    int rc = DTB_OK;
-    switch (op) {
-      case DTB_OP_SUM:
-        rc = isflt ? dispatch_T<CAT_SUMF>(stype, value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 0, s)
-                   : dispatch_T<CAT_SUMI>(stype, value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 0, s);
-        break;
-      case DTB_OP_MEAN: rc = dispatch_T<CAT_MEAN>(stype, value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 0, s); break;
-      case DTB_OP_MIN:  rc = dispatch_T<CAT_MINMAX>(stype, value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 1, s); break;
-      case DTB_OP_MAX:  rc = dispatch_T<CAT_MINMAX>(stype, value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 0, s); break;
-      case DTB_OP_COUNT:   rc = dispatch_T<CAT_COUNT>(stype, value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 0, s); break;
-      case DTB_OP_COUNTNA: rc = dispatch_T<CAT_COUNT>(stype, value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 1, s); break;
-      default: set_error("unknown reducer"); return DTB_EINVAL;
-    }
-    if (rc != DTB_OK) return rc;
+    DTB_TRY(with_stype(stype, "internal: reducer of stype ", [&](auto t) {
+      typedef typename decltype(t)::type T;
+      constexpr int SUM = std::is_floating_point<T>::value ? CAT_SUMF : CAT_SUMI;
+      switch (op) {
+        case DTB_OP_SUM:     return run_reduce<T, SUM>(value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 0, s);
+        case DTB_OP_MEAN:    return run_reduce<T, CAT_MEAN>(value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 0, s);
+        case DTB_OP_MIN:     return run_reduce<T, CAT_MINMAX>(value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 1, s);
+        case DTB_OP_MAX:     return run_reduce<T, CAT_MINMAX>(value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 0, s);
+        case DTB_OP_COUNT:   return run_reduce<T, CAT_COUNT>(value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 0, s);
+        case DTB_OP_COUNTNA: return run_reduce<T, CAT_COUNT>(value, nv, order, order_is64, offsets, ng, n, acc0, acc1, 1, s);
+      }
+      set_error("unknown reducer"); return DTB_EINVAL;
+    }));
   }
   GroupRows gr;                                 // extra: the zero lookup's marks, float min / max (reduce_extra_bytes)
   gr.v = value; gr.nv = nv; gr.order = order; gr.order_is64 = order_is64; gr.offsets = offsets; gr.n = n;
   gr.zpos = (u64*)extra;
-  DTB_TRY(zero_fix_begin(op, stype, gr, ng, s));
-  finalize_kernel<<<fgrid, 256, 0, s>>>(op, stype, out_st, acc0, acc1, ng, out, gr);
-  count_launch();
-  DTB_CUDA_CHECK(cudaGetLastError());
-  return zero_fix_end(op, stype, gr, ng, out, s);
+  return finalize(op, stype, acc0, acc1, nullptr, ng, out, gr, s);
 }
 
 int reduce_out_stype_host(int op, int st) { return reduce_out_stype(op, st); }
@@ -670,7 +645,7 @@ __global__ void offsets_check_kernel(const int32_t* __restrict__ offsets, int64_
 
 int launch_offsets_check(const int32_t* offsets, int64_t ng, int* d_bad, cudaStream_t s) {
   if (ng == 0) return DTB_OK;
-  const int fgrid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
+  const int fgrid = grid_for((ng + 255) / 256, 8);
   offsets_check_kernel<<<fgrid, 256, 0, s>>>(offsets, ng, d_bad);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
@@ -679,7 +654,7 @@ int launch_offsets_check(const int32_t* offsets, int64_t ng, int* d_bad, cudaStr
 
 int launch_nrows(const int32_t* offsets, int64_t ng, void* out, cudaStream_t s) {
   if (ng == 0) return DTB_OK;
-  const int fgrid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
+  const int fgrid = grid_for((ng + 255) / 256, 8);
   nrows_kernel<<<fgrid, 256, 0, s>>>(offsets, ng, (int64_t*)out);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
@@ -705,14 +680,6 @@ int launch_nrows(const int32_t* offsets, int64_t ng, void* out, cudaStream_t s) 
 enum { CUM_SUMI, CUM_SUMF, CUM_PRODI, CUM_PRODF, CUM_MIN, CUM_MAX, CUM_FILL };
 
 template <typename T> struct CumMM { typename RawKey<T>::load_t b; };   // the latest extreme, or T's NA = none
-
-// T's NA as stored: the integer sentinel, or the quiet NaN dtb_gather writes
-template <typename T> __device__ __forceinline__ typename RawKey<T>::load_t raw_na() {
-  typedef typename RawKey<T>::load_t O;
-  if constexpr (std::is_same<T, float>::value) return (O)0x7FC00000u;
-  else if constexpr (std::is_same<T, double>::value) return (O)0x7FF8000000000000ull;
-  else return NaOf<T>::v();
-}
 
 template <int K, typename T> struct Cum;
 
@@ -774,8 +741,8 @@ template <typename T> struct Cum<CUM_PRODF, T> {
   static __device__ __forceinline__ O result(const S& a) {
     bool valid;
     const double r = prodf_value(a, valid);
-    if constexpr (std::is_same<T, float>::value) return valid ? (O)__float_as_uint((float)r) : (O)0x7FC00000u;
-    else return valid ? (O)__double_as_longlong(r) : (O)0x7FF8000000000000ull;
+    if constexpr (std::is_same<T, float>::value) return valid ? (O)__float_as_uint((float)r) : raw_na<T>();
+    else return valid ? (O)__double_as_longlong(r) : raw_na<T>();
   }
 };
 
@@ -1010,12 +977,9 @@ static int run_cumulative(const void* v, int64_t nv, const void* order, int orde
   typename C::S* tagg = (typename C::S*)scratch;
   u32* thead = (u32*)((char*)scratch + (size_t)ntiles * sizeof(Partial<CAT_PRODF>));
   typename C::O* o = (typename C::O*)out;
-  if (order_is64)
-    cum_tile_kernel<K, T, REV, int64_t><<<(unsigned)ntiles, RT, 0, s>>>((const L*)v, nv, (const int64_t*)order,
-                                                                         offsets, ng, n, o, tagg, thead);
-  else
-    cum_tile_kernel<K, T, REV, int32_t><<<(unsigned)ntiles, RT, 0, s>>>((const L*)v, nv, (const int32_t*)order,
-                                                                         offsets, ng, n, o, tagg, thead);
+  with_order(order, order_is64, [&](auto ord) {
+    cum_tile_kernel<K, T, REV><<<(unsigned)ntiles, RT, 0, s>>>((const L*)v, nv, ord, offsets, ng, n, o, tagg, thead);
+  });
   cum_carry_kernel<K, T><<<1, CARRY_T, 0, s>>>(tagg, thead, ntiles);
   cum_emit_kernel<K, T, REV><<<(unsigned)ntiles, RT, 0, s>>>(offsets, ng, n, o, tagg);
   count_launch(3);
@@ -1037,33 +1001,19 @@ int launch_cumulative(int op, int reverse, const void* v, int stype, int64_t nv,
                       const int32_t* offsets, int64_t ng, int64_t n, void* scratch, void* out, cudaStream_t s)
 {
   if (n <= 0) return DTB_OK;
-#define DTB_CUM_ARGS reverse, v, nv, order, order_is64, offsets, ng, n, scratch, out, s
-#define DTB_CUM_INT(T) \
-  switch (op) {                                                                                    \
-    case DTB_OP_SUM:  return run_cumulative_dir<CUM_SUMI, T>(DTB_CUM_ARGS);                        \
-    case DTB_OP_PROD: return run_cumulative_dir<CUM_PRODI, T>(DTB_CUM_ARGS);                       \
-    case DTB_OP_MIN:  return run_cumulative_dir<CUM_MIN, T>(DTB_CUM_ARGS);                         \
-    case DTB_OP_MAX:  return run_cumulative_dir<CUM_MAX, T>(DTB_CUM_ARGS);                         \
-  } break;
-#define DTB_CUM_FLT(T) \
-  switch (op) {                                                                                    \
-    case DTB_OP_SUM:  return run_cumulative_dir<CUM_SUMF, T>(DTB_CUM_ARGS);                        \
-    case DTB_OP_PROD: return run_cumulative_dir<CUM_PRODF, T>(DTB_CUM_ARGS);                       \
-    case DTB_OP_MIN:  return run_cumulative_dir<CUM_MIN, T>(DTB_CUM_ARGS);                         \
-    case DTB_OP_MAX:  return run_cumulative_dir<CUM_MAX, T>(DTB_CUM_ARGS);                         \
-  } break;
-  switch (stype) {
-    case DTB_STYPE_BOOL: case DTB_STYPE_INT8: DTB_CUM_INT(int8_t)
-    case DTB_STYPE_INT16: DTB_CUM_INT(int16_t)
-    case DTB_STYPE_INT32: case DTB_STYPE_DATE32: DTB_CUM_INT(int32_t)
-    case DTB_STYPE_INT64: case DTB_STYPE_TIME64: DTB_CUM_INT(int64_t)
-    case DTB_STYPE_FLOAT32: DTB_CUM_FLT(float)
-    case DTB_STYPE_FLOAT64: DTB_CUM_FLT(double)
-  }
-#undef DTB_CUM_FLT
-#undef DTB_CUM_INT
-#undef DTB_CUM_ARGS
-  set_error("internal: cumulative function / stype combination"); return DTB_EINVAL;
+  return with_stype(stype, "internal: cumulative function of stype ", [&](auto t) {
+    typedef typename decltype(t)::type T;
+    constexpr bool ISF = std::is_floating_point<T>::value;
+    switch (op) {
+      case DTB_OP_SUM:
+        return run_cumulative_dir<ISF ? CUM_SUMF : CUM_SUMI, T>(reverse, v, nv, order, order_is64, offsets, ng, n, scratch, out, s);
+      case DTB_OP_PROD:
+        return run_cumulative_dir<ISF ? CUM_PRODF : CUM_PRODI, T>(reverse, v, nv, order, order_is64, offsets, ng, n, scratch, out, s);
+      case DTB_OP_MIN: return run_cumulative_dir<CUM_MIN, T>(reverse, v, nv, order, order_is64, offsets, ng, n, scratch, out, s);
+      case DTB_OP_MAX: return run_cumulative_dir<CUM_MAX, T>(reverse, v, nv, order, order_is64, offsets, ng, n, scratch, out, s);
+    }
+    set_error("internal: cumulative function / stype combination"); return DTB_EINVAL;
+  });
 }
 
 // ===========================================================================
@@ -1161,12 +1111,9 @@ static int run_shift(const void* v, int64_t nv, const void* order, int order_is6
 {
   typedef typename RawKey<T>::load_t L;
   const unsigned grid = (unsigned)((n + RTILE - 1) / RTILE);
-  if (order_is64)
-    group_row_kernel<ROW_SHIFT, T, int64_t><<<grid, RT, 0, s>>>((const L*)v, nv, (const int64_t*)order, offsets, ng, n,
-                                                                 shift, 0, (L*)out);
-  else
-    group_row_kernel<ROW_SHIFT, T, int32_t><<<grid, RT, 0, s>>>((const L*)v, nv, (const int32_t*)order, offsets, ng, n,
-                                                                 shift, 0, (L*)out);
+  with_order(order, order_is64, [&](auto o) {
+    group_row_kernel<ROW_SHIFT, T><<<grid, RT, 0, s>>>((const L*)v, nv, o, offsets, ng, n, shift, 0, (L*)out);
+  });
   count_launch(1);
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;
@@ -1180,17 +1127,9 @@ int launch_shift(const void* v, int stype, int64_t nv, const void* order, int or
   // positions are below 2^31, so every |shift| beyond that puts each source outside its group
   const int64_t lim = (int64_t)1 << 32;
   shift = shift > lim ? lim : (shift < -lim ? -lim : shift);
-#define DTB_SHIFT_ARGS v, nv, order, order_is64, offsets, ng, n, shift, out, s
-  switch (stype) {
-    case DTB_STYPE_BOOL: case DTB_STYPE_INT8: return run_shift<int8_t>(DTB_SHIFT_ARGS);
-    case DTB_STYPE_INT16: return run_shift<int16_t>(DTB_SHIFT_ARGS);
-    case DTB_STYPE_INT32: case DTB_STYPE_DATE32: return run_shift<int32_t>(DTB_SHIFT_ARGS);
-    case DTB_STYPE_INT64: case DTB_STYPE_TIME64: return run_shift<int64_t>(DTB_SHIFT_ARGS);
-    case DTB_STYPE_FLOAT32: return run_shift<float>(DTB_SHIFT_ARGS);
-    case DTB_STYPE_FLOAT64: return run_shift<double>(DTB_SHIFT_ARGS);
-  }
-#undef DTB_SHIFT_ARGS
-  set_error("internal: shift of stype " + std::to_string(stype)); return DTB_EINVAL;
+  return with_stype(stype, "internal: shift of stype ", [&](auto t) {
+    return run_shift<typename decltype(t)::type>(v, nv, order, order_is64, offsets, ng, n, shift, out, s);
+  });
 }
 
 // out: n elements of the value's stype; scratch: cumulative_scratch_bytes(n) of device memory.
@@ -1198,17 +1137,10 @@ int launch_fillna(int reverse, const void* v, int stype, int64_t nv, const void*
                   const int32_t* offsets, int64_t ng, int64_t n, void* scratch, void* out, cudaStream_t s)
 {
   if (n <= 0) return DTB_OK;
-#define DTB_FILL_ARGS reverse, v, nv, order, order_is64, offsets, ng, n, scratch, out, s
-  switch (stype) {
-    case DTB_STYPE_BOOL: case DTB_STYPE_INT8: return run_cumulative_dir<CUM_FILL, int8_t>(DTB_FILL_ARGS);
-    case DTB_STYPE_INT16: return run_cumulative_dir<CUM_FILL, int16_t>(DTB_FILL_ARGS);
-    case DTB_STYPE_INT32: case DTB_STYPE_DATE32: return run_cumulative_dir<CUM_FILL, int32_t>(DTB_FILL_ARGS);
-    case DTB_STYPE_INT64: case DTB_STYPE_TIME64: return run_cumulative_dir<CUM_FILL, int64_t>(DTB_FILL_ARGS);
-    case DTB_STYPE_FLOAT32: return run_cumulative_dir<CUM_FILL, float>(DTB_FILL_ARGS);
-    case DTB_STYPE_FLOAT64: return run_cumulative_dir<CUM_FILL, double>(DTB_FILL_ARGS);
-  }
-#undef DTB_FILL_ARGS
-  set_error("internal: fillna of stype " + std::to_string(stype)); return DTB_EINVAL;
+  return with_stype(stype, "internal: fillna of stype ", [&](auto t) {
+    return run_cumulative_dir<CUM_FILL, typename decltype(t)::type>(reverse, v, nv, order, order_is64, offsets, ng, n,
+                                                                    scratch, out, s);
+  });
 }
 
 // kind: DTB_GROUP_CUMCOUNT or DTB_GROUP_NGROUP (checked by the caller); out: n int64 values.
@@ -1256,39 +1188,6 @@ direct_reduce_kernel(KSrc ksrc, int gshift, const typename RawKey<T>::load_t* __
     Partial<CAT> part; p_init(part, flag);
     p_add<T, CAT>(part, v[i], true, flag);
     p_flush(part, (int64_t)x, acc0, acc1, flag);
-  }
-}
-
-__global__ void finalize_direct_kernel(int op, int in_stype, int out_stype, const u64* __restrict__ acc0,
-                                       const u64* __restrict__ acc1, const u32* __restrict__ gkeys,
-                                       int64_t ng, void* out, const GroupRows gr)
-{
-  const bool in_float = (in_stype == DTB_STYPE_FLOAT32 || in_stype == DTB_STYPE_FLOAT64);
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += stride) {
-    const u32 x = gkeys ? gkeys[g] : (u32)g;          // NULL: the accumulators are indexed by group
-    const u64 a = acc0[x];
-    bool valid = true; u64 bits = a;
-    switch (op) {
-      case DTB_OP_SUM:
-        if (out_stype == DTB_STYPE_FLOAT32) bits = __float_as_uint((float)__longlong_as_double((long long)a));
-        break;
-      case DTB_OP_MEAN: {
-        const u64 c = acc1[x];
-        valid = c != 0;
-        const double m = __longlong_as_double((long long)a) / (double)c;
-        bits = (out_stype == DTB_STYPE_FLOAT32) ? (u64)__float_as_uint((float)m) : (u64)__double_as_longlong(m);
-        break; }
-      case DTB_OP_MIN: case DTB_OP_MAX: {
-        const bool is_min = (op == DTB_OP_MIN);
-        valid = is_min ? (a != ~0ull) : (a != 0ull);
-        if (in_float) bits = (in_stype == DTB_STYPE_FLOAT32) ? (u64)f32_unimage((u32)a) : f64_unimage(a);
-        else bits = (is_min ? a + 1 : a) ^ 0x8000000000000000ull;
-        if (in_float && valid && is_float_zero(in_stype, bits)) bits = zero_minmax_bits(gr, in_stype, g, ng, bits);
-        break; }
-      default: break;
-    }
-    store_result(out, out_stype, g, valid, bits);
   }
 }
 
@@ -1445,65 +1344,32 @@ static int run_direct(const DirectPlan& dp, const KSrc& ks, int gshift, const vo
                       int flag, cudaStream_t s)
 {
   typedef typename RawKey<T>::load_t L;
-  int64_t want = (n + 511) / 512;
-  if (dp.kind == DIRECT_SMALL) {
-    int grid = (int)(want > NUM_SMS * 4 ? NUM_SMS * 4 : want);
-    direct_reduce_small_kernel<T, CAT, KSrc><<<grid, 512, 0, s>>>(ks, gshift, (const L*)v, n, (int)dp.nslots,
-                                                                  (const uint16_t*)dp.map, acc0, acc1, flag);
-    count_launch();
-    DTB_CUDA_CHECK(cudaGetLastError());
-    return DTB_OK;
-  }
-  if (dp.kind == DIRECT_HOT) {
-    int grid = (int)(want > NUM_SMS * 4 ? NUM_SMS * 4 : want);
-    direct_reduce_hot_kernel<T, CAT, KSrc><<<grid, 512, 0, s>>>(ks, gshift, (const L*)v, n, (const uint8_t*)dp.map,
-                                                                acc0, acc1, flag);
-    count_launch();
-    DTB_CUDA_CHECK(cudaGetLastError());
-    return DTB_OK;
-  }
-  int grid = (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : want);
-  direct_reduce_kernel<T, CAT, KSrc><<<grid, 512, 0, s>>>(ks, gshift, (const L*)v, n, acc0, acc1, flag);
+  const int64_t want = (n + 511) / 512;
+  if (dp.kind == DIRECT_SMALL)
+    direct_reduce_small_kernel<T, CAT, KSrc><<<grid_for(want, 4), 512, 0, s>>>(ks, gshift, (const L*)v, n, (int)dp.nslots,
+                                                                               (const uint16_t*)dp.map, acc0, acc1, flag);
+  else if (dp.kind == DIRECT_HOT)
+    direct_reduce_hot_kernel<T, CAT, KSrc><<<grid_for(want, 4), 512, 0, s>>>(ks, gshift, (const L*)v, n,
+                                                                             (const uint8_t*)dp.map, acc0, acc1, flag);
+  else
+    direct_reduce_kernel<T, CAT, KSrc><<<grid_for(want, 16), 512, 0, s>>>(ks, gshift, (const L*)v, n, acc0, acc1, flag);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;
 }
 
-template <int CAT, typename KSrc>
-static int direct_T(const DirectPlan& dp, int st, const KSrc& ks, int gshift, const void* v, int64_t n, u64* acc0,
-                    u64* acc1, int flag, cudaStream_t s)
-{
-  switch (st) {
-    case DTB_STYPE_BOOL: case DTB_STYPE_INT8:
-      if constexpr (CAT != CAT_SUMF) return run_direct<int8_t, CAT>(dp, ks, gshift, v, n, acc0, acc1, flag, s); break;
-    case DTB_STYPE_INT16:
-      if constexpr (CAT != CAT_SUMF) return run_direct<int16_t, CAT>(dp, ks, gshift, v, n, acc0, acc1, flag, s); break;
-    case DTB_STYPE_INT32:
-      if constexpr (CAT != CAT_SUMF) return run_direct<int32_t, CAT>(dp, ks, gshift, v, n, acc0, acc1, flag, s); break;
-    case DTB_STYPE_INT64:
-      if constexpr (CAT != CAT_SUMF) return run_direct<int64_t, CAT>(dp, ks, gshift, v, n, acc0, acc1, flag, s); break;
-    case DTB_STYPE_FLOAT32:
-      if constexpr (CAT != CAT_SUMI) return run_direct<float, CAT>(dp, ks, gshift, v, n, acc0, acc1, flag, s); break;
-    case DTB_STYPE_FLOAT64:
-      if constexpr (CAT != CAT_SUMI) return run_direct<double, CAT>(dp, ks, gshift, v, n, acc0, acc1, flag, s); break;
-  }
-  set_error("internal: reducer/stype combination"); return DTB_EINVAL;
-}
-
-template <typename KSrc>
-static int direct_op(const DirectPlan& dp, int op, int st, const KSrc& ks, int gshift, const void* v, int64_t n,
+template <typename T, typename KSrc>
+static int direct_op(const DirectPlan& dp, int op, const KSrc& ks, int gshift, const void* v, int64_t n,
                      u64* acc0, u64* acc1, cudaStream_t s)
 {
-  const bool isflt = (st == DTB_STYPE_FLOAT32 || st == DTB_STYPE_FLOAT64);
+  constexpr int SUM = std::is_floating_point<T>::value ? CAT_SUMF : CAT_SUMI;
   switch (op) {
-    case DTB_OP_SUM:
-      return isflt ? direct_T<CAT_SUMF>(dp, st, ks, gshift, v, n, acc0, acc1, 0, s)
-                   : direct_T<CAT_SUMI>(dp, st, ks, gshift, v, n, acc0, acc1, 0, s);
-    case DTB_OP_MEAN:    return direct_T<CAT_MEAN>(dp, st, ks, gshift, v, n, acc0, acc1, 0, s);
-    case DTB_OP_MIN:     return direct_T<CAT_MINMAX>(dp, st, ks, gshift, v, n, acc0, acc1, 1, s);
-    case DTB_OP_MAX:     return direct_T<CAT_MINMAX>(dp, st, ks, gshift, v, n, acc0, acc1, 0, s);
-    case DTB_OP_COUNT:   return direct_T<CAT_COUNT>(dp, st, ks, gshift, v, n, acc0, acc1, 0, s);
-    case DTB_OP_COUNTNA: return direct_T<CAT_COUNT>(dp, st, ks, gshift, v, n, acc0, acc1, 1, s);
+    case DTB_OP_SUM:     return run_direct<T, SUM>(dp, ks, gshift, v, n, acc0, acc1, 0, s);
+    case DTB_OP_MEAN:    return run_direct<T, CAT_MEAN>(dp, ks, gshift, v, n, acc0, acc1, 0, s);
+    case DTB_OP_MIN:     return run_direct<T, CAT_MINMAX>(dp, ks, gshift, v, n, acc0, acc1, 1, s);
+    case DTB_OP_MAX:     return run_direct<T, CAT_MINMAX>(dp, ks, gshift, v, n, acc0, acc1, 0, s);
+    case DTB_OP_COUNT:   return run_direct<T, CAT_COUNT>(dp, ks, gshift, v, n, acc0, acc1, 0, s);
+    case DTB_OP_COUNTNA: return run_direct<T, CAT_COUNT>(dp, ks, gshift, v, n, acc0, acc1, 1, s);
   }
   set_error("unknown reducer"); return DTB_EINVAL;
 }
@@ -1541,7 +1407,7 @@ int plan_direct(int64_t table, const uint32_t* gkeys, const int32_t* offsets, in
   if (gmax > hot_at) {
     const int64_t key_thresh = (n / 2048 > 1024) ? n / 2048 : 1024;  // at most 2048 keys can exceed it
     DTB_CUDA_CHECK(cudaMemsetAsync(map_scratch, 0, (size_t)table, s));
-    const int grid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
+    const int grid = grid_for((ng + 255) / 256, 8);
     hot_map_kernel<<<grid, 256, 0, s>>>(gkeys, offsets, ng, (u32)key_thresh, (uint8_t*)map_scratch);
     count_launch();
     DTB_CUDA_CHECK(cudaGetLastError());
@@ -1556,7 +1422,7 @@ int plan_direct(int64_t table, const uint32_t* gkeys, const int32_t* offsets, in
 int launch_direct_init(int op, const DirectPlan& dp, int64_t table, u64* acc0, u64* acc1, cudaStream_t s)
 {
   if (dp.kind == DIRECT_SMALL) table = dp.nslots;                // only the used accumulators are initialised
-  const int tgrid = (int)((table + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (table + 255) / 256);
+  const int tgrid = grid_for((table + 255) / 256, 8);
   fill_u64_kernel<<<tgrid, 256, 0, s>>>(acc0, table, (op == DTB_OP_MIN) ? ~0ull : 0ull);
   count_launch();
   if (op == DTB_OP_MEAN) { fill_u64_kernel<<<tgrid, 256, 0, s>>>(acc1, table, 0ull); count_launch(); }
@@ -1570,29 +1436,17 @@ int launch_direct_accumulate_rows(int op, const KeyPlan& kp, const DirectPlan& d
 {
   const int out_st = reduce_out_stype(op, stype);
   if (!out_st) { set_error("Invalid column type in reducer"); return DTB_EINVAL; }
-  if (n > 0) {
-    int rc;
-    if (kp.nkeys == 1) {
-      const KeyNorm& k = kp.k[0];
-#define DTB_CASE(TK) { DirectRawKey<TK> ks; ks.src.init(k); \
-                       rc = direct_op(dp, op, stype, ks, kp.group_shift, value, n, acc0, acc1, s); break; }
-      switch (k.stype) {
-        case DTB_STYPE_BOOL: case DTB_STYPE_INT8:    DTB_CASE(int8_t)
-        case DTB_STYPE_INT16:                        DTB_CASE(int16_t)
-        case DTB_STYPE_INT32: case DTB_STYPE_DATE32: DTB_CASE(int32_t)
-        case DTB_STYPE_INT64: case DTB_STYPE_TIME64: DTB_CASE(int64_t)
-        case DTB_STYPE_FLOAT32:                      DTB_CASE(float)
-        case DTB_STYPE_FLOAT64:                      DTB_CASE(double)
-        default: set_error("internal: bad key stype"); return DTB_EINVAL;
-      }
-#undef DTB_CASE
-    } else {
-      DirectComposite ks; ks.kp = kp;
-      rc = direct_op(dp, op, stype, ks, kp.group_shift, value, n, acc0, acc1, s);
-    }
-    if (rc != DTB_OK) return rc;
-  }
-  return DTB_OK;
+  if (n <= 0) return DTB_OK;
+  auto accumulate = [&](const auto& ks) {
+    return with_stype(stype, "internal: reducer of stype ", [&](auto t) {
+      return direct_op<typename decltype(t)::type>(dp, op, ks, kp.group_shift, value, n, acc0, acc1, s);
+    });
+  };
+  if (kp.nkeys != 1) { DirectComposite ks; ks.kp = kp; return accumulate(ks); }
+  return with_stype(kp.k[0].stype, "internal: key of stype ", [&](auto t) {
+    DirectRawKey<typename decltype(t)::type> ks; ks.src.init(kp.k[0]);
+    return accumulate(ks);
+  });
 }
 
 // Stage 2: out[g] = finalize(acc[gkeys[g]]) in the reference's output stype / NA rules; a dense-mapped small table
@@ -1600,16 +1454,7 @@ int launch_direct_accumulate_rows(int op, const KeyPlan& kp, const DirectPlan& d
 int launch_direct_finalize(int op, int stype, const u64* acc0, const u64* acc1, const DirectPlan& dp,
                            const uint32_t* gkeys, int64_t ng, void* out, const GroupRows& rows, cudaStream_t s)
 {
-  const int out_st = reduce_out_stype(op, stype);
-  if (!out_st) { set_error("Invalid column type in reducer"); return DTB_EINVAL; }
-  if (ng == 0) return DTB_OK;
-  if (dp.kind == DIRECT_SMALL && dp.map) gkeys = nullptr;
-  const int fgrid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
-  DTB_TRY(zero_fix_begin(op, stype, rows, ng, s));
-  finalize_direct_kernel<<<fgrid, 256, 0, s>>>(op, stype, out_st, acc0, acc1, gkeys, ng, out, rows);
-  count_launch();
-  DTB_CUDA_CHECK(cudaGetLastError());
-  return zero_fix_end(op, stype, rows, ng, out, s);
+  return finalize(op, stype, acc0, acc1, (dp.kind == DIRECT_SMALL && dp.map) ? nullptr : gkeys, ng, out, rows, s);
 }
 
 // ---- reducers fed piecewise: the first valid zero of every group, for float min / max ----------------
@@ -1620,7 +1465,7 @@ __global__ void inverse_order_kernel(const int32_t* __restrict__ order, int64_t 
 
 int launch_inverse_order(const int32_t* order, int64_t n, int32_t* inv, cudaStream_t s) {
   if (n == 0) return DTB_OK;
-  const int grid = (int)((n + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (n + 255) / 256);
+  const int grid = grid_for((n + 255) / 256, 8);
   inverse_order_kernel<<<grid, 256, 0, s>>>(order, n, inv);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
@@ -1647,7 +1492,7 @@ __global__ void first_zero_rows_kernel(const typename RawKey<T>::load_t* __restr
 int launch_first_zero_rows(const void* value_rows, int stype, int64_t row0, int64_t nrows, const int32_t* inv,
                            const int32_t* offsets, int64_t ng, u64* first_zero, cudaStream_t s) {
   if (nrows == 0 || ng == 0) return DTB_OK;
-  const int grid = (int)((nrows + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (nrows + 255) / 256);
+  const int grid = grid_for((nrows + 255) / 256, 8);
   if (stype == DTB_STYPE_FLOAT32)
     first_zero_rows_kernel<float><<<grid, 256, 0, s>>>((const u32*)value_rows, row0, nrows, inv, offsets, ng, first_zero);
   else
@@ -1671,7 +1516,7 @@ int launch_group_keys(const void* sorted_keys, int key_bytes, const int32_t* off
                       int64_t ng, uint32_t* gkeys, cudaStream_t s)
 {
   if (ng == 0) return DTB_OK;
-  const int grid = (int)((ng + 255) / 256 > NUM_SMS * 8 ? NUM_SMS * 8 : (ng + 255) / 256);
+  const int grid = grid_for((ng + 255) / 256, 8);
   if (key_bytes == 4) group_keys_kernel<u32><<<grid, 256, 0, s>>>((const u32*)sorted_keys, offsets, gshift, ng, gkeys);
   else                group_keys_kernel<u64><<<grid, 256, 0, s>>>((const u64*)sorted_keys, offsets, gshift, ng, gkeys);
   count_launch();
@@ -1700,39 +1545,21 @@ gather_kernel(const E* __restrict__ src, int64_t nsrc, const OrdT* __restrict__ 
   }
 }
 
-template <typename E>
-static int run_gather(const void* src, int64_t nsrc, const void* order, int order_is64, int64_t n,
-                      void* out, E na, cudaStream_t s)
-{
-  if (n == 0) return DTB_OK;
-  int64_t want = (n + 1023) / 1024;
-  int grid = (int)(want > NUM_SMS * 16 ? NUM_SMS * 16 : want);
-  if (order_is64) gather_kernel<E, int64_t><<<grid, 256, 0, s>>>((const E*)src, nsrc, (const int64_t*)order, n, (E*)out, na);
-  else            gather_kernel<E, int32_t><<<grid, 256, 0, s>>>((const E*)src, nsrc, (const int32_t*)order, n, (E*)out, na);
-  count_launch();
-  DTB_CUDA_CHECK(cudaGetLastError());
-  return DTB_OK;
-}
-
 int launch_gather(const void* src, int stype, int64_t nrows_src, const void* order,
                   int order_is64, int64_t n, void* out, cudaStream_t s)
 {
-  switch (stype) {
-    case DTB_STYPE_BOOL: case DTB_STYPE_INT8:
-      return run_gather<uint8_t>(src, nrows_src, order, order_is64, n, out, (uint8_t)0x80, s);
-    case DTB_STYPE_INT16:
-      return run_gather<uint16_t>(src, nrows_src, order, order_is64, n, out, (uint16_t)0x8000, s);
-    case DTB_STYPE_INT32: case DTB_STYPE_DATE32:
-      return run_gather<u32>(src, nrows_src, order, order_is64, n, out, 0x80000000u, s);
-    case DTB_STYPE_FLOAT32:
-      return run_gather<u32>(src, nrows_src, order, order_is64, n, out, 0x7FC00000u, s);
-    case DTB_STYPE_INT64: case DTB_STYPE_TIME64:
-      return run_gather<u64>(src, nrows_src, order, order_is64, n, out, 0x8000000000000000ull, s);
-    case DTB_STYPE_FLOAT64:
-      return run_gather<u64>(src, nrows_src, order, order_is64, n, out, 0x7FF8000000000000ull, s);
-  }
-  set_error("Unable to gather Column of stype " + std::to_string(stype));
-  return DTB_ENOTIMPL;
+  return with_stype(stype, "Unable to gather Column of stype ", [&](auto t) {
+    typedef typename decltype(t)::type T;
+    typedef bits_t<T> E;
+    if (n == 0) return DTB_OK;
+    with_order(order, order_is64, [&](auto o) {
+      gather_kernel<E><<<grid_for((n + 1023) / 1024, 16), 256, 0, s>>>((const E*)src, nrows_src, o, n, (E*)out,
+                                                                       (E)raw_na<T>());
+    });
+    count_launch();
+    DTB_CUDA_CHECK(cudaGetLastError());
+    return DTB_OK;
+  });
 }
 
 }  // namespace dtb

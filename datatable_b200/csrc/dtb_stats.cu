@@ -202,7 +202,7 @@ col_stats_hist_kernel(const typename RawKey<T>::load_t* __restrict__ data, int64
 
 template <typename T, bool IS_FLOAT>
 static int run_stats(const void* data, int64_t n, ColStats* d_stats, cudaStream_t s,
-                     unsigned short* tile_hist = nullptr, unsigned short* tile_na = nullptr) {
+                     unsigned short* tile_hist, unsigned short* tile_na) {
   ColStats init;
   if (IS_FLOAT) { init.lo = ~0ull; init.hi = 0ull; }
   else { init.lo = (u64)INT64_MAX; init.hi = (u64)INT64_MIN; }
@@ -216,9 +216,8 @@ static int run_stats(const void* data, int64_t n, ColStats* d_stats, cudaStream_
     DTB_CUDA_CHECK(cudaGetLastError());
   } else if (n > 0) {
     const int threads = 512;
-    int64_t want = (n / (16 / (int)sizeof(T)) + threads - 1) / threads;
-    int grid = (int)(want < 1 ? 1 : (want > NUM_SMS * 8 ? NUM_SMS * 8 : want));
-    col_stats_kernel<T, IS_FLOAT><<<grid, threads, 0, s>>>(
+    const int64_t want = (n / (16 / (int)sizeof(T)) + threads - 1) / threads;
+    col_stats_kernel<T, IS_FLOAT><<<grid_for(want, 8), threads, 0, s>>>(
         reinterpret_cast<const typename RawKey<T>::load_t*>(data), n, d_stats);
     count_launch();
     DTB_CUDA_CHECK(cudaGetLastError());
@@ -227,17 +226,7 @@ static int run_stats(const void* data, int64_t n, ColStats* d_stats, cudaStream_
 }
 
 int launch_col_stats(const void* data, int stype, int64_t n, ColStats* d_stats, cudaStream_t s) {
-  switch (stype) {
-    case DTB_STYPE_BOOL: case DTB_STYPE_INT8:    return run_stats<int8_t,  false>(data, n, d_stats, s);
-    case DTB_STYPE_INT16:                        return run_stats<int16_t, false>(data, n, d_stats, s);
-    case DTB_STYPE_INT32: case DTB_STYPE_DATE32: return run_stats<int32_t, false>(data, n, d_stats, s);
-    case DTB_STYPE_INT64: case DTB_STYPE_TIME64: return run_stats<int64_t, false>(data, n, d_stats, s);
-    case DTB_STYPE_FLOAT32:                      return run_stats<float,   true >(data, n, d_stats, s);
-    case DTB_STYPE_FLOAT64:                      return run_stats<double,  true >(data, n, d_stats, s);
-    default:
-      set_error("Unable to sort Column of stype " + std::to_string(stype));
-      return DTB_ENOTIMPL;
-  }
+  return launch_col_stats_hist(data, stype, n, d_stats, nullptr, nullptr, s);
 }
 
 size_t stats_hist_bytes(int64_t n) { return sizeof(unsigned short) * 256 * (size_t)((n + PASS_TILE - 1) / PASS_TILE) + 256; }
@@ -245,17 +234,10 @@ size_t stats_na_bytes(int64_t n) { return sizeof(unsigned short) * (size_t)((n +
 
 int launch_col_stats_hist(const void* data, int stype, int64_t n, ColStats* d_stats, unsigned short* tile_hist,
                           unsigned short* tile_na, cudaStream_t s) {
-  switch (stype) {
-    case DTB_STYPE_BOOL: case DTB_STYPE_INT8:    return run_stats<int8_t,  false>(data, n, d_stats, s, tile_hist, tile_na);
-    case DTB_STYPE_INT16:                        return run_stats<int16_t, false>(data, n, d_stats, s, tile_hist, tile_na);
-    case DTB_STYPE_INT32: case DTB_STYPE_DATE32: return run_stats<int32_t, false>(data, n, d_stats, s, tile_hist, tile_na);
-    case DTB_STYPE_INT64: case DTB_STYPE_TIME64: return run_stats<int64_t, false>(data, n, d_stats, s, tile_hist, tile_na);
-    case DTB_STYPE_FLOAT32:                      return run_stats<float,   true >(data, n, d_stats, s, tile_hist, tile_na);
-    case DTB_STYPE_FLOAT64:                      return run_stats<double,  true >(data, n, d_stats, s, tile_hist, tile_na);
-    default:
-      set_error("Unable to sort Column of stype " + std::to_string(stype));
-      return DTB_ENOTIMPL;
-  }
+  return with_stype(stype, "Unable to sort Column of stype ", [&](auto t) {
+    typedef typename decltype(t)::type T;
+    return run_stats<T, std::is_floating_point<T>::value>(data, n, d_stats, s, tile_hist, tile_na);
+  });
 }
 
 }  // namespace dtb
