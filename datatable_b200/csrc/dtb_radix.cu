@@ -9,9 +9,9 @@
 //             (shared-memory histogram) -> counts[chunk][digit]
 //   scan    : per digit, exclusive prefix over the chunks; exclusive prefix over the digit
 //             totals -> every (chunk, digit) knows its first output slot
-//   scatter : the CTA walks its chunk tile by tile (4096 rows), ranks the rows of a tile with
-//             warp-level peer masks in shared memory, reorders the tile in shared memory and
-//             writes digit runs out coalesced, keeping the running digit offsets in registers.
+//   scatter : one CTA per tile (8192 rows for 32-bit keys, 4096 for 64-bit keys; PassCfg) ranks the rows
+//             of its tile with warp-level ballots, reorders the tile in shared memory and writes
+//             digit runs out coalesced.
 //
 // No look-back, no status words, no spinning: a first version used single-sweep tiles with
 // a decoupled look-back; with ~600 tiles in flight the look-back walk was 40 % of the stall
@@ -101,7 +101,8 @@ int launch_compose_keys(const KeyPlan& kp, int64_t n, const int32_t* idx, void* 
 // Digits are at most 8 bits (256 bins).  Wider digits were built and measured twice and removed: round 1, two
 // 10-bit ballot-ranked passes over 1024 bins, slower than three 7/7/6-bit passes on 20-bit keys; round 2,
 // 1024/2048 bins ranked with shared-memory atomics, slower scatter -- 16-byte output runs and 16-32 KB of per-warp tables cost more LSU
-// wavefronts than the pass they save.
+// wavefronts than the pass they save.  Round 3, on H100 with the keys narrowed between passes: two 10-bit passes
+// over 1024 bins took 18.3 + 13.0 ms on C2 against 7.8 + 7.3 + 4.5 ms for 7/7/6 (DESIGN 4.2).
 // PASS_THREADS / PASS_IPT / PASS_TILE (4096 rows) / CHUNK_TILES / CHUNK_ROWS (65536 rows per count CTA): dtb_common.cuh
 
 int64_t radix_num_chunks(int64_t n) { return (n + CHUNK_ROWS - 1) / CHUNK_ROWS; }
@@ -359,13 +360,23 @@ template <typename KeyT, int NBINS> struct PassCfg {
   static constexpr int WARPS = PASS_THREADS / 32;
   // the incoming row ids of the tile are staged in shared memory by one TMA bulk copy
   static constexpr bool USE_RIDX = true;
-  static constexpr int MINB = (sizeof(KeyT) == 4) ? 4 : 3;
+  // A scatter tile is TILES consecutive count tiles (of one chunk), ranked and written together.  With 32-bit keys it
+  // is two (8192 rows, 32 per thread): a digit's run per tile is twice as long, so fewer of the written sectors are
+  // partial.  On C2 at 4096 rows the 7-bit passes, 32-row runs, took 1.7 ms more each than the 6-bit passes of 17-bit
+  // keys, 64-row runs, with the same kernel (DESIGN 4.2).  101 KB of shared memory: 2 CTAs (16 warps) per SM.
+  // 64-bit keys keep 4096-row tiles: 8192 would need 134 KB, one CTA per SM.
+  static constexpr int TILES = (sizeof(KeyT) == 4) ? 2 : 1;
+  static constexpr int TILE = PASS_TILE * TILES;
+  static constexpr int IPT = PASS_IPT * TILES;
+  static constexpr int MINB = (sizeof(KeyT) == 4) ? 2 : 3;
   static constexpr size_t SMEM = sizeof(unsigned short) * WARPS * NBINS + sizeof(u32) * (NBINS + 4)
-                               + (sizeof(KeyT) + sizeof(int32_t)) * PASS_TILE
-                               + (USE_RIDX ? sizeof(int32_t) * PASS_TILE : 0);
+                               + (sizeof(KeyT) + sizeof(int32_t)) * TILE
+                               + (USE_RIDX ? sizeof(int32_t) * TILE : 0);
+  static_assert(CHUNK_TILES % TILES == 0, "a scatter tile lies inside one count chunk");
+  static_assert(TILE <= 65536, "tile positions and per-warp counts are 16-bit");
 };
 
-// One tile per CTA.
+// One tile (PassCfg::TILE rows) per CTA.
 // Shared memory: whist[WARPS][NBINS] u16 | bin_dst[NBINS] u32 | skey[TILE] | sidx[TILE] | ridx[TILE]
 // (the per-warp peer-mask table of the rank phase aliases skey/sidx, idle until the reorder phase).
 // With 32-bit keys the sorted tile is staged as interleaved (key, row id) pairs so that the
@@ -377,7 +388,7 @@ __device__ __forceinline__ void scatter_tile(const PassArgs<KeyT, Src>& a, unsig
                                              uint64_t* s_bar, const int64_t base, const int tile_n,
                                              const u32 (&bin_run)[NBINS / PASS_THREADS], const uint2 tl)
 {
-  constexpr int THREADS = PASS_THREADS, IPT = PASS_IPT, TILE = PASS_TILE;
+  constexpr int THREADS = PASS_THREADS, IPT = PassCfg<KeyT, NBINS>::IPT, TILE = PassCfg<KeyT, NBINS>::TILE;
   constexpr int WARPS = THREADS / 32;
   constexpr int BPT = NBINS / THREADS;
   constexpr bool USE_RIDX = PassCfg<KeyT, NBINS>::USE_RIDX;
@@ -552,7 +563,7 @@ template <typename KeyT, typename Src, int NBINS, int MINB, int NB>
 __global__ void __launch_bounds__(PASS_THREADS, MINB)
 scatter_kernel(const __grid_constant__ PassArgs<KeyT, Src> a)
 {
-  constexpr int THREADS = PASS_THREADS, TILE = PASS_TILE;
+  constexpr int THREADS = PASS_THREADS, TILE = PassCfg<KeyT, NBINS>::TILE, TILES = PassCfg<KeyT, NBINS>::TILES;
   constexpr int WARPS = THREADS / 32;
   constexpr int BPT = NBINS / THREADS;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -565,9 +576,9 @@ scatter_kernel(const __grid_constant__ PassArgs<KeyT, Src> a)
   // One tile per CTA: neighbouring tiles run at the same time on different SMs, so the partial
   // sectors at the ends of their digit runs meet in L2 before they are evicted.
   const int tid = threadIdx.x;
-  const int64_t tile = blockIdx.x;
-  const int64_t base = tile * TILE;
+  const int64_t base = (int64_t)blockIdx.x * TILE;
   const int tile_n = (int)((a.n - base) < (int64_t)TILE ? (a.n - base) : (int64_t)TILE);
+  const int64_t tile = (int64_t)blockIdx.x * TILES;             // its first count tile
   const int64_t chunk = tile / CHUNK_TILES;
 
   // first output slot of the thread's digits for this tile: digit base + earlier chunks + earlier
@@ -579,7 +590,12 @@ scatter_kernel(const __grid_constant__ PassArgs<KeyT, Src> a)
     bin_run[j] = a.digit_base[b] + a.chunk_offs[(size_t)chunk * NBINS + b] + (u32)a.tile_pre[(size_t)tile * NBINS + b];
   }
   uint2 tl = make_uint2(0, 0);
-  if constexpr (Src::packed && sizeof(typename Src::raw_t) == 1) { if (a.low_base) tl = a.tile_low[tile]; }
+  if constexpr (Src::packed && sizeof(typename Src::raw_t) == 1) {
+    if (a.low_base) {                                            // v of the first slot of its first count tile and
+      const int64_t last = tile + (tile_n - 1) / PASS_TILE;      // of the last slot of its last one
+      tl = make_uint2(a.tile_low[tile].x, a.tile_low[last].y);
+    }
+  }
 
   if (tile_n == TILE) scatter_tile<KeyT, Src, NBINS, true,  NB>(a, smem_raw, s_wsum, &s_bar, base, tile_n, bin_run, tl);
   else                scatter_tile<KeyT, Src, NBINS, false, NB>(a, smem_raw, s_wsum, &s_bar, base, tile_n, bin_run, tl);
@@ -649,6 +665,7 @@ static int run_scatter(Src src, const PassIO& io, int64_t n, int shift, u32 mask
   a.out_shift = io.out_shift; a.out_bytes = io.out_bytes ? io.out_bytes : (int)sizeof(KeyT);
   a.low_base = io.low_base; a.low_bits = io.low_bits; a.tile_low = tile_low;
   constexpr size_t smem = PassCfg<KeyT, NBINS>::SMEM;
+  constexpr int TILE = PassCfg<KeyT, NBINS>::TILE;
   // NB = ballots per row in the rank phase = digit width, rounded up to a built variant
   const int bits = __builtin_popcount(mask);
   void (*kern)(const PassArgs<KeyT, Src>) =
@@ -656,7 +673,7 @@ static int run_scatter(Src src, const PassIO& io, int64_t n, int shift, u32 mask
     : bits == 7 ? scatter_kernel<KeyT, Src, NBINS, MINB, 7> : scatter_kernel<KeyT, Src, NBINS, MINB, 8>;
   DTB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   ProfScope ps("radix_scatter", s);
-  kern<<<(unsigned)ntiles, PASS_THREADS, smem, s>>>(a);
+  kern<<<(unsigned)((n + TILE - 1) / TILE), PASS_THREADS, smem, s>>>(a);
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;

@@ -507,7 +507,7 @@ DTB_API int dtb_memcpy(void* dst, const void* src, int64_t nbytes, dtb_stream st
 /*
  * Engine options, the analogue of dt.options.sort.* (sort.cc:259-349).
  *   "radix_bits"   largest digit width of the LSD passes: 4..8, or 0 (default) = 8 bits (wider digits were
- *                  built and measured slower twice, DESIGN.md 4.2)
+ *                  built and measured slower three times, the last time on H100, DESIGN.md 4.2)
  *   "verbose"      1 = print the pass plan to stderr: the key columns' bits and shifts, and per sort round
  *                  its passes, the pass that narrows 64-bit keys to 32 bits (-1 = none), whether the first pass
  *                  takes the statistics kernel's histogram, and whether the last pass fills the count table
