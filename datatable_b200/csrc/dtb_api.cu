@@ -156,6 +156,8 @@ struct Arena {
     return DTB_OK;
   }
   void end() { if (depth > 0) depth--; }
+  // bytes the current slab can still hand out without an allocator call
+  size_t room() const { return cur < slabs.size() ? slabs[cur].cap - off : 0; }
   int take(size_t bytes, void** out) {
     bytes = (bytes + 255) & ~(size_t)255;
     while (cur < slabs.size()) {
@@ -472,6 +474,11 @@ struct GroupPlan {
   int64_t ftable = 0;             // entries of each streaming reducer's accumulator tables
   std::vector<BucketCol> bcols;   // the bucketed multi-reducer's value columns
   std::vector<int> bcol_of;       // per fused reducer: its column in bcols, or -1
+  // The first pass carries the value column of fused reducer region_col, and every fused SUM of that column adds the
+  // rows up per digit region of that pass (launch_region_sum) instead of with one L2 atomic per row
+  bool    region_sum = false;
+  int     region_col = -1;
+  dtb_col region_value = {};
 };
 
 // What the stages of one group() call share besides the plan: the key columns in HBM and their statistics, the
@@ -487,6 +494,8 @@ struct GroupBufs {
   DevBuf gcount;                  // the count table (GroupPlan::count_table)
   DevBuf facc;                    // the streaming fused reducers' accumulator tables
   DevBuf bxk;                     // the rows' composite keys, kept for the bucketed reducers
+  DevBuf vperm, rbases;           // region sum: the values in the first pass's slot order, and that pass's digit bases
+  void*  region_keys = nullptr;   // region sum: the keys the first pass wrote
   void*  sorted_keys = nullptr;   // the last round's sorted composite keys
 };
 
@@ -644,6 +653,29 @@ static void plan_group(const dtb_col* keys, int nkeys, const int* flags, int na_
     // buffer the passes only read, and the bucket kernels read them again afterwards
     r.keep_composite = !gp.bcols.empty() && !gp.fused_raw && nrounds == 1 && r.key_bytes == 4;
   }
+
+  // Region sum: a sum over spread-out group keys (more than SMALL_TABLE, every one in its own accumulator) costs one
+  // L2 atomic per row on the direct path.  The first pass puts every row in the region of its first digit and writes
+  // the key bits above it; with at most REGION_MAX_LBITS of them a region's groups fit a 64 KB shared-memory table.
+  // The pass then carries the value column too, and the next passes must leave its keys alone (at most 3 passes).
+  // Few groups in a wide key domain (DIRECT_SMALL, known only after the sort) keep their own path.
+  if (gp.fused_direct && gp.fused_raw && gp.bcols.empty() && gp.ftable > SMALL_TABLE) {
+    const RoundPlan& r = gp.rounds[0];
+    const int np = r.pp.npasses;
+    const bool layout = np >= 2 && np <= 3 && r.pp.shift[0] == 0 && r.kp.group_shift == 0 && r.kdrop[1] == r.pp.bits[0] &&
+                        (r.kout_bytes[0] == 1 || r.kout_bytes[0] == 2) && gp.dbits - r.pp.bits[0] <= REGION_MAX_LBITS;
+    for (int i = 0; layout && i < fr->n; i++)
+      if (fr->spec[i].op == DTB_OP_SUM && reduce_out_stype_host(DTB_OP_SUM, fr->spec[i].value.stype)) {
+        gp.region_sum = true; gp.region_col = i; gp.region_value = fr->spec[i].value;
+        break;
+      }
+  }
+}
+
+// The fused reducer `sp` is a sum over the column the first pass carried (GroupPlan::region_sum).
+static bool takes_region_sum(const GroupPlan& gp, const dtb_reduce_spec& sp) {
+  return gp.region_sum && sp.op == DTB_OP_SUM && sp.value.data == gp.region_value.data &&
+         sp.value.stype == gp.region_value.stype;
 }
 
 static void print_plan(const GroupPlan& gp, int64_t n, int nkeys, const ColStats* st) {
@@ -664,10 +696,13 @@ static void print_plan(const GroupPlan& gp, int64_t n, int nkeys, const ColStats
             ri, r.kp.nkeys, r.kp.total_bits, r.kp.group_shift, r.pp.npasses, r.narrow_after, (int)r.fold,
             (int)(gp.count_table && ri == nrounds - 1), kw.c_str(), r.low_bits);
   }
+  if (gp.region_sum)                                   // planned: the first pass carries the column
+    fprintf(stderr, "[dtb200]   region_sum: reducer=%d stype=%d regions=%d bits_per_region=%d\n", gp.region_col,
+            gp.region_value.stype, 1 << gp.rounds[0].pp.bits[0], gp.dbits - gp.rounds[0].pp.bits[0]);
 }
 
 // The stable LSD passes of every round; the last round writes the RowIndex into `order`.
-static int sort_rounds(const GroupPlan& gp, int64_t n, int nfused, int32_t* order, cudaStream_t s, GroupBufs& b)
+static int sort_rounds(GroupPlan& gp, int64_t n, int nfused, int32_t* order, cudaStream_t s, GroupBufs& b)
 {
   const int nrounds = (int)gp.rounds.size();
   DTB_TRY(b.keyA.alloc((size_t)n * gp.buf_key_bytes, s));
@@ -681,6 +716,26 @@ static int sort_rounds(const GroupPlan& gp, int64_t n, int nfused, int32_t* orde
     DTB_CUDA_CHECK(cudaMemsetAsync(b.gcount.p, 0, sizeof(u32) * (size_t)gp.ctable, s));
   }
   if (gp.fused_direct) DTB_TRY(b.facc.alloc(sizeof(u64) * (size_t)gp.ftable * 2 * (size_t)nfused, s));
+  // The region sum's copy of the values is the last large buffer of the call.  It is taken only if the call's later
+  // scratch (offsets scans, group keys, maps, reducer outputs: O(key domain + groups), at most 2^22 entries of a few
+  // words each) still fits afterwards, in the arena's slab or in free device memory; otherwise the sum takes the
+  // direct path and the arena hands out the same memory as before.
+  if (gp.region_sum) {
+    const size_t arena_cur = t_arena.cur, arena_off = t_arena.off;
+    const int64_t scratch0 = t_stats.scratch_bytes;
+    const size_t later = sizeof(u64) * 8 * (size_t)gp.ftable + ((size_t)64 << 20);
+    size_t free_b = 0, total_b = 0;
+    bool ok = b.rbases.alloc(sizeof(u32) * 256, s) == DTB_OK &&
+              b.vperm.alloc((size_t)n * stype_bytes(gp.region_value.stype), s) == DTB_OK;
+    if (ok && t_arena.room() < later) ok = cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && free_b >= later;
+    if (!ok) {
+      cudaGetLastError();
+      gp.region_sum = false;
+      t_arena.cur = arena_cur; t_arena.off = arena_off;
+      t_stats.scratch_bytes = scratch0;
+      set_error("");
+    }
+  }
   DTB_TL("scratch allocated");
   const int32_t* idx_cur = nullptr;        // rows in the order established by the previous rounds
   for (int ri = 0; ri < nrounds; ri++) {
@@ -730,8 +785,16 @@ static int sort_rounds(const GroupPlan& gp, int64_t n, int nfused, int32_t* orde
       io.keys_out = (last && !r.want_sorted_keys) ? nullptr : kout;
       int32_t* iout = last ? round_out : ((p & 1) ? b.idxB.as<int32_t>() : b.idxA.as<int32_t>());
       io.idx_out = iout;
+      const bool carry = gp.region_sum && p == 0;
+      if (carry) {
+        io.vals = gp.region_value.data; io.vperm = b.vperm.p; io.vbytes = stype_bytes(gp.region_value.stype);
+        if (!io.bases_out) io.bases_out = b.rbases.as<u32>();
+        b.region_keys = kout;                          // no later pass of the round writes this buffer (<= 3 passes)
+      }
       DTB_TRY(launch_radix_pass(io, rk, r.kin_bytes[p], n, pp.shift[p] - r.kdrop[p], pp.bits[p], work.as<u32>(), s,
                                 (gp.count_table && last) ? b.gcount.as<u32>() : nullptr, rk.group_shift));
+      if (carry && io.bases_out != b.rbases.p)
+        DTB_CUDA_CHECK(cudaMemcpyAsync(b.rbases.p, io.bases_out, sizeof(u32) * 256, cudaMemcpyDeviceToDevice, s));
       if (last && r.want_sorted_keys) b.sorted_keys = kout;
       kin = kout;
       kout = (kout == b.keyA.p) ? b.keyB.p : b.keyA.p;
@@ -867,9 +930,11 @@ static int bucketed_reduce(const GroupPlan& gp, int64_t n, GroupBufs& b, std::ve
 // A reducer of the direct-address path (sum..countna over a device column): out[g] = finalize(acc0 / acc1 at the key
 // of group g).  accumulate: every row first folds into the accumulators of its key, in plan_direct's streaming mode
 // dp; otherwise the bucketed sweep has filled them.
+// region (a sum over the column the first pass carried, GroupPlan::region_sum): the rows are added up per digit region
+// of that pass.
 static int direct_reduce(const DirectGroups& dg, const DirectPlan& dp, int op, dtb_col value, const int32_t* order,
                          const int32_t* offsets, int64_t n, int64_t ng, u64* acc0, u64* acc1, bool accumulate,
-                         void* out, cudaStream_t s)
+                         void* out, cudaStream_t s, const GroupPlan* region = nullptr, const GroupBufs* rb = nullptr)
 {
   GroupRows rows;                                  // for the zero lookup: every row is in a group (no NA_REMOVE)
   rows.v = value.data; rows.nv = n; rows.order = order; rows.offsets = offsets; rows.n = n;
@@ -878,7 +943,16 @@ static int direct_reduce(const DirectGroups& dg, const DirectPlan& dp, int op, d
   if (accumulate && ng > 0) {
     ProfScope ps("reduce_direct", s);
     DTB_TRY(launch_direct_init(op, dp, dg.table, acc0, acc1, s));
-    DTB_TRY(launch_direct_accumulate_rows(op, dg.kp, dp, value.data, value.stype, n, acc0, acc1, s));
+    if (region) {
+      const bool hot = dp.kind == DIRECT_HOT;
+      ProfScope pr(hot ? "region_sum_hot" : "region_sum", s);     // inside reduce_direct: tells the paths apart
+      const RoundPlan& r = region->rounds[0];
+      DTB_TRY(launch_region_sum(rb->region_keys, r.kout_bytes[0], r.pp.bits[0], region->dbits - r.pp.bits[0],
+                                (const u32*)rb->rbases.p, rb->vperm.p, value.stype, n,
+                                hot ? (const uint8_t*)dp.map : nullptr, acc0, s));
+    } else {
+      DTB_TRY(launch_direct_accumulate_rows(op, dg.kp, dp, value.data, value.stype, n, acc0, acc1, s));
+    }
   }
   return launch_direct_finalize(op, value.stype, acc0, acc1, dp, (const uint32_t*)dg.gkeys, ng, out, rows, s);
 }
@@ -933,7 +1007,11 @@ static int fused_reduce(const GroupPlan& gp, int64_t n, const int32_t* order, co
                             bw.a1 >= 0 ? w[bw.a1] : nullptr, false, ob.p, s));
     } else if (gp.fused_direct) {
       u64* acc = b.facc.as<u64>() + (size_t)gp.ftable * 2 * i;
-      DTB_TRY(direct_reduce(res.direct, dp, sp.op, sp.value, order, offsets, n, ng, acc, acc + gp.ftable, true, ob.p, s));
+      const bool region = takes_region_sum(gp, sp) && dp.kind != DIRECT_SMALL;
+      if (opt_verbose && takes_region_sum(gp, sp))
+        fprintf(stderr, "[dtb200]   reducer %d: %s\n", i, region ? "region sum" : "direct (few groups)");
+      DTB_TRY(direct_reduce(res.direct, dp, sp.op, sp.value, order, offsets, n, ng, acc, acc + gp.ftable, true, ob.p, s,
+                            region ? &gp : nullptr, &b));
     } else {
       DevIn dv;
       if (sp.op != DTB_OP_NROWS) DTB_TRY(dv.bind(sp.value.data, (size_t)n * stype_bytes(sp.value.stype), s));

@@ -176,6 +176,13 @@ __device__ __forceinline__ void st_relaxed_u64(u64* p, u64 v) {
   asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" :: "l"(p), "l"(v) : "memory");
 }
 
+// The v in [lo, hi] whose rows occupy slot s: the last v with b[v] <= s (b = exclusive scan of the rows per v, so
+// b[lo] <= s; an empty v shares its b with the next one and is never the last).
+__device__ __forceinline__ u32 slot_owner(const u32* b, u32 lo, u32 hi, u32 s) {
+  while (lo < hi) { const u32 mid = (lo + hi + 1) >> 1; if (b[mid] <= s) lo = mid; else hi = mid - 1; }
+  return lo;
+}
+
 __device__ __forceinline__ unsigned lanemask_lt() {
   unsigned m; asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m)); return m;
 }

@@ -129,6 +129,11 @@ struct PassIO {
   uint32_t*       low_hist = nullptr;
   const uint32_t* low_base = nullptr;
   int             low_bits = 0;
+  // First pass over a raw column with 32-bit keys (row id = position) of a region sum (launch_region_sum): the value
+  // column `vals` (vbytes = 1, 2, 4 or 8 per row) travels with the rows, vperm[slot] = vals[row of the slot]
+  const void*     vals = nullptr;
+  void*           vperm = nullptr;
+  int             vbytes = 0;
 };
 
 // One stable pass = count + scan + scatter kernels.  work: radix_pass_work_bytes(n) of scratch.
@@ -213,6 +218,8 @@ int reduce_out_stype_host(int op, int stype);
 int launch_offsets_check(const int32_t* offsets, int64_t ng, int* d_bad, cudaStream_t s);
 
 // Direct-address reducers over a small normalised key domain (see dtb_reduce.cu).
+// Few distinct group keys (<= SMALL_TABLE) fold in per-CTA shared-memory tables (DIRECT_SMALL).
+constexpr int SMALL_TABLE = 2048;
 enum { DIRECT_PLAIN = 0,        // one L2 atomic per row into acc[x]
        DIRECT_SMALL = 1,        // <= 2048 accumulators: per-CTA shared-memory tables (map: uint16 x -> group, or NULL)
        DIRECT_HOT = 2 };        // skewed group sizes: rows of hot keys (map: uint8 hot[x]) fold in shared memory
@@ -230,6 +237,13 @@ int plan_direct(int64_t table, const uint32_t* gkeys, const int32_t* offsets, in
 int launch_direct_init(int op, const DirectPlan& dp, int64_t table, unsigned long long* acc0, unsigned long long* acc1, cudaStream_t s);
 int launch_direct_accumulate_rows(int op, const KeyPlan& kp, const DirectPlan& dp, const void* value, int stype, int64_t n,
                                   unsigned long long* acc0, unsigned long long* acc1, cudaStream_t s);
+// A sum over the rows as the first radix pass left them (GroupPlan::region_sum): the pass put every row in the region of
+// its low rbits key bits (region d = slots [bases[d], bases[d + 1]), bases: the pass's 256 digit bases), and wrote the
+// rest of its group key (lbits <= 13 bits, in words of key_bytes = 1 or 2) to lkey[slot] and its value to vperm[slot].
+// Every row adds its value to acc0[lkey << rbits | d].  hot: the hot-key map of a DIRECT_HOT plan, or NULL.
+constexpr int REGION_MAX_LBITS = 13;
+int launch_region_sum(const void* lkey, int key_bytes, int rbits, int lbits, const uint32_t* bases, const void* vperm,
+                      int stype, int64_t n, const uint8_t* hot, unsigned long long* acc0, cudaStream_t s);
 // out[g] from the accumulators of group key gkeys[g], or of group g when dp is a dense-mapped small table.
 int launch_direct_finalize(int op, int stype, const unsigned long long* acc0, const unsigned long long* acc1,
                            const DirectPlan& dp, const uint32_t* gkeys, int64_t ngroups, void* out, const GroupRows& rows,

@@ -110,13 +110,6 @@ int64_t radix_num_chunks(int64_t n) { return (n + CHUNK_ROWS - 1) / CHUNK_ROWS; 
 // ===========================================================================
 // count: tile_pre[tile][digit] (u16, rows of the digit in the earlier tiles of the chunk) and counts[chunk][digit]
 // ===========================================================================
-// The v in [lo, hi] whose rows occupy slot s: the last v with b[v] <= s (b = exclusive scan of the rows per v, so
-// b[lo] <= s; an empty v shares its b with the next one and is never the last).
-__device__ __forceinline__ u32 slot_owner(const u32* b, u32 lo, u32 hi, u32 s) {
-  while (lo < hi) { const u32 mid = (lo + hi + 1) >> 1; if (b[mid] <= s) lo = mid; else hi = mid - 1; }
-  return lo;
-}
-
 // regions (optional): the previous pass's digit bases.  A slot's region is the previous pass's digit of its row,
 // so low_hist[digit << region_bits | region] counts the rows by the low bits both passes consume.  A tile inside one
 // region adds its digit counts (summed over the chunk's consecutive tiles of that region); only the few tiles that
@@ -331,6 +324,9 @@ struct PassArgs {
   const u32*     low_base;      // 1-byte packed keys of a count-table last pass: key = (in << low_bits) | v(slot)
   int            low_bits;
   const uint2*   tile_low;      // [ntiles] v of the tile's first and last slot
+  const void*    vals;          // first pass of a region sum: vperm[dst] = vals[row] in words of vbytes (PassIO)
+  void*          vperm;
+  int            vbytes;
 };
 
 // ---- TMA 1-D bulk copy (cp.async.bulk, SASS UBLKCP) completing on an mbarrier -----------------------
@@ -559,19 +555,52 @@ __device__ __forceinline__ KeyT staged_key(const KeyT* skey, int q) {
   else return skey[q];
 }
 
-template <typename KeyT, typename Src, int NBINS, int MINB, int NB>
+// The values of a region sum's first pass (VALS below): once the tile's (key, row id) pairs are written, the values are
+// read in row order, coalesced, staged at their rows' tile slots in the pair buffer and written in the same digit runs.
+// inv[tile position] = tile slot and dig[tile slot] = digit were recorded by the write loop.
+template <typename W>
+__device__ __forceinline__ void carry_values(const W* __restrict__ vals, W* __restrict__ vperm, int64_t base, int tile_n,
+                                             const unsigned short* inv, const unsigned char* dig, const u32* bin_dst,
+                                             W* sv)
+{
+  constexpr int VB = 16;                                         // loads in flight per thread
+  for (int p0 = 0; p0 < tile_n; p0 += PASS_THREADS * VB) {
+    W w[VB];
+#pragma unroll
+    for (int j = 0; j < VB; j++) {
+      const int pos = p0 + j * PASS_THREADS + (int)threadIdx.x;
+      w[j] = pos < tile_n ? vals[base + pos] : (W)0;
+    }
+#pragma unroll
+    for (int j = 0; j < VB; j++) {
+      const int pos = p0 + j * PASS_THREADS + (int)threadIdx.x;
+      if (pos < tile_n) sv[inv[pos]] = w[j];
+    }
+  }
+  __syncthreads();
+#pragma unroll 4
+  for (int p = threadIdx.x; p < tile_n; p += PASS_THREADS) vperm[bin_dst[dig[p]] + (u32)p] = sv[p];
+}
+
+// VALS: the first pass of a region sum (PassIO::vals), over a raw column (row id = position) with 32-bit keys
+template <typename KeyT, typename Src, int NBINS, int MINB, int NB, bool VALS>
 __global__ void __launch_bounds__(PASS_THREADS, MINB)
 scatter_kernel(const __grid_constant__ PassArgs<KeyT, Src> a)
 {
   constexpr int THREADS = PASS_THREADS, TILE = PassCfg<KeyT, NBINS>::TILE, TILES = PassCfg<KeyT, NBINS>::TILES;
   constexpr int WARPS = THREADS / 32;
   constexpr int BPT = NBINS / THREADS;
+  static_assert(!VALS || (sizeof(KeyT) == 4 && !Src::packed && PassCfg<KeyT, NBINS>::USE_RIDX),
+                "values travel in the first pass over a raw column with 32-bit keys, staged in the row-id buffer");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ u32 s_wsum[WARPS];
   __shared__ __align__(8) uint64_t s_bar;                       // mbarrier of the row-id TMA copy
   u32* bin_dst    = reinterpret_cast<u32*>(smem_raw + sizeof(unsigned short) * WARPS * NBINS);
   KeyT* skey      = reinterpret_cast<KeyT*>(bin_dst + NBINS + 4);
   int32_t* sidx   = reinterpret_cast<int32_t*>(skey + TILE);
+  // VALS: the first pass has no incoming row ids, so their buffer holds inv (u16[TILE]) and dig (u8[TILE])
+  unsigned short* inv = reinterpret_cast<unsigned short*>(sidx + TILE);
+  unsigned char* dig  = reinterpret_cast<unsigned char*>(inv + TILE);
 
   // One tile per CTA: neighbouring tiles run at the same time on different SMs, so the partial
   // sectors at the ends of their digit runs meet in L2 before they are evicted.
@@ -599,6 +628,11 @@ scatter_kernel(const __grid_constant__ PassArgs<KeyT, Src> a)
 
   if (tile_n == TILE) scatter_tile<KeyT, Src, NBINS, true,  NB>(a, smem_raw, s_wsum, &s_bar, base, tile_n, bin_run, tl);
   else                scatter_tile<KeyT, Src, NBINS, false, NB>(a, smem_raw, s_wsum, &s_bar, base, tile_n, bin_run, tl);
+  if constexpr (VALS) {                                          // the tile's values are read once the pairs are out
+    const char* vp = reinterpret_cast<const char*>(a.vals) + base * a.vbytes;
+    for (int l = tid; l < (tile_n * a.vbytes + 127) / 128; l += THREADS)
+      asm volatile("prefetch.global.L2 [%0];" :: "l"(vp + (size_t)l * 128));
+  }
 
   // ---- coalesced scatter: consecutive threads write consecutive slots of a digit run ----
   const int lane = tid & 31;
@@ -648,6 +682,16 @@ scatter_kernel(const __grid_constant__ PassArgs<KeyT, Src> a)
         }
       }
       a.idx_out[dst] = rid;
+      if constexpr (VALS) { inv[(u32)rid - (u32)base] = (unsigned short)p; dig[p] = (unsigned char)d; }
+    }
+  }
+  if constexpr (VALS) {
+    __syncthreads();                                             // the pair buffer is free: it stages the values
+    switch (a.vbytes) {
+      case 1:  carry_values((const uint8_t*)a.vals, (uint8_t*)a.vperm, base, tile_n, inv, dig, bin_dst, (uint8_t*)skey); break;
+      case 2:  carry_values((const uint16_t*)a.vals, (uint16_t*)a.vperm, base, tile_n, inv, dig, bin_dst, (uint16_t*)skey); break;
+      case 4:  carry_values((const u32*)a.vals, (u32*)a.vperm, base, tile_n, inv, dig, bin_dst, (u32*)skey); break;
+      default: carry_values((const u64*)a.vals, (u64*)a.vperm, base, tile_n, inv, dig, bin_dst, (u64*)skey); break;
     }
   }
 }
@@ -664,13 +708,22 @@ static int run_scatter(Src src, const PassIO& io, int64_t n, int shift, u32 mask
   a.tile_pre = tile_counts; a.group_count = group_count; a.group_shift = group_shift;
   a.out_shift = io.out_shift; a.out_bytes = io.out_bytes ? io.out_bytes : (int)sizeof(KeyT);
   a.low_base = io.low_base; a.low_bits = io.low_bits; a.tile_low = tile_low;
+  a.vals = io.vals; a.vperm = io.vperm; a.vbytes = io.vbytes;
   constexpr size_t smem = PassCfg<KeyT, NBINS>::SMEM;
   constexpr int TILE = PassCfg<KeyT, NBINS>::TILE;
   // NB = ballots per row in the rank phase = digit width, rounded up to a built variant
   const int bits = __builtin_popcount(mask);
   void (*kern)(const PassArgs<KeyT, Src>) =
-      bits <= 6 ? scatter_kernel<KeyT, Src, NBINS, MINB, 6>
-    : bits == 7 ? scatter_kernel<KeyT, Src, NBINS, MINB, 7> : scatter_kernel<KeyT, Src, NBINS, MINB, 8>;
+      bits <= 6 ? scatter_kernel<KeyT, Src, NBINS, MINB, 6, false>
+    : bits == 7 ? scatter_kernel<KeyT, Src, NBINS, MINB, 7, false> : scatter_kernel<KeyT, Src, NBINS, MINB, 8, false>;
+  if (io.vals) {
+    if constexpr (sizeof(KeyT) == 4 && !Src::packed) {
+      kern = bits <= 6 ? scatter_kernel<KeyT, Src, NBINS, MINB, 6, true>
+           : bits == 7 ? scatter_kernel<KeyT, Src, NBINS, MINB, 7, true> : scatter_kernel<KeyT, Src, NBINS, MINB, 8, true>;
+    } else {
+      set_error("internal: values travel only in the first pass over a raw column with 32-bit keys"); return DTB_EINVAL;
+    }
+  }
   DTB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   ProfScope ps("radix_scatter", s);
   kern<<<(unsigned)((n + TILE - 1) / TILE), PASS_THREADS, smem, s>>>(a);
@@ -759,6 +812,10 @@ int launch_radix_pass(const PassIO& io, const KeyPlan& kp, int key_bytes, int64_
       (io.regions && (io.raw_hist || !io.low_hist || io.region_bits < 1 || io.region_bits + bits > 16)) ||
       io.out_bytes > (key_bytes == 8 ? 8 : 4)) {
     set_error("internal: bad key widths for a radix pass"); return DTB_EINVAL;
+  }
+  if (io.vals && (io.src_kind != 1 || io.idx_in || !io.vperm || (io.vbytes != 1 && io.vbytes != 2 && io.vbytes != 4 &&
+                                                                  io.vbytes != 8))) {
+    set_error("internal: bad value column for a radix pass"); return DTB_EINVAL;
   }
   if (io.src_kind == 0) {
     switch (key_bytes) {

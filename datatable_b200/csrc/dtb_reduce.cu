@@ -1226,8 +1226,8 @@ __device__ __forceinline__ void slot_flush(u64 a0, u64 a1, int64_t g, u64* acc0,
 
 // Few distinct group keys (<= 2048): every CTA folds its rows into a shared-memory copy of the
 // accumulator table and flushes it once, so the L2 sees gridDim x groups atomics instead of one per row
-// (100 keys at 2e8 rows = 1.6e8 same-address L2 atomics; low-cardinality by() is the common case).
-constexpr int SMALL_TABLE = 2048;
+// (100 keys at 2e8 rows = 1.6e8 same-address L2 atomics; low-cardinality by() is the common case).  SMALL_TABLE:
+// dtb_internal.h.
 
 template <typename T, int CAT, typename KSrc>
 __global__ void __launch_bounds__(512)
@@ -1447,6 +1447,135 @@ int launch_direct_accumulate_rows(int op, const KeyPlan& kp, const DirectPlan& d
     DirectRawKey<typename decltype(t)::type> ks; ks.src.init(kp.k[0]);
     return accumulate(ks);
   });
+}
+
+// Sum over spread-out group keys from the first radix pass's digit regions (GroupPlan::region_sum; the layout is in
+// dtb_internal.h).  One L2 atomic per row runs at the L2's atomic rate: measured on an H100 80GB HBM3 (700 W,
+// scripts/ubench/atomics_bench.cu), 77.5 G float64 atomics/s into an 8 MB table, which is C2's 12.9 ms for 1e9 rows.
+// Here a CTA takes a contiguous range of slots, folds every region piece of it into a shared-memory table of
+// 2^lbits accumulators (64 KB at 13 bits) and flushes each touched entry with one L2 atomic: (CTAs + regions) x
+// 2^lbits atomics in all.  Within a region the rows keep their row order, and the shared-memory add of a u64 or a
+// float64 is a CAS loop (ATOMS.CAST.SPIN.64): lanes of a warp that add to one key retry one after another, 32 deep
+// in a warp of one key.  So the lanes whose key repeats in the warp -- the left neighbour holds it (sorted or
+// clustered input), or it is hot (DIRECT_HOT's map) -- are summed key by key with a warp butterfly first
+// (warp_key_sums), and only the other lanes add on their own.
+constexpr int REGION_THREADS = 256;
+constexpr int REGION_IPT = 8;                    // rows per thread in flight
+
+// The lanes with `join` add their partials to tab[] once per distinct key among them: per key, one butterfly over the
+// warp (the other lanes give zero) and one shared-memory add by the key's lowest lane.  Every lane calls it.
+template <int CAT>
+__device__ __forceinline__ void warp_key_sums(const Partial<CAT>& part, u32 key, bool join, int lane, u64* tab) {
+  for (unsigned m = __ballot_sync(0xffffffffu, join); m; m = __ballot_sync(0xffffffffu, join)) {
+    const int src = __ffs(m) - 1;
+    const u32 kk = __shfl_sync(0xffffffffu, key, src);
+    const bool mine = join && key == kk;
+    Partial<CAT> t; p_init(t, 0);
+    if (mine) t = part;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) t.s += __shfl_xor_sync(0xffffffffu, t.s, o);
+    if (lane == src) p_flush(t, (int64_t)kk, tab, nullptr, 0);
+    join = join && !mine;
+  }
+}
+
+template <typename T, int CAT, typename KW, bool HOT>
+__global__ void __launch_bounds__(REGION_THREADS, 3)
+region_sum_kernel(const KW* __restrict__ lkey, const typename RawKey<T>::load_t* __restrict__ v,
+                  const u32* __restrict__ bases, int rbits, int lbits, int64_t n, int64_t per,
+                  const uint8_t* __restrict__ hot, u64* acc0)
+{
+  typedef typename RawKey<T>::load_t L;
+  extern __shared__ u64 tab[];                                // 2^lbits accumulators of the current region
+  __shared__ u32 rb[256];
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int nl = 1 << lbits;
+  rb[tid] = bases[tid];
+  const int64_t s_end = ((int64_t)blockIdx.x + 1) * per < n ? ((int64_t)blockIdx.x + 1) * per : n;
+  for (int i = tid; i < nl; i += REGION_THREADS) tab[i] = 0;
+  __syncthreads();
+  for (int64_t s0 = (int64_t)blockIdx.x * per; s0 < s_end;) {
+    const u32 d = slot_owner(rb, 0, 255, (u32)s0);
+    const int64_t rend = d < 255 ? (int64_t)rb[d + 1] : n;
+    const int64_t e = rend < s_end ? rend : s_end;
+    for (int64_t i0 = s0; i0 < e; i0 += REGION_THREADS * REGION_IPT) {
+      KW k[REGION_IPT]; L w[REGION_IPT];
+#pragma unroll
+      for (int j = 0; j < REGION_IPT; j++) {
+        const int64_t i = i0 + j * REGION_THREADS + tid;
+        k[j] = i < e ? lkey[i] : (KW)0;
+        w[j] = i < e ? v[i] : (L)0;
+      }
+      // lanes that repeat their left neighbour's key (runs) or hold a hot key join the warp's per-key sums; one vote
+      // per batch tells whether any lane of the warp joins at all (spread-out keys: none)
+      Partial<CAT> part[REGION_IPT];
+      u32 jm = 0;                                              // bit j: row j joins
+#pragma unroll
+      for (int j = 0; j < REGION_IPT; j++) {
+        const bool in = i0 + j * REGION_THREADS + tid < e;
+        p_init(part[j], 0);
+        p_add<T, CAT>(part[j], w[j], in, 0);
+        const u32 x = (u32)k[j], up = __shfl_up_sync(0xffffffffu, x, 1);
+        bool join = in && lane > 0 && up == x;
+        if constexpr (HOT) join = join || (in && hot[(x << rbits) | d]);
+        jm |= (u32)join << j;
+      }
+      if (__any_sync(0xffffffffu, jm != 0)) {
+#pragma unroll
+        for (int j = 0; j < REGION_IPT; j++)
+          if (__any_sync(0xffffffffu, (jm >> j) & 1u)) warp_key_sums(part[j], (u32)k[j], (jm >> j) & 1u, lane, tab);
+      }
+#pragma unroll
+      for (int j = 0; j < REGION_IPT; j++)
+        if (!((jm >> j) & 1u)) p_flush(part[j], (int64_t)k[j], tab, nullptr, 0);         // shared-memory atomics
+    }
+    __syncthreads();
+    for (int i = tid; i < nl; i += REGION_THREADS) {
+      slot_flush<CAT>(tab[i], 0, ((int64_t)i << rbits) | d, acc0, nullptr, 0);
+      tab[i] = 0;
+    }
+    __syncthreads();
+    s0 = e;
+  }
+}
+
+template <typename T, typename KW, bool HOT>
+static void run_region_sum(const void* lkey, int rbits, int lbits, const uint32_t* bases, const void* vperm, int64_t n,
+                           const uint8_t* hot, u64* acc0, cudaStream_t s, cudaError_t& err)
+{
+  constexpr int CAT = std::is_floating_point<T>::value ? CAT_SUMF : CAT_SUMI;
+  typedef typename RawKey<T>::load_t L;
+  auto kern = region_sum_kernel<T, CAT, KW, HOT>;
+  const int smem = (int)sizeof(u64) << lbits;
+  err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (err != cudaSuccess) return;
+  const int grid = grid_for((n + 65535) / 65536, 3);
+  const int64_t per = (n + grid - 1) / grid;
+  kern<<<grid, REGION_THREADS, smem, s>>>((const KW*)lkey, (const L*)vperm, bases, rbits, lbits, n, per, hot, acc0);
+  err = cudaGetLastError();
+}
+
+int launch_region_sum(const void* lkey, int key_bytes, int rbits, int lbits, const uint32_t* bases, const void* vperm,
+                      int stype, int64_t n, const uint8_t* hot, u64* acc0, cudaStream_t s)
+{
+  if ((key_bytes != 1 && key_bytes != 2) || lbits < 1 || lbits > REGION_MAX_LBITS || lbits > 8 * key_bytes ||
+      rbits < 1 || rbits > 8 || rbits + lbits > 22) {
+    set_error("internal: bad region sum layout"); return DTB_EINVAL;
+  }
+  if (n <= 0) return DTB_OK;
+  cudaError_t err = cudaSuccess;
+  const int rc = with_stype(stype, "internal: region sum of stype ", [&](auto t) {
+    typedef typename decltype(t)::type T;
+    if (key_bytes == 1) { if (hot) run_region_sum<T, uint8_t, true>(lkey, rbits, lbits, bases, vperm, n, hot, acc0, s, err);
+                          else     run_region_sum<T, uint8_t, false>(lkey, rbits, lbits, bases, vperm, n, hot, acc0, s, err); }
+    else                { if (hot) run_region_sum<T, uint16_t, true>(lkey, rbits, lbits, bases, vperm, n, hot, acc0, s, err);
+                          else     run_region_sum<T, uint16_t, false>(lkey, rbits, lbits, bases, vperm, n, hot, acc0, s, err); }
+    return DTB_OK;
+  });
+  DTB_TRY(rc);
+  count_launch();
+  DTB_CUDA_CHECK(err);
+  return DTB_OK;
 }
 
 // Stage 2: out[g] = finalize(acc[gkeys[g]]) in the reference's output stype / NA rules; a dense-mapped small table
