@@ -32,7 +32,7 @@ EXPORTS = [
     "dtb_profile_count", "dtb_profile_get", "dtb_profile_reset",
     "dtb_dense_scatter", "dtb_dense_compact",
     "dtb_sort_grouped", "dtb_qcut", "dtb_cumulative_out_stype", "dtb_cumulative", "dtb_shift", "dtb_fillna", "dtb_group_index",
-    "dtb_set_select", "dtb_largest_group", "dtb_join", "dtb_cache_begin", "dtb_cache_end", "dtb_lower_bound",
+    "dtb_set_select", "dtb_largest_group", "dtb_join", "dtb_join_gather", "dtb_cache_begin", "dtb_cache_end", "dtb_lower_bound",
 ]
 
 
@@ -139,6 +139,8 @@ def _load():
                                       c.POINTER(c.c_int64)]
     lib.dtb_join.argtypes = [c.POINTER(dtb_col), c.POINTER(dtb_col), c.c_int, c.c_int64, c.c_int64, c.c_void_p,
                              c.c_void_p]
+    lib.dtb_join_gather.argtypes = [c.POINTER(dtb_col), c.POINTER(dtb_col), c.c_int, c.c_int64, c.c_int64,
+                                    c.POINTER(dtb_col), c.c_int, c.c_void_p, c.c_void_p, c.POINTER(c.c_void_p)]
     lib.dtb_lower_bound.argtypes = [dtb_col, c.c_int64, dtb_col, c.c_int64, c.c_void_p, c.c_void_p]
     lib.dtb_memcpy.argtypes = [c.c_void_p, c.c_void_p, c.c_int64, c.c_void_p]
     lib.dtb_set_option.argtypes = [c.c_char_p, c.c_int64]

@@ -1981,9 +1981,21 @@ int dtb_slice_groups(const void* offsets, int64_t ngroups, int64_t start, int64_
 int dtb_join(const dtb_col* xkeys, const dtb_col* jkeys, int nkeys, int64_t nrows_x, int64_t nrows_j,
              dtb_stream stream, void* index_out)
 {
+  return dtb_join_gather(xkeys, jkeys, nkeys, nrows_x, nrows_j, nullptr, 0, stream, index_out, nullptr);
+}
+
+int dtb_join_gather(const dtb_col* xkeys, const dtb_col* jkeys, int nkeys, int64_t nrows_x, int64_t nrows_j,
+                    const dtb_col* jvals, int nvals, dtb_stream stream, void* index_out, void* const* vals_out)
+{
   cudaStream_t s = (cudaStream_t)stream;
   t_stats = dtb_call_stats{0, 0, 0, 0, 0};
   if (nkeys < 1 || nkeys > MAX_KEYS || !xkeys || !jkeys) { set_error("number of key columns must be in 1.." + std::to_string(MAX_KEYS)); return DTB_EINVAL; }
+  if (nvals < 0 || (nvals > 0 && (!jvals || !vals_out))) { set_error("bad join value columns"); return DTB_EINVAL; }
+  for (int c = 0; c < nvals; c++) {
+    if (!stype_supported(jvals[c].stype)) {
+      set_error("Unable to join a column of stype " + std::to_string(jvals[c].stype)); return DTB_ENOTIMPL;
+    }
+  }
   if (nrows_x < 0 || nrows_j < 0 || nrows_j > (int64_t)INT32_MAX) { set_error("bad row counts"); return DTB_EINVAL; }
   for (int c = 0; c < nkeys; c++) {
     if (!stype_supported(xkeys[c].stype) || !stype_supported(jkeys[c].stype)) {
@@ -1998,18 +2010,35 @@ int dtb_join(const dtb_col* xkeys, const dtb_col* jkeys, int nkeys, int64_t nrow
   }
   DTB_TRY(ensure_context());
   if (nrows_x == 0) return DTB_OK;
-  if (!index_out) { set_error("index_out is NULL"); return DTB_EINVAL; }
+  if (!index_out && nvals == 0) { set_error("index_out is NULL"); return DTB_EINVAL; }
+  for (int c = 0; c < nvals; c++) if (!vals_out[c]) { set_error("vals_out[" + std::to_string(c) + "] is NULL"); return DTB_EINVAL; }
   ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
-  std::vector<DevIn> xin(nkeys), jin(nkeys);
+  std::vector<DevIn> xin(nkeys), jin(nkeys), vin(nvals);
+  std::vector<DevOut> vout(nvals);
   const void* xp[MAX_KEYS]; const void* jp[MAX_KEYS]; int xst[MAX_KEYS], jst[MAX_KEYS];
   for (int c = 0; c < nkeys; c++) {
     DTB_TRY(xin[c].bind(xkeys[c].data, (size_t)nrows_x * stype_bytes(xkeys[c].stype), s));
     DTB_TRY(jin[c].bind(jkeys[c].data, (size_t)nrows_j * stype_bytes(jkeys[c].stype), s));
     xp[c] = xin[c].dptr; jp[c] = jin[c].dptr; xst[c] = xkeys[c].stype; jst[c] = jkeys[c].stype;
   }
+  std::vector<const void*> vp(nvals); std::vector<void*> op(nvals); std::vector<int> vst(nvals);
+  for (int c = 0; c < nvals; c++) {
+    const size_t esz = stype_bytes(jvals[c].stype);
+    DTB_TRY(vin[c].bind(jvals[c].data, (size_t)nrows_j * esz, s));
+    DTB_TRY(vout[c].bind(vals_out[c], (size_t)nrows_x * esz, s));
+    vp[c] = vin[c].dptr; op[c] = vout[c].dptr; vst[c] = jvals[c].stype;
+  }
   DevOut d_out; DTB_TRY(d_out.bind(index_out, (size_t)nrows_x * 4, s));
-  DTB_TRY(launch_join(nkeys, xp, xst, jp, jst, nrows_x, nrows_j, (int32_t*)d_out.dptr, s));
-  if (d_out.staged()) { DTB_TRY(d_out.finish((size_t)nrows_x * 4, s)); DTB_CUDA_CHECK(cudaStreamSynchronize(s)); }
+  DTB_TRY(launch_join(nkeys, xp, xst, jp, jst, nrows_x, nrows_j, (int32_t*)d_out.dptr, nvals, vp.data(), vst.data(),
+                      op.data(), s));
+  bool staged = d_out.staged();
+  if (d_out.staged()) DTB_TRY(d_out.finish((size_t)nrows_x * 4, s));
+  for (int c = 0; c < nvals; c++) {
+    if (!vout[c].staged()) continue;
+    DTB_TRY(vout[c].finish((size_t)nrows_x * stype_bytes(jvals[c].stype), s));
+    staged = true;
+  }
+  if (staged) DTB_CUDA_CHECK(cudaStreamSynchronize(s));
   return DTB_OK;
 }
 

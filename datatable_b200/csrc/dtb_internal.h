@@ -334,7 +334,11 @@ int launch_set_emit(const int32_t* pos, int64_t nsel, const int32_t* order, cons
                     cudaStream_t s);
 int launch_largest_group(const int32_t* offsets, int64_t ng, int64_t skip, unsigned long long* d_result, cudaStream_t s);
 int launch_lower_bound(const void* sorted, int stype, int64_t n, const void* values, int64_t m, int64_t* out, cudaStream_t s);
+// natural join (dtb_join_gather): index[r] (may be NULL) = J's row matched by X row r or INT32_MIN, and for each of
+// the nvals value columns of J vout[c][r] = vals[c][that row], or the stype's NA
+constexpr int JOIN_MAX_VALS = 16;
 int launch_join(int nkeys, const void* const* xcols, const int* xst, const void* const* jcols, const int* jst,
-                int64_t nx, int64_t nj, int32_t* out, cudaStream_t s);
+                int64_t nx, int64_t nj, int32_t* index, int nvals, const void* const* vals, const int* vst,
+                void* const* vout, cudaStream_t s);
 
 }  // namespace dtb

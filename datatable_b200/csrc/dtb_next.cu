@@ -740,9 +740,15 @@ int launch_largest_group(const int32_t* offsets, int64_t ng, int64_t skip, unsig
 // unique keys, NA first) whose key columns all compare equal, or NA.  Comparison per column follows
 // FwCmp (join.cc:199-232): NA == NA, NA < valid, values compared in J's type; an X value that J's
 // integer type cannot represent (out of range, or a fraction) matches nothing.
+// At the row found, the kernel also writes J's value columns in X's row order (NA where nothing matches), so a
+// query that reads J's columns through the join never materialises the index.
+// Lookup: a single integer / date32 / time64 key column of J whose valid keys are consecutive (J is keyed: sorted,
+// unique, NA first, so jkey[last] - jkey[first valid] == nvalid - 1 decides it from two reads) is addressed
+// directly, row = x - kmin + (J has an NA row); every other J takes the binary search.
 // ===========================================================================
 struct JoinCol { const void* x; const void* j; int32_t xst, jst; };
-struct JoinPlan { int nkeys; JoinCol c[MAX_KEYS]; };
+struct JoinVal { const void* src; void* out; u64 na; int32_t bytes; };
+struct JoinPlan { int nkeys, nvals; int32_t* index; JoinCol c[MAX_KEYS]; JoinVal v[JOIN_MAX_VALS]; };
 
 __device__ __forceinline__ bool load_any(const void* p, int st, int64_t i, long long& iv, double& dv, bool& isf) {
   switch (st) {
@@ -764,8 +770,25 @@ __device__ __forceinline__ void int_range(int st, long long& lo, long long& hi) 
   }
 }
 
-__global__ void join_kernel(JoinPlan jp, int64_t nx, int64_t nj, int32_t* __restrict__ out)
+__device__ __forceinline__ bool is_float_stype(int st) { return st == DTB_STYPE_FLOAT32 || st == DTB_STYPE_FLOAT64; }
+
+__global__ void join_kernel(JoinPlan jp, int64_t nx, int64_t nj)
 {
+  // direct address: one integer key column whose valid keys are kmin .. kmin + nvalid - 1
+  bool direct = false;
+  long long kmin = 0;
+  int64_t jna = 0, nvalid = 0;
+  if (jp.nkeys == 1 && nj > 0 && !is_float_stype(jp.c[0].jst)) {
+    long long k0 = 0, kl = 0; double d; bool f;
+    jna = load_any(jp.c[0].j, jp.c[0].jst, 0, k0, d, f) ? 0 : 1;
+    nvalid = nj - jna;
+    if (nvalid > 0) {
+      load_any(jp.c[0].j, jp.c[0].jst, jna, k0, d, f);
+      load_any(jp.c[0].j, jp.c[0].jst, nj - 1, kl, d, f);
+      direct = (unsigned long long)kl - (unsigned long long)k0 == (unsigned long long)(nvalid - 1);
+      kmin = k0;
+    }
+  }
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < nx; r += stride) {
     // set_xrow: the X values of this row, converted to J's types
@@ -790,7 +813,13 @@ __global__ void join_kernel(JoinPlan jp, int64_t nx, int64_t nj, int32_t* __rest
       }
     }
     int32_t res = INT32_MIN;
-    if (!impossible && nj > 0) {
+    if (!impossible && direct) {
+      if (!xvalid[0]) { if (jna) res = 0; }
+      else {
+        const unsigned long long off = (unsigned long long)xi[0] - (unsigned long long)kmin;
+        if (off < (unsigned long long)nvalid) res = (int32_t)(off + jna);
+      }
+    } else if (!impossible && nj > 0) {
       int64_t start = 0, end = nj - 1;
       bool found = false;
       int64_t at = 0;
@@ -812,19 +841,45 @@ __global__ void join_kernel(JoinPlan jp, int64_t nx, int64_t nj, int32_t* __rest
       }
       if (found) res = (int32_t)at;
     }
-    out[r] = res;
+    if (jp.index) jp.index[r] = res;
+    for (int v = 0; v < jp.nvals; v++) {
+      const JoinVal& c = jp.v[v];
+      switch (c.bytes) {
+        case 1: ((uint8_t*)c.out)[r]  = res >= 0 ? ((const uint8_t*)c.src)[res]  : (uint8_t)c.na;  break;
+        case 2: ((uint16_t*)c.out)[r] = res >= 0 ? ((const uint16_t*)c.src)[res] : (uint16_t)c.na; break;
+        case 4: ((u32*)c.out)[r]      = res >= 0 ? ((const u32*)c.src)[res]      : (u32)c.na;      break;
+        default: ((u64*)c.out)[r]     = res >= 0 ? ((const u64*)c.src)[res]      : c.na;           break;
+      }
+    }
   }
 }
 
 int launch_join(int nkeys, const void* const* xcols, const int* xst, const void* const* jcols, const int* jst,
-                int64_t nx, int64_t nj, int32_t* out, cudaStream_t s)
+                int64_t nx, int64_t nj, int32_t* index, int nvals, const void* const* vals, const int* vst,
+                void* const* vout, cudaStream_t s)
 {
   if (nx == 0) return DTB_OK;
-  JoinPlan jp; jp.nkeys = nkeys;
+  JoinPlan jp; jp.nkeys = nkeys; jp.index = index;
   for (int c = 0; c < nkeys; c++) { jp.c[c].x = xcols[c]; jp.c[c].j = jcols[c]; jp.c[c].xst = xst[c]; jp.c[c].jst = jst[c]; }
-  join_kernel<<<grid_for((nx + 255) / 256, 16), 256, 0, s>>>(jp, nx, nj, out);
-  count_launch();
-  DTB_CUDA_CHECK(cudaGetLastError());
+  // at most JOIN_MAX_VALS value columns per launch; every further batch repeats the lookup (J stays in L2)
+  int v0 = 0;
+  do {
+    jp.nvals = nvals - v0 < JOIN_MAX_VALS ? nvals - v0 : JOIN_MAX_VALS;
+    for (int v = 0; v < jp.nvals; v++) {
+      JoinVal& c = jp.v[v];
+      c.src = vals[v0 + v]; c.out = vout[v0 + v]; c.bytes = stype_bytes(vst[v0 + v]);
+      DTB_TRY(with_stype(vst[v0 + v], "Unable to join a column of stype ", [&](auto t) {
+        typedef typename decltype(t)::type T;
+        c.na = (u64)raw_na<T>();
+        return DTB_OK;
+      }));
+    }
+    join_kernel<<<grid_for((nx + 255) / 256, 16), 256, 0, s>>>(jp, nx, nj);
+    count_launch();
+    DTB_CUDA_CHECK(cudaGetLastError());
+    jp.index = nullptr;
+    v0 += jp.nvals;
+  } while (v0 < nvals);
   return DTB_OK;
 }
 

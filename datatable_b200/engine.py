@@ -546,6 +546,30 @@ def join_index(xcols, jcols):
     return out
 
 
+def join_gather(xcols, jcols, jvals, index=False):
+    """J's columns `jvals` seen through natural_join: for every X row the value of the J row whose key matches, or
+    NA (dtb_join_gather; the same lookup as join_index, without materialising the index).  Returns the list of
+    X-aligned columns, each of its J column's stype, or (index, columns) when index is True; in HBM when every
+    column is."""
+    xs, js, vs = [Col(c) for c in xcols], [Col(c) for c in jcols], [Col(c) for c in jvals]
+    if len(xs) != len(js) or not xs:
+        raise _lib.DtbValueError("join needs the same number (>= 1) of key columns on both sides")
+    nx, nj = xs[0].nrows, js[0].nrows
+    if any(v.nrows != nj for v in vs):
+        raise _lib.DtbValueError("every gathered column of J needs J's number of rows")
+    device = all(c.on_device for c in xs + js + vs)
+    idx, iptr = _alloc(nx, INT32, device) if index or not vs else (None, None)
+    outs = [_alloc(nx, v.stype, device) for v in vs]
+    nk, nv = len(xs), len(vs)
+    cx = (dtb_col * nk)(*[c.c() for c in xs])
+    cj = (dtb_col * nk)(*[c.c() for c in js])
+    cv = (dtb_col * max(nv, 1))(*[c.c() for c in vs])
+    po = (ctypes.c_void_p * max(nv, 1))(*[p for _, p in outs])
+    check(lib.dtb_join_gather(cx, cj, nk, nx, nj, cv, nv, _stream(), ctypes.c_void_p(iptr), po))
+    vals = [o for o, _ in outs]
+    return (idx, vals) if index else vals
+
+
 def set_option(name, value):
     check(lib.dtb_set_option(name.encode(), int(value)))
 

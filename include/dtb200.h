@@ -463,6 +463,17 @@ DTB_API int dtb_join(const dtb_col* xkeys, const dtb_col* jkeys, int nkeys, int6
              dtb_stream stream, void* index_out);
 
 /*
+ * dtb_join_gather -- dtb_join that also reads J's columns through the match: for each of the nvals fixed-width
+ * columns jvals[c] (nrows_j rows, J's row order) vals_out[c][r] = jvals[c][match of X row r], or the stype's NA
+ * where X row r matches nothing -- the column of J that a query sees through natural_join's RowIndex
+ * (eval_context.cc:577-582), without materialising the index.  index_out may be NULL (then nvals >= 1);
+ * dtb_join is the nvals = 0 case.  Same lookup, same key rules.  A single integer / date32 / time64 key column of J
+ * whose valid keys are consecutive is addressed directly instead of searched.  Host or device buffers.
+ */
+DTB_API int dtb_join_gather(const dtb_col* xkeys, const dtb_col* jkeys, int nkeys, int64_t nrows_x, int64_t nrows_j,
+                    const dtb_col* jvals, int nvals, dtb_stream stream, void* index_out, void* const* vals_out);
+
+/*
  * Multi-GPU merge of per-group partials over a small group-key domain (one process per GPU; the
  * reference is single-process, SURVEY.md 8e -- this is north_star's "final NCCL reduce of per-group
  * partials").  Each rank scatters its (group key, 8-byte partial) list into a dense table indexed by
