@@ -9,7 +9,8 @@
 //             (shared-memory histogram) -> counts[chunk][digit]
 //   scan    : per digit, exclusive prefix over the chunks; exclusive prefix over the digit
 //             totals -> every (chunk, digit) knows its first output slot
-//   scatter : one CTA per tile (8192 rows for 32-bit keys, 4096 for 64-bit keys; PassCfg) ranks the rows
+//   scatter : one CTA per tile (8192 rows for 32-bit keys, 4096 for 64-bit keys and for the last of several
+//             count-table passes; PassCfg) ranks the rows
 //             of its tile with warp-level ballots, reorders the tile in shared memory and writes
 //             digit runs out coalesced.
 //
@@ -352,7 +353,8 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, u32 parity) {
       "WAIT_DONE:\n\t}" :: "r"(b), "r"(parity) : "memory");
 }
 
-template <typename KeyT, int NBINS> struct PassCfg {
+// COUNTS: the last of several passes of a count table (PassArgs::group_count; run_scatter).
+template <typename KeyT, int NBINS, bool COUNTS> struct PassCfg {
   static constexpr int WARPS = PASS_THREADS / 32;
   // the incoming row ids of the tile are staged in shared memory by one TMA bulk copy
   static constexpr bool USE_RIDX = true;
@@ -361,10 +363,13 @@ template <typename KeyT, int NBINS> struct PassCfg {
   // partial.  On C2 at 4096 rows the 7-bit passes, 32-row runs, took 1.7 ms more each than the 6-bit passes of 17-bit
   // keys, 64-row runs, with the same kernel (DESIGN 4.2).  101 KB of shared memory: 2 CTAs (16 warps) per SM.
   // 64-bit keys keep 4096-row tiles: 8192 would need 134 KB, one CTA per SM.
-  static constexpr int TILES = (sizeof(KeyT) == 4) ? 2 : 1;
+  // A count-table last pass keeps 4096-row tiles too: its digit is at most 6 bits wide in the 7/7/6 plans, so its runs
+  // are 64 rows long already, and at 53 KB 4 CTAs (32 warps) per SM hide its group-count atomics better.  On C2 the
+  // pass took 5.41 ms on 8192-row tiles and takes 4.52 ms on 4096-row tiles (DESIGN 4.2).
+  static constexpr int TILES = (sizeof(KeyT) == 4 && !COUNTS) ? 2 : 1;
   static constexpr int TILE = PASS_TILE * TILES;
   static constexpr int IPT = PASS_IPT * TILES;
-  static constexpr int MINB = (sizeof(KeyT) == 4) ? 2 : 3;
+  static constexpr int MINB = (sizeof(KeyT) == 4) ? (COUNTS ? 4 : 2) : 3;
   static constexpr size_t SMEM = sizeof(unsigned short) * WARPS * NBINS + sizeof(u32) * (NBINS + 4)
                                + (sizeof(KeyT) + sizeof(int32_t)) * TILE
                                + (USE_RIDX ? sizeof(int32_t) * TILE : 0);
@@ -379,15 +384,15 @@ template <typename KeyT, int NBINS> struct PassCfg {
 // scattered shared-memory write of the reorder phase is ONE 8-byte store per row, not two
 // 4-byte stores: shared-memory wavefronts, not HBM, bound this kernel.
 // Thread t owns the BPT = NBINS/256 consecutive digits t*BPT.. in the scan phase.
-template <typename KeyT, typename Src, int NBINS, bool FULL, int NB>
+template <typename KeyT, typename Src, int NBINS, bool COUNTS, bool FULL, int NB>
 __device__ __forceinline__ void scatter_tile(const PassArgs<KeyT, Src>& a, unsigned char* smem_raw, u32* s_wsum,
                                              uint64_t* s_bar, const int64_t base, const int tile_n,
                                              const u32 (&bin_run)[NBINS / PASS_THREADS], const uint2 tl)
 {
-  constexpr int THREADS = PASS_THREADS, IPT = PassCfg<KeyT, NBINS>::IPT, TILE = PassCfg<KeyT, NBINS>::TILE;
+  constexpr int THREADS = PASS_THREADS, IPT = PassCfg<KeyT, NBINS, COUNTS>::IPT, TILE = PassCfg<KeyT, NBINS, COUNTS>::TILE;
   constexpr int WARPS = THREADS / 32;
   constexpr int BPT = NBINS / THREADS;
-  constexpr bool USE_RIDX = PassCfg<KeyT, NBINS>::USE_RIDX;
+  constexpr bool USE_RIDX = PassCfg<KeyT, NBINS, COUNTS>::USE_RIDX;
   unsigned short* whist = reinterpret_cast<unsigned short*>(smem_raw);
   u32* bin_dst    = reinterpret_cast<u32*>(smem_raw + sizeof(unsigned short) * WARPS * NBINS);
   KeyT* skey      = reinterpret_cast<KeyT*>(bin_dst + NBINS + 4);
@@ -558,12 +563,15 @@ __device__ __forceinline__ KeyT staged_key(const KeyT* skey, int q) {
 // The values of a region sum's first pass (VALS below): once the tile's (key, row id) pairs are written, the values are
 // read in row order, coalesced, staged at their rows' tile slots in the pair buffer and written in the same digit runs.
 // inv[tile position] = tile slot and dig[tile slot] = digit were recorded by the write loop.
+// Every thread has all its loads of an 8192-row tile in flight at once (VB = TILE / THREADS), and nothing prefetches
+// them to L2: on C2 (H100, 1e9 rows) an L2 prefetch issued after ranking took the pass to 12.3 ms and one issued at
+// kernel entry to 13.2 ms; without it, 16 loads per round took 11.6 ms and 32 take 11.2 ms.
 template <typename W>
 __device__ __forceinline__ void carry_values(const W* __restrict__ vals, W* __restrict__ vperm, int64_t base, int tile_n,
                                              const unsigned short* inv, const unsigned char* dig, const u32* bin_dst,
                                              W* sv)
 {
-  constexpr int VB = 16;                                         // loads in flight per thread
+  constexpr int VB = 32;                                         // loads in flight per thread
   for (int p0 = 0; p0 < tile_n; p0 += PASS_THREADS * VB) {
     W w[VB];
 #pragma unroll
@@ -583,14 +591,15 @@ __device__ __forceinline__ void carry_values(const W* __restrict__ vals, W* __re
 }
 
 // VALS: the first pass of a region sum (PassIO::vals), over a raw column (row id = position) with 32-bit keys
-template <typename KeyT, typename Src, int NBINS, int MINB, int NB, bool VALS>
-__global__ void __launch_bounds__(PASS_THREADS, MINB)
+template <typename KeyT, typename Src, int NBINS, bool COUNTS, int NB, bool VALS>
+__global__ void __launch_bounds__(PASS_THREADS, (PassCfg<KeyT, NBINS, COUNTS>::MINB))
 scatter_kernel(const __grid_constant__ PassArgs<KeyT, Src> a)
 {
-  constexpr int THREADS = PASS_THREADS, TILE = PassCfg<KeyT, NBINS>::TILE, TILES = PassCfg<KeyT, NBINS>::TILES;
+  typedef PassCfg<KeyT, NBINS, COUNTS> Cfg;
+  constexpr int THREADS = PASS_THREADS, TILE = Cfg::TILE, TILES = Cfg::TILES;
   constexpr int WARPS = THREADS / 32;
   constexpr int BPT = NBINS / THREADS;
-  static_assert(!VALS || (sizeof(KeyT) == 4 && !Src::packed && PassCfg<KeyT, NBINS>::USE_RIDX),
+  static_assert(!VALS || (sizeof(KeyT) == 4 && !Src::packed && !COUNTS && Cfg::USE_RIDX),
                 "values travel in the first pass over a raw column with 32-bit keys, staged in the row-id buffer");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ u32 s_wsum[WARPS];
@@ -626,13 +635,8 @@ scatter_kernel(const __grid_constant__ PassArgs<KeyT, Src> a)
     }
   }
 
-  if (tile_n == TILE) scatter_tile<KeyT, Src, NBINS, true,  NB>(a, smem_raw, s_wsum, &s_bar, base, tile_n, bin_run, tl);
-  else                scatter_tile<KeyT, Src, NBINS, false, NB>(a, smem_raw, s_wsum, &s_bar, base, tile_n, bin_run, tl);
-  if constexpr (VALS) {                                          // the tile's values are read once the pairs are out
-    const char* vp = reinterpret_cast<const char*>(a.vals) + base * a.vbytes;
-    for (int l = tid; l < (tile_n * a.vbytes + 127) / 128; l += THREADS)
-      asm volatile("prefetch.global.L2 [%0];" :: "l"(vp + (size_t)l * 128));
-  }
+  if (tile_n == TILE) scatter_tile<KeyT, Src, NBINS, COUNTS, true,  NB>(a, smem_raw, s_wsum, &s_bar, base, tile_n, bin_run, tl);
+  else                scatter_tile<KeyT, Src, NBINS, COUNTS, false, NB>(a, smem_raw, s_wsum, &s_bar, base, tile_n, bin_run, tl);
 
   // ---- coalesced scatter: consecutive threads write consecutive slots of a digit run ----
   const int lane = tid & 31;
@@ -701,7 +705,6 @@ static int run_scatter(Src src, const PassIO& io, int64_t n, int shift, u32 mask
                        const u32* counts, const u32* base, const unsigned short* tile_counts,
                        u32* group_count, int group_shift, const uint2* tile_low, cudaStream_t s)
 {
-  constexpr int MINB = PassCfg<KeyT, NBINS>::MINB;
   PassArgs<KeyT, Src> a;
   a.src = src; a.idx_in = io.idx_in; a.keys_out = (KeyT*)io.keys_out; a.idx_out = io.idx_out;
   a.n = n; a.shift = shift + io.low_bits; a.mask = mask; a.chunk_offs = counts; a.digit_base = base;
@@ -709,27 +712,37 @@ static int run_scatter(Src src, const PassIO& io, int64_t n, int shift, u32 mask
   a.out_shift = io.out_shift; a.out_bytes = io.out_bytes ? io.out_bytes : (int)sizeof(KeyT);
   a.low_base = io.low_base; a.low_bits = io.low_bits; a.tile_low = tile_low;
   a.vals = io.vals; a.vperm = io.vperm; a.vbytes = io.vbytes;
-  constexpr size_t smem = PassCfg<KeyT, NBINS>::SMEM;
-  constexpr int TILE = PassCfg<KeyT, NBINS>::TILE;
   // NB = ballots per row in the rank phase = digit width, rounded up to a built variant
   const int bits = __builtin_popcount(mask);
-  void (*kern)(const PassArgs<KeyT, Src>) =
-      bits <= 6 ? scatter_kernel<KeyT, Src, NBINS, MINB, 6, false>
-    : bits == 7 ? scatter_kernel<KeyT, Src, NBINS, MINB, 7, false> : scatter_kernel<KeyT, Src, NBINS, MINB, 8, false>;
+  auto launch = [&](auto counts, auto vals) -> int {
+    constexpr bool COUNTS = decltype(counts)::value, VALS = decltype(vals)::value;
+    typedef PassCfg<KeyT, NBINS, COUNTS> Cfg;
+    void (*kern)(const PassArgs<KeyT, Src>) =
+        bits <= 6 ? scatter_kernel<KeyT, Src, NBINS, COUNTS, 6, VALS>
+      : bits == 7 ? scatter_kernel<KeyT, Src, NBINS, COUNTS, 7, VALS> : scatter_kernel<KeyT, Src, NBINS, COUNTS, 8, VALS>;
+    DTB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
+    ProfScope ps("radix_scatter", s);
+    kern<<<(unsigned)((n + Cfg::TILE - 1) / Cfg::TILE), PASS_THREADS, Cfg::SMEM, s>>>(a);
+    count_launch();
+    DTB_CUDA_CHECK(cudaGetLastError());
+    return DTB_OK;
+  };
   if (io.vals) {
     if constexpr (sizeof(KeyT) == 4 && !Src::packed) {
-      kern = bits <= 6 ? scatter_kernel<KeyT, Src, NBINS, MINB, 6, true>
-           : bits == 7 ? scatter_kernel<KeyT, Src, NBINS, MINB, 7, true> : scatter_kernel<KeyT, Src, NBINS, MINB, 8, true>;
+      return launch(std::false_type(), std::true_type());
     } else {
       set_error("internal: values travel only in the first pass over a raw column with 32-bit keys"); return DTB_EINVAL;
     }
   }
-  DTB_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  ProfScope ps("radix_scatter", s);
-  kern<<<(unsigned)((n + TILE - 1) / TILE), PASS_THREADS, smem, s>>>(a);
-  count_launch();
-  DTB_CUDA_CHECK(cudaGetLastError());
-  return DTB_OK;
+  // The last of several passes of a count table (rows arrive from a previous pass, sorted by its lower digits, so a
+  // tile holds few long runs) takes 4096-row tiles.  A count table's only pass (at most 8 key bits, rows in input
+  // order) keeps 8192: there every tile has a run per distinct key, and twice the tiles meant twice the run-head
+  // atomics on the same few addresses (100 keys at 2e8 rows: 2.8 ms became 5.1 ms).  64-bit keys run every pass on
+  // 4096-row tiles.
+  if constexpr (sizeof(KeyT) == 4) {
+    if (group_count && io.idx_in) return launch(std::true_type(), std::false_type());
+  }
+  return launch(std::false_type(), std::false_type());
 }
 
 template <typename KeyT, typename Src, int NBINS>
