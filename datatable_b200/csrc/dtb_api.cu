@@ -1978,6 +1978,82 @@ int dtb_slice_groups(const void* offsets, int64_t ngroups, int64_t start, int64_
   return DTB_OK;
 }
 
+int dtb_mask_rows(dtb_col mask, int64_t nrows, dtb_stream stream, void* rows_out, int64_t rows_capacity,
+                  int64_t* nrows_out)
+{
+  cudaStream_t s = (cudaStream_t)stream;
+  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
+  if (!nrows_out) { set_error("nrows_out is NULL"); return DTB_EINVAL; }
+  if (mask.stype != DTB_STYPE_BOOL) {
+    set_error("dtb_mask_rows takes a bool8 column, not stype " + std::to_string(mask.stype)); return DTB_EINVAL;
+  }
+  if (nrows < 0 || nrows > (int64_t)INT32_MAX) { set_error("nrows must be in 0..INT32_MAX"); return DTB_EINVAL; }
+  if (rows_capacity < 0) { set_error("rows_capacity must be non-negative"); return DTB_EINVAL; }
+  if (nrows > 0 && !mask.data) { set_error("mask data is NULL"); return DTB_EINVAL; }
+  if (rows_capacity > 0 && !rows_out) { set_error("rows_out is NULL"); return DTB_EINVAL; }
+  *nrows_out = 0;
+  DTB_TRY(ensure_context());
+  if (nrows == 0) return DTB_OK;
+  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
+  DevIn d_mask; DTB_TRY(d_mask.bind(mask.data, (size_t)nrows, s));
+  DevBuf tiles, tot;
+  DTB_TRY(tiles.alloc(sizeof(u64) * (size_t)mask_num_tiles(nrows), s));
+  DTB_TRY(tot.alloc(sizeof(u64), s));
+  DTB_TRY(launch_mask_count((const int8_t*)d_mask.dptr, nrows, tiles.as<u64>(), tot.as<u64>(), s));
+  u64 h_tot = 0;                                                        // the one wait: the result's size
+  DTB_CUDA_CHECK(cudaMemcpyAsync(&h_tot, tot.p, sizeof(u64), cudaMemcpyDeviceToHost, s));
+  DTB_CUDA_CHECK(cudaStreamSynchronize(s));
+  const int64_t nout = (int64_t)h_tot;
+  *nrows_out = nout;
+  if (nout > rows_capacity) { set_error("rows_out is too small: " + std::to_string(nout) + " rows selected"); return DTB_ENOSPACE; }
+  if (nout == 0) return DTB_OK;
+  DevOut d_rows; DTB_TRY(d_rows.bind(rows_out, sizeof(int32_t) * (size_t)nout, s));
+  DTB_TRY(launch_mask_emit((const int8_t*)d_mask.dptr, nrows, tiles.as<u64>(), (int32_t*)d_rows.dptr, s));
+  if (d_rows.staged()) {
+    DTB_TRY(d_rows.finish(sizeof(int32_t) * (size_t)nout, s));
+    DTB_CUDA_CHECK(cudaStreamSynchronize(s));
+  }
+  return DTB_OK;
+}
+
+int dtb_int_rows(dtb_col sel, int64_t nrows, dtb_stream stream, void* rows_out, int64_t* min_out, int64_t* max_out,
+                 int64_t* nacount_out)
+{
+  cudaStream_t s = (cudaStream_t)stream;
+  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
+  if (!min_out || !max_out || !nacount_out) { set_error("min_out / max_out / nacount_out is NULL"); return DTB_EINVAL; }
+  const int st = sel.stype;
+  if (st != DTB_STYPE_INT8 && st != DTB_STYPE_INT16 && st != DTB_STYPE_INT32 && st != DTB_STYPE_INT64) {
+    set_error("dtb_int_rows takes an int8, int16, int32 or int64 column, not stype " + std::to_string(st));
+    return DTB_EINVAL;
+  }
+  if (nrows < 0 || nrows > (int64_t)INT32_MAX) { set_error("nrows must be in 0..INT32_MAX"); return DTB_EINVAL; }
+  if (nrows > 0 && !sel.data) { set_error("selector data is NULL"); return DTB_EINVAL; }
+  if (nrows > 0 && st != DTB_STYPE_INT32 && !rows_out) { set_error("rows_out is NULL"); return DTB_EINVAL; }
+  *min_out = 0; *max_out = 0; *nacount_out = 0;
+  DTB_TRY(ensure_context());
+  if (nrows == 0) return DTB_OK;
+  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
+  const size_t esz = stype_bytes(st);
+  DevIn d_sel; DTB_TRY(d_sel.bind(sel.data, (size_t)nrows * esz, s));
+  DevOut d_rows; DTB_TRY(d_rows.bind(rows_out, sizeof(int32_t) * (size_t)nrows, s));
+  if (rows_out) {
+    if (st == DTB_STYPE_INT32)
+      DTB_CUDA_CHECK(cudaMemcpyAsync(d_rows.dptr, d_sel.dptr, sizeof(int32_t) * (size_t)nrows, cudaMemcpyDeviceToDevice, s));
+    else
+      DTB_TRY(launch_narrow_rows(d_sel.dptr, st, nrows, (int32_t*)d_rows.dptr, s));
+    DTB_TRY(d_rows.finish(sizeof(int32_t) * (size_t)nrows, s));
+  }
+  DevBuf d_stats; DTB_TRY(d_stats.alloc(sizeof(ColStats), s));
+  DTB_TRY(launch_col_stats(d_sel.dptr, st, nrows, d_stats.as<ColStats>(), s));
+  ColStats h;
+  DTB_CUDA_CHECK(cudaMemcpyAsync(&h, d_stats.p, sizeof(h), cudaMemcpyDeviceToHost, s));
+  DTB_CUDA_CHECK(cudaStreamSynchronize(s));                             // the one wait: the statistics
+  *nacount_out = (int64_t)h.nacount;
+  if (h.nvalid) { *min_out = (int64_t)h.lo; *max_out = (int64_t)h.hi; }
+  return DTB_OK;
+}
+
 int dtb_join(const dtb_col* xkeys, const dtb_col* jkeys, int nkeys, int64_t nrows_x, int64_t nrows_j,
              dtb_stream stream, void* index_out)
 {

@@ -292,6 +292,16 @@ int launch_slice_groups_plan(const int32_t* offsets, int64_t ng, const SlicePara
                              int32_t* gsel, unsigned long long* totals, cudaStream_t s);
 int launch_slice_groups_emit(const int32_t* offsets, const SliceParams& p, const int32_t* offsets_out, const int32_t* gsel,
                              int64_t ng_out, int64_t nout, int32_t* gid, int32_t* rows_out, cudaStream_t s);
+// rows selected by a bool8 column (dtb_mask_rows): launch_mask_count writes the selected rows of every tile and turns
+// them into each tile's first output position in tile_count (u64[mask_num_tiles(n)]), and their sum to *total
+// (device u64); launch_mask_emit then writes the ascending positions, *total of them, to rows_out
+int64_t mask_num_tiles(int64_t n);
+int launch_mask_count(const int8_t* mask, int64_t n, unsigned long long* tile_count, unsigned long long* total,
+                      cudaStream_t s);
+int launch_mask_emit(const int8_t* mask, int64_t n, const unsigned long long* tile_start, int32_t* rows_out,
+                     cudaStream_t s);
+// an int8 / int16 / int64 selector as an int32 RowIndex, NA -> INT32_MIN (dtb_int_rows)
+int launch_narrow_rows(const void* sel, int stype, int64_t n, int32_t* out, cudaStream_t s);
 // sum/cnt: u64[ng] each, m2: double[2 * ng] (m2, then the groups' pivots), all zeroed
 int launch_sd(const void* v, int stype, int64_t nv, const int32_t* order, const int32_t* offsets, int64_t ng, int64_t n,
               unsigned long long* sum, unsigned long long* cnt, double* m2, void* out, cudaStream_t s);

@@ -13,9 +13,13 @@
 //   union / intersect / setdiff / symdiff   set_funcs.cc:126-456
 //   mode / nmodal         stats.cc:955-1003
 //   natural join          frame/join.cc:392-470               binary search of every X row in the sorted keys of J
+//   boolean / integer i   rowindex_array.cc:63-203            the rows a bool8 column selects (two passes over the
+//                                                             mask, no look-back); an integer column as an int32
+//                                                             RowIndex
 //
 // Bound: none of these is a bandwidth kernel except the row-parallel ones (group ids, distinct
 // flags, join), which are random-gather bound like reduce_kernel.
+#include <limits>
 #include <type_traits>
 #include "dtb_common.cuh"
 
@@ -974,35 +978,51 @@ slice_count_kernel(const int32_t* __restrict__ offsets, int64_t ng, SliceParams 
   }
 }
 
-// exclusive scan of the block sums in place (one CTA walks them); totals[0] = rows, totals[1] = groups
+// exclusive scan of K interleaved block sums in place (one CTA walks them): bsum[K * b + k] becomes the sum of
+// component k over the blocks before b, totals[k] its sum over all blocks.  The slices scan K = 2 (rows, groups),
+// the boolean compaction K = 1 (selected rows per tile).
+template <int K>
 __global__ void __launch_bounds__(1024)
-slice_scan_kernel(u64* __restrict__ bsum, int64_t nb, u64* __restrict__ totals)
+block_sums_scan_kernel(u64* __restrict__ bsum, int64_t nb, u64* __restrict__ totals)
 {
-  __shared__ u64 sr[32], sg[32];
-  __shared__ u64 carry_r, carry_g;
+  __shared__ u64 sw[K][32];
+  __shared__ u64 carry[K];
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-  if (t == 0) { carry_r = 0; carry_g = 0; }
+  if (t < K) carry[t] = 0;
   __syncthreads();
   for (int64_t b0 = 0; b0 < nb; b0 += 1024) {
     const int64_t b = b0 + t;
-    const u64 r = b < nb ? bsum[2 * b] : 0, g = b < nb ? bsum[2 * b + 1] : 0;
-    u64 ir = r, ig = g;
+    u64 v[K], in[K];
+#pragma unroll
+    for (int k = 0; k < K; k++) { v[k] = b < nb ? bsum[K * b + k] : 0; in[k] = v[k]; }
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) {
-      const u64 a = __shfl_up_sync(0xffffffffu, ir, d), c = __shfl_up_sync(0xffffffffu, ig, d);
-      if (lane >= d) { ir += a; ig += c; }
+#pragma unroll
+      for (int k = 0; k < K; k++) {
+        const u64 a = __shfl_up_sync(0xffffffffu, in[k], d);
+        if (lane >= d) in[k] += a;
+      }
     }
-    if (lane == 31) { sr[warp] = ir; sg[warp] = ig; }
+    if (lane == 31) {
+#pragma unroll
+      for (int k = 0; k < K; k++) sw[k][warp] = in[k];
+    }
     __syncthreads();
-    u64 pr = 0, pg = 0;
-    for (int w = 0; w < warp; w++) { pr += sr[w]; pg += sg[w]; }
-    const u64 cr = carry_r, cg = carry_g;
-    if (b < nb) { bsum[2 * b] = cr + pr + ir - r; bsum[2 * b + 1] = cg + pg + ig - g; }
+    u64 pre[K];
+#pragma unroll
+    for (int k = 0; k < K; k++) {
+      pre[k] = carry[k];
+      for (int w = 0; w < warp; w++) pre[k] += sw[k][w];
+      if (b < nb) bsum[K * b + k] = pre[k] + in[k] - v[k];
+    }
     __syncthreads();
-    if (t == 1023) { carry_r = cr + pr + ir; carry_g = cg + pg + ig; }
+    if (t == 1023) {
+#pragma unroll
+      for (int k = 0; k < K; k++) carry[k] = pre[k] + in[k];
+    }
     __syncthreads();
   }
-  if (t == 0) { totals[0] = carry_r; totals[1] = carry_g; }
+  if (t < K) totals[t] = carry[t];
 }
 
 // offsets_out[k] = rows selected before the k-th non-empty group, gsel[k] = its index
@@ -1071,7 +1091,7 @@ int launch_slice_groups_plan(const int32_t* offsets, int64_t ng, const SlicePara
   u32* cnt = (u32*)scratch;
   u64* bsum = (u64*)((char*)scratch + ((sizeof(u32) * (size_t)(ng + 4) + 7) / 8) * 8);
   slice_count_kernel<<<(unsigned)nb, 256, 0, s>>>(offsets, ng, p, cnt, bsum);
-  slice_scan_kernel<<<1, 1024, 0, s>>>(bsum, nb, totals);
+  block_sums_scan_kernel<2><<<1, 1024, 0, s>>>(bsum, nb, totals);
   slice_compact_kernel<<<(unsigned)nb, 256, 0, s>>>(cnt, bsum, ng, offsets_out, gsel);
   count_launch(3);
   DTB_CUDA_CHECK(cudaGetLastError());
@@ -1085,6 +1105,181 @@ int launch_slice_groups_emit(const int32_t* offsets, const SliceParams& p, const
   if (nout == 0) return DTB_OK;
   DTB_TRY(launch_expand_gid(offsets_out, ng_out, nout, gid, s));
   slice_emit_kernel<<<grid_for((nout + 255) / 256, 16), 256, 0, s>>>(offsets, p, offsets_out, gsel, gid, nout, rows_out);
+  count_launch();
+  DTB_CUDA_CHECK(cudaGetLastError());
+  return DTB_OK;
+}
+
+// ===========================================================================
+// i = a boolean column: the ascending positions of its selected rows (ArrayRowIndexImpl::init_from_boolean_column,
+// rowindex_array.cc:130-170, a serial loop there).  A row is selected when its byte is neither 0 nor the NA -128,
+// i.e. when its low 7 bits are not all zero.  Two passes over the mask, no look-back: mask_count_kernel writes the
+// selected rows of every MASK_TILE-row tile, block_sums_scan_kernel<1> turns them into each tile's first output
+// position, and mask_emit_kernel reads its tile again and writes the tile's positions as one contiguous run.
+// ===========================================================================
+constexpr int MASK_THREADS = 256;
+constexpr int MASK_VECS = 8;                                   // 16-byte loads per thread and tile
+constexpr int MASK_CHUNK = MASK_THREADS * 16;                  // rows of one round of loads: 4096
+constexpr int MASK_TILE = MASK_CHUNK * MASK_VECS;              // 32768 rows per tile
+
+// 16 bytes of the mask: rows [16 v, 16 v + 16) of the column; rows at or past n read as 0.  aligned: the column's
+// base is 16-byte aligned, so that whole vectors are read with one load.
+__device__ __forceinline__ uint4 mask_vec(const int8_t* __restrict__ m, int64_t n, int64_t v, bool aligned)
+{
+  const int64_t r0 = v * 16;
+  if (aligned && r0 + 16 <= n) return __ldg(reinterpret_cast<const uint4*>(m) + v);
+  u32 w[4] = {0, 0, 0, 0};
+  for (int b = 0; b < 16; b++)
+    if (r0 + b < n) w[b >> 2] |= (u32)(uint8_t)m[r0 + b] << (8 * (b & 3));
+  return make_uint4(w[0], w[1], w[2], w[3]);
+}
+
+// bit b (0..3) set when byte b of w is selected
+__device__ __forceinline__ u32 mask_bits4(u32 w)
+{
+  const u32 s = ((w & 0x7f7f7f7fu) + 0x7f7f7f7fu) & 0x80808080u;   // high bit of a byte: its low 7 bits are not 0
+  return ((s >> 7) & 1u) | ((s >> 14) & 2u) | ((s >> 21) & 4u) | ((s >> 28) & 8u);
+}
+
+// bit b (0..15) set when row 16 v + b is selected
+__device__ __forceinline__ u32 mask_bits16(uint4 q)
+{
+  return mask_bits4(q.x) | (mask_bits4(q.y) << 4) | (mask_bits4(q.z) << 8) | (mask_bits4(q.w) << 12);
+}
+
+__global__ void __launch_bounds__(MASK_THREADS)
+mask_count_kernel(const int8_t* __restrict__ mask, int64_t n, bool aligned, u64* __restrict__ tile_count)
+{
+  __shared__ u32 ws[MASK_THREADS / 32];
+  const int t = threadIdx.x;
+  const int64_t v0 = (int64_t)blockIdx.x * (MASK_TILE / 16) + t;
+  uint4 q[MASK_VECS];
+#pragma unroll
+  for (int j = 0; j < MASK_VECS; j++) q[j] = mask_vec(mask, n, v0 + j * MASK_THREADS, aligned);
+  u32 c = 0;
+#pragma unroll
+  for (int j = 0; j < MASK_VECS; j++) c += __popc(mask_bits16(q[j]));
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) c += __shfl_xor_sync(0xffffffffu, c, d);
+  if ((t & 31) == 0) ws[t >> 5] = c;
+  __syncthreads();
+  if (t == 0) {
+    u32 sum = 0;
+#pragma unroll
+    for (int w = 0; w < MASK_THREADS / 32; w++) sum += ws[w];
+    tile_count[blockIdx.x] = sum;
+  }
+}
+
+// One CTA per tile.  Every round of loads covers MASK_CHUNK consecutive rows, 16 per thread in thread order: a
+// thread's rank is the popcount of its 16 bits plus a warp scan of the counts plus the counts of the warps before
+// it.  The positions go to shared memory at their rank, then out as one coalesced run after the tile's start.
+__global__ void __launch_bounds__(MASK_THREADS)
+mask_emit_kernel(const int8_t* __restrict__ mask, int64_t n, bool aligned, const u64* __restrict__ tile_start,
+                 int32_t* __restrict__ rows_out)
+{
+  __shared__ int32_t pos[MASK_CHUNK];
+  __shared__ u32 ws[MASK_THREADS / 32];
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int64_t v0 = (int64_t)blockIdx.x * (MASK_TILE / 16) + t;
+  uint4 q[MASK_VECS];
+#pragma unroll
+  for (int j = 0; j < MASK_VECS; j++) q[j] = mask_vec(mask, n, v0 + j * MASK_THREADS, aligned);
+  int32_t* out = rows_out + tile_start[blockIdx.x];
+#pragma unroll
+  for (int j = 0; j < MASK_VECS; j++) {
+    u32 bits = mask_bits16(q[j]);
+    const u32 c = __popc(bits);
+    u32 inc = c;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const u32 a = __shfl_up_sync(0xffffffffu, inc, d);
+      if (lane >= d) inc += a;
+    }
+    if (lane == 31) ws[warp] = inc;
+    __syncthreads();
+    u32 rank = inc - c, total = 0;
+#pragma unroll
+    for (int w = 0; w < MASK_THREADS / 32; w++) {
+      const u32 x = ws[w];
+      rank += w < warp ? x : 0;
+      total += x;
+    }
+    const int32_t row0 = (int32_t)((v0 + j * MASK_THREADS) * 16);
+    while (bits) {
+      pos[rank++] = row0 + (__ffs(bits) - 1);
+      bits &= bits - 1;
+    }
+    __syncthreads();
+    for (u32 i = t; i < total; i += MASK_THREADS) out[i] = pos[i];
+    out += total;
+    __syncthreads();                                           // pos and ws are reused by the next round
+  }
+}
+
+int64_t mask_num_tiles(int64_t n) { return (n + MASK_TILE - 1) / MASK_TILE; }
+
+int launch_mask_count(const int8_t* mask, int64_t n, u64* tile_count, u64* total, cudaStream_t s)
+{
+  const int64_t nt = mask_num_tiles(n);
+  if (nt == 0) { DTB_CUDA_CHECK(cudaMemsetAsync(total, 0, sizeof(u64), s)); return DTB_OK; }
+  const bool aligned = (reinterpret_cast<uintptr_t>(mask) & 15) == 0;
+  mask_count_kernel<<<(unsigned)nt, MASK_THREADS, 0, s>>>(mask, n, aligned, tile_count);
+  block_sums_scan_kernel<1><<<1, 1024, 0, s>>>(tile_count, nt, total);
+  count_launch(2);
+  DTB_CUDA_CHECK(cudaGetLastError());
+  return DTB_OK;
+}
+
+int launch_mask_emit(const int8_t* mask, int64_t n, const u64* tile_start, int32_t* rows_out, cudaStream_t s)
+{
+  const int64_t nt = mask_num_tiles(n);
+  if (nt == 0) return DTB_OK;
+  const bool aligned = (reinterpret_cast<uintptr_t>(mask) & 15) == 0;
+  mask_emit_kernel<<<(unsigned)nt, MASK_THREADS, 0, s>>>(mask, n, aligned, tile_start, rows_out);
+  count_launch();
+  DTB_CUDA_CHECK(cudaGetLastError());
+  return DTB_OK;
+}
+
+// ===========================================================================
+// i = an int8 / int16 / int64 column: its values as an int32 RowIndex, NA -> INT32_MIN (the NA row).  The caller
+// has checked the valid values against the frame's rows, so they fit.  16-byte loads of the selector.
+// ===========================================================================
+template <typename T>
+__global__ void __launch_bounds__(256)
+narrow_rows_kernel(const T* __restrict__ sel, int64_t n, int32_t* __restrict__ out)
+{
+  constexpr int VEC = 16 / sizeof(T);
+  constexpr T NA = std::numeric_limits<T>::min();
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const bool aligned = (reinterpret_cast<uintptr_t>(sel) & 15) == 0;
+  const int64_t nvec = aligned ? n / VEC : 0;
+  for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += stride) {
+    const uint4 q = __ldg(reinterpret_cast<const uint4*>(sel) + v);
+    const T* e = reinterpret_cast<const T*>(&q);
+#pragma unroll
+    for (int k = 0; k < VEC; k++) out[v * VEC + k] = e[k] == NA ? INT32_MIN : (int32_t)e[k];
+  }
+  for (int64_t i = nvec * VEC + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+    out[i] = sel[i] == NA ? INT32_MIN : (int32_t)sel[i];
+}
+
+int launch_narrow_rows(const void* sel, int stype, int64_t n, int32_t* out, cudaStream_t s)
+{
+  if (n == 0) return DTB_OK;
+  auto run = [&](auto tag) {
+    typedef decltype(tag) T;
+    constexpr int VEC = 16 / sizeof(T);
+    narrow_rows_kernel<T><<<grid_for((n / VEC + 255) / 256 + 1, 8), 256, 0, s>>>((const T*)sel, n, out);
+    return DTB_OK;
+  };
+  switch (stype) {
+    case DTB_STYPE_INT8:  run(int8_t()); break;
+    case DTB_STYPE_INT16: run(int16_t()); break;
+    case DTB_STYPE_INT64: run(int64_t()); break;
+    default: set_error("narrow_rows takes int8, int16 or int64, not stype " + std::to_string(stype)); return DTB_EINVAL;
+  }
   count_launch();
   DTB_CUDA_CHECK(cudaGetLastError());
   return DTB_OK;

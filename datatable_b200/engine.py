@@ -530,6 +530,31 @@ def slice_groups(offsets, start=None, stop=None, step=None):
     return rows[:nro.value], offs[:ngo.value + 1]
 
 
+def mask_rows(mask):
+    """The ascending int32 positions of the rows a bool8 column selects: its byte is neither 0 nor the NA -128
+    (dtb_mask_rows; ArrayRowIndexImpl::init_from_boolean_column, rowindex_array.cc:130-170).  In HBM when the mask
+    is."""
+    m = Col(mask, BOOL)
+    out, optr = _alloc(m.nrows, INT32, m.on_device)
+    nout = ctypes.c_int64(0)
+    check(lib.dtb_mask_rows(m.c(), m.nrows, _stream(), ctypes.c_void_p(optr), m.nrows, ctypes.byref(nout)))
+    return out[:nout.value]
+
+
+def int_rows(sel, stype=None):
+    """An integer column as an int32 RowIndex, NA as INT32_MIN (dtb_int_rows): (rows, min, max, nacount), with min and
+    max over the valid values (0 when there is none).  An int32 column is returned as it is; in HBM when sel is."""
+    s = Col(sel, stype)
+    if s.stype == INT32:
+        out, optr = s.data, None
+    else:
+        out, optr = _alloc(s.nrows, INT32, s.on_device)
+    lo, hi, nna = ctypes.c_int64(0), ctypes.c_int64(0), ctypes.c_int64(0)
+    check(lib.dtb_int_rows(s.c(), s.nrows, _stream(), ctypes.c_void_p(optr), ctypes.byref(lo), ctypes.byref(hi),
+                           ctypes.byref(nna)))
+    return out, lo.value, hi.value, nna.value
+
+
 def join_index(xcols, jcols):
     """natural_join (frame/join.cc:392-470): for every X row the row of J (sorted by its key columns) with
     equal key, or the NA index; int32, in HBM when every column is."""

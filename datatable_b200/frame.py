@@ -600,14 +600,15 @@ class Frame:
         if not (isinstance(i, slice) and i == slice(None)):
             ok = (isinstance(i, int) and not isinstance(i, bool)) or (
                 isinstance(i, slice) and all(x is None or (isinstance(x, int) and not isinstance(x, bool)) for x in (i.start, i.stop, i.step)))
-            if not ok:
+            if not ok and not isinstance(i, _ROW_SELECTORS):
                 raise NotImplementedError("row filters other than an integer or an integer slice are outside the GPU hot path")
             isel = i
         # EvalContext::evaluate (eval_context.cc:144-172) for the hot-path shapes: the join first (J's columns the
         # query reads are looked up once, X-aligned, by _Upload), then group / sort, then `i`, then j
         DT = self if join_ is None else _join_view(self, join_.frame)
-        names, exprs, by_, sort_ = _resolve(DT, j, by_, sort_)
-        up = _Upload(DT, [r.name for m in (by_, sort_) if m is not None for r in m.cols], exprs)
+        names, exprs, by_, sort_, isel = _resolve(DT, j, by_, sort_, isel)
+        masks = isel.mask_columns() if isinstance(isel, _Rows) else []
+        up = _Upload(DT, masks + [r.name for m in (by_, sort_) if m is not None for r in m.cols], exprs)
         order, groups, ngroups, late = _group(DT, up, by_, sort_, isel, exprs)
         keys = by_.cols if by_ is not None else []
         if any(isinstance(e, Reducer) for e in exprs):
@@ -676,9 +677,10 @@ def _result(cols, nrows, host=False):
     return out
 
 
-def _resolve(DT, j, by_, sort_):
-    """(names, expressions of j, by_, sort_) with every column reference bound to the column it names (_bind).
-    Every check of the query's arguments runs here, before the device is touched."""
+def _resolve(DT, j, by_, sort_, isel=None):
+    """(names, expressions of j, by_, sort_, isel) with every column reference bound to the column it names (_bind),
+    and `i` other than an integer or an integer slice resolved into _Rows (_resolve_i).  Every check of the query's
+    arguments runs here, before the device is touched."""
     if by_ is not None and sort_ is not None and sort_.na_position == "remove":
         # the rows dropped from the front of the RowIndex would still be counted by the groups
         raise ValueError("na_position = \"remove\" in sort() is not supported together with by()")
@@ -688,10 +690,240 @@ def _resolve(DT, j, by_, sort_):
     if sort_ is not None:
         sort_ = copy.copy(sort_)
         sort_.cols = [_bind(DT, r) for r in sort_.cols]
+    if isinstance(isel, _ROW_SELECTORS):
+        isel = _resolve_i(DT, isel, by_ is not None or sort_ is not None)
     names, exprs = _resolve_j(DT, j, [r.name for r in by_.cols] if by_ is not None else ())
     if torch is None or not torch.cuda.is_available():
         raise _lib.DtbCudaError("no usable CUDA device: datatable_b200 has no CPU fallback")
-    return names, exprs, by_, sort_
+    return names, exprs, by_, sort_, isel
+
+
+# ---------------------------------------------------------------------------
+# `i` as a boolean or integer column, a list or a range (evaluate_i without by() / sort())
+# ---------------------------------------------------------------------------
+class _Rows:
+    """A resolved `i`: the pieces whose RowIndices are concatenated, in order (RowIndex::concat of FExpr_List's
+    _evaluate_i_other, fexpr_list.cc:225-243; one piece for every other form).  A piece is
+        ("rows", int32 ndarray)   positions built on the host (ints, bools, slices, ranges)
+        ("mask", name)            a bool8 column of the queried frame, X's own or J's (_JKey), read from HBM
+        ("mask", Col)             a bool8 selector Frame's column
+        ("ints", Col)             an integer selector Frame's column, checked against the rows once its min / max
+                                  are known (fexpr_frame.cc:183-195)"""
+
+    def __init__(self, pieces):
+        self.pieces = pieces
+
+    def mask_columns(self):
+        """The queried frame's columns that select rows: uploaded first, as group keys are."""
+        return [x for kind, x in self.pieces if kind == "mask" and not isinstance(x, engine.Col)]
+
+
+_ROW_SELECTORS = (Frame, ColRef, list, tuple, range, np.ndarray)
+
+
+def _i_kind(x):
+    """The reference's name of the kind of expression x is (_name_type, fexpr_list.cc:117-132)."""
+    if x is None:
+        return "None"
+    if isinstance(x, (bool, np.bool_)):
+        return "bool"
+    if isinstance(x, (int, np.integer)):
+        return "integer"
+    if isinstance(x, (float, np.floating)):
+        return "float"
+    if isinstance(x, str):
+        return "string"
+    if isinstance(x, ColRef):
+        return "expression"
+    if isinstance(x, range):
+        return "integer slice"
+    if isinstance(x, slice):
+        if x == slice(None):
+            return "slice"
+        return "integer slice" if _int_slice(x) else "string-slice"
+    return "?"                                   # a Frame, a numpy array, a nested list
+
+
+def _int_slice(s):
+    return all(v is None or (isinstance(v, (int, np.integer)) and not isinstance(v, (bool, np.bool_)))
+               for v in (s.start, s.stop, s.step))
+
+
+def _rows_s(n):
+    return f"{n} row{'' if n == 1 else 's'}"
+
+
+def _resolve_i(DT, i, grouped):
+    """_Rows of `i` over the rows of DT (FExpr_*::evaluate_i); under by() / sort() the reference's refusal
+    (FExpr_*::evaluate_iby)."""
+    if isinstance(i, (Frame, np.ndarray)):
+        if grouped:
+            raise TypeError("A Frame cannot be used as an i-selector in the presence of a groupby")
+        return _Rows([_frame_piece(DT, i)])
+    if isinstance(i, ColRef):
+        if grouped:
+            raise NotImplementedError("FExpr_Func::evaluate_iby() not implemented yet")
+        return _Rows([_mask_piece(DT, i)])
+    if isinstance(i, range):
+        if grouped:
+            raise NotImplementedError("A range selector cannot yet be used in i in the presence of by clause")
+        return _Rows([_range_piece(DT.nrows, i)])
+    if grouped:
+        raise NotImplementedError("FExpr_List::evaluate_iby() not implemented yet")
+    return _Rows(_list_pieces(DT, list(i)))
+
+
+def _mask_piece(DT, ref):
+    """f.b / g.b (FExpr_Func::evaluate_i, fexpr_func.cc:61-73): a bool8 column of X or, through the join, of J."""
+    if ref.negated or isinstance(ref.name, slice):
+        raise NotImplementedError(f"{ref!r} as a row filter is outside the GPU hot path")
+    ref = _bind(DT, ref)
+    if ref.name not in DT._stypes:
+        raise KeyError(f"Column `{ref.name}` does not exist in the Frame")
+    st = DT._stypes[ref.name]
+    if st != BOOL:
+        raise TypeError(f"Filter expression must be boolean, instead it was of type {_STYPE_NAMES.get(st, st)}")
+    return ("mask", ref.name)
+
+
+def _frame_piece(DT, sel):
+    """A single-column Frame or a numpy array (FExpr_Frame::evaluate_i, fexpr_frame.cc:159-198): a bool8 column
+    selects its rows whose value is true, an integer column lists rows."""
+    if isinstance(sel, np.ndarray):
+        if sel.ndim == 2:
+            if sel.shape[1] != 1:
+                raise ValueError(f"Only a single-column Frame may be used as `i` selector, instead got a Frame with "
+                                 f"{sel.shape[1]} columns")
+            sel = sel[:, 0]
+        elif sel.ndim != 1:
+            raise NotImplementedError(f"a {sel.ndim}-dimensional array as a row filter is outside the GPU hot path")
+        sel = Frame({"C0": sel})
+    if sel.ncols != 1:
+        raise ValueError(f"Only a single-column Frame may be used as `i` selector, instead got a Frame with "
+                         f"{sel.ncols} columns")
+    if sel.key:
+        raise NotImplementedError("A keyed frame cannot be used as an i selector")
+    c = sel._col(sel.names[0])
+    if c.stype == BOOL:
+        if c.nrows != DT.nrows:
+            raise ValueError(f"A boolean column used as `i` selector has {_rows_s(c.nrows)}, but applied to a Frame "
+                             f"with {_rows_s(DT.nrows)}")
+        return ("mask", c)
+    if c.stype not in (INT8, INT16, INT32, INT64):
+        raise TypeError(f"A Frame which is used as an `i` selector should be either boolean or integer, instead got "
+                        f"`{_STYPE_NAMES.get(c.stype, c.stype)}`")
+    return ("ints", c)
+
+
+def _range_piece(n, r):
+    """range(a, b, s) (FExpr_Literal_Range::evaluate_i, fexpr_literal_range.cc:87-96; orange::normalize)."""
+    count = len(r)
+    if count == 0:
+        return ("rows", np.zeros(0, np.int32))
+    a, z = r.start, r.start + (count - 1) * r.step
+    if not (-n <= a < n and -n <= z < n) or (a >= 0) != (z >= 0):
+        raise ValueError(f"{r!r} cannot be applied to a Frame with {_rows_s(n)}")
+    if a < 0:
+        a += n
+    return ("rows", np.arange(a, a + count * r.step, r.step, dtype=np.int32)[:count])
+
+
+def _slice_piece(n, s):
+    """An integer slice (FExpr_Literal_SliceInt::evaluate_i, fexpr_literal_sliceint.cc:57-62) or f[:]'s every row."""
+    if s.step == 0:
+        raise NotImplementedError("repeat slices (step 0) without by() are outside the GPU hot path")
+    return ("rows", np.arange(*s.indices(n), dtype=np.int32))
+
+
+def _list_pieces(DT, items):
+    """A list or tuple (FExpr_List::evaluate_i, fexpr_list.cc:225-316)."""
+    n = DT.nrows
+    if not items:
+        return [("rows", np.zeros(0, np.int32))]
+    kind0 = _i_kind(items[0])
+    if kind0 == "bool":                                           # _evaluate_i_bools
+        if len(items) != n:
+            raise ValueError(f"The length of boolean list in i selector does not match the number of rows in the "
+                             f"Frame: {len(items)} vs {n}")
+        for k, x in enumerate(items):
+            if _i_kind(x) != "bool":
+                raise TypeError(f"Element {k} in the i-selector list is {_i_kind(x)}, whereas the previous elements "
+                                f"were boolean")
+        return [("rows", np.flatnonzero(np.array(items, dtype=bool)).astype(np.int32))]
+    if kind0 == "integer":                                        # _evaluate_i_ints
+        rows = []
+        for k, x in enumerate(items):
+            kind = _i_kind(x)
+            if kind == "integer":
+                x = int(x)
+                if not -n <= x < n:
+                    raise ValueError(f"Index {x} is invalid for a Frame with {n} rows")
+                rows.append(x % n)
+            elif kind in ("slice", "integer slice"):
+                return _other_pieces(DT, items)
+            elif kind != "None":
+                raise TypeError(f"Invalid item of type {kind} at index {k} in the i-selector list")
+        return [("rows", np.array(rows, dtype=np.int32))]
+    return _other_pieces(DT, items)
+
+
+def _other_pieces(DT, items):
+    """_evaluate_i_other (fexpr_list.cc:225-243): every item's own RowIndex, None skipped."""
+    n = DT.nrows
+    pieces = []
+    for k, x in enumerate(items):
+        kind = _i_kind(x)
+        if kind == "None":
+            continue
+        if isinstance(x, (Frame, np.ndarray)):
+            pieces.append(_frame_piece(DT, x))
+        elif kind == "integer":
+            x = int(x)
+            if not -n <= x < n:
+                raise ValueError(f"Row `{x}` is invalid for a frame with {_rows_s(n)}")
+            pieces.append(("rows", np.array([x % n], dtype=np.int32)))
+        elif kind == "expression":
+            pieces.append(_mask_piece(DT, x))
+        elif isinstance(x, range):
+            pieces.append(_range_piece(n, x))
+        elif kind in ("slice", "integer slice"):
+            pieces.append(_slice_piece(n, x))
+        else:
+            raise TypeError(f"Invalid expression of type {kind} at index {k} in the i-selector list")
+    return pieces or [("rows", np.zeros(0, np.int32))]
+
+
+def _selected_rows(DT, up, sel):
+    """The int32 RowIndex in HBM of the resolved `i` sel (_Rows): the compaction of every boolean piece
+    (dtb_mask_rows), every integer piece checked and made int32 (dtb_int_rows), the host-built pieces uploaded, and
+    the pieces concatenated in order."""
+    n = DT.nrows
+    parts = []
+    for kind, x in sel.pieces:
+        if kind == "rows":
+            parts.append(x)
+        elif kind == "mask":
+            parts.append(engine.mask_rows((up.col(x) if isinstance(x, str) else engine.Col(_dev(x), BOOL)).data))
+        else:
+            rows, lo, hi, nna = engine.int_rows(_dev(x), x.stype)
+            if nna < x.nrows:                                     # fexpr_frame.cc:183-195
+                if lo < 0:
+                    raise ValueError(f"An integer column used as an `i` selector contains an invalid negative index: "
+                                     f"{lo}")
+                if hi >= n:
+                    raise ValueError(f"An integer column used as an `i` selector contains index {hi} which is not "
+                                     f"valid for a Frame with {_rows_s(n)}")
+            parts.append(rows)
+    if len(parts) == 1 and engine.is_tensor(parts[0]):
+        return parts[0]
+    if all(isinstance(p, np.ndarray) for p in parts):
+        return torch.from_numpy(np.concatenate(parts) if len(parts) != 1 else parts[0]).cuda()
+    out = torch.empty(builtins.sum(len(p) for p in parts), dtype=torch.int32, device="cuda")
+    a = 0
+    for p in parts:
+        out[a:a + len(p)].copy_(torch.from_numpy(p) if isinstance(p, np.ndarray) else p)
+        a += len(p)
+    return out
 
 
 def _join_view(X, J):
@@ -834,7 +1066,8 @@ def _group(DT, up, by_, sort_, isel, exprs):
     order: the RowIndex of the selected rows, None for every row in place.  groups: the Groupby offsets, the Groupby
     handle for by() with reducers, or None without by() / sort().  late: the handle was made without the reducers
     (see _groupby_handle).  isel, an integer or integer slice for `i`, is applied inside every group under by() /
-    sort() (iexpr_->evaluate_iby, eval_context.cc:154-158), to the rows otherwise (evaluate_i, :159-163)."""
+    sort() (iexpr_->evaluate_iby, eval_context.cc:154-158), to the rows otherwise (evaluate_i, :159-163); the other
+    forms of `i` (_Rows) only exist without by() / sort()."""
     keycols, flags = [], []
     na_pos = NA_FIRST
     if by_ is not None:
@@ -861,6 +1094,8 @@ def _group(DT, up, by_, sort_, isel, exprs):
             st_, sp_, se_ = isel.start, isel.stop, isel.step
         sel, offsets = engine.slice_groups(offsets, st_, sp_, se_)
         return engine.gather(order, sel), offsets, len(offsets) - 1, False
+    if isinstance(isel, _Rows):
+        return _selected_rows(DT, up, isel), None, None, False
     if isel is not None:
         # no by() / sort(): evaluate_i -- a plain row slice (python slice semantics; step 0 = repeat is not taken here)
         n_ = DT.nrows

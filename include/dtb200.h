@@ -405,6 +405,33 @@ DTB_API int dtb_slice_groups(const void* offsets, int64_t ngroups, int64_t start
                      int64_t* ngroups_out, int64_t* nrows_out);
 
 /*
+ * dtb_mask_rows -- the `i` node of DT[i, j] when i is a boolean column (DT[f.b, j], DT[dt.Frame(b), j]); replaces
+ * ArrayRowIndexImpl::init_from_boolean_column (rowindex_array.cc:130-170).  mask: a bool8 column of nrows rows
+ * (0 <= nrows <= INT32_MAX).  rows_out receives the ascending int32 positions of the rows whose byte is neither 0
+ * nor the NA -128, at most rows_capacity of them (DTB_ENOSPACE with *nrows_out = the number needed otherwise;
+ * nrows always suffices); *nrows_out = how many.  Two passes over the mask (count per tile, scan, emit); the call
+ * waits once, for the count.  The arguments are checked, in this order, before any CUDA call: nrows_out NULL,
+ * stype, nrows, rows_capacity < 0, mask data NULL (nrows > 0), rows_out NULL (rows_capacity > 0): DTB_EINVAL.
+ * Host or device buffers.
+ */
+DTB_API int dtb_mask_rows(dtb_col mask, int64_t nrows, dtb_stream stream, void* rows_out, int64_t rows_capacity,
+                          int64_t* nrows_out);
+
+/*
+ * dtb_int_rows -- the `i` node of DT[i, j] when i is an integer column (DT[dt.Frame(idx), j]); the checks and the
+ * RowIndex of FExpr_Frame::evaluate_i (expr/fexpr_frame.cc:175-198) and RowIndex(const Column&)
+ * (rowindex_array.cc:63-128).  sel: an int8 / int16 / int32 / int64 column of nrows rows (<= INT32_MAX).
+ * *min_out / *max_out: the smallest / largest valid value (0 when every value is NA), *nacount_out: the NA values;
+ * the caller checks them against the frame's rows.  rows_out: int32[nrows], sel's values in its order with NA as
+ * INT32_MIN (the NA row); it may be NULL for an int32 column, which is the RowIndex as it stands.  The call waits
+ * once, for the statistics.  The arguments are checked, in this order, before any CUDA call: min_out / max_out /
+ * nacount_out NULL, stype, nrows, selector data NULL (nrows > 0), rows_out NULL (nrows > 0, not int32): DTB_EINVAL.
+ * Host or device buffers.
+ */
+DTB_API int dtb_int_rows(dtb_col sel, int64_t nrows, dtb_stream stream, void* rows_out, int64_t* min_out,
+                         int64_t* max_out, int64_t* nacount_out);
+
+/*
  * dtb_sort_grouped -- replaces Column::sort_grouped (sort.cc:1499-1530): reorders the rows INSIDE every
  * group of (order, offsets) by `value` ascending, NA first, stable; the groups themselves stay where
  * they are.  order: int32 RowIndex; arguments as in "Per-group functions", order_out is its `out`.
