@@ -1459,8 +1459,19 @@ int launch_direct_accumulate_rows(int op, const KeyPlan& kp, const DirectPlan& d
 // in a warp of one key.  So the lanes whose key repeats in the warp -- the left neighbour holds it (sorted or
 // clustered input), or it is hot (DIRECT_HOT's map) -- are summed key by key with a warp butterfly first
 // (warp_key_sums), and only the other lanes add on their own.
-constexpr int REGION_THREADS = 256;
-constexpr int REGION_IPT = 8;                    // rows per thread in flight
+// The fold waits on its shared-memory adds more than on HBM: each row's CAS loop is a chain of a shared load, a
+// float add and the CAS, and a warp cannot start the next row's loop before this one ends.  So the kernel runs as
+// many warps as the 64 KB tables allow: two 1024-thread CTAs per SM (64 warps, at most 32 registers), two rows per
+// thread, and the next two rows' loads issued before the current ones are folded.  On C2 (H100 80GB HBM3, 700 W)
+// the sum took 5.11 ms with 256 threads and 8 rows per thread (3 CTAs, 24 warps per SM), 5.02 ms with the loads
+// issued one batch ahead, 4.69 ms with 512 threads and 4 rows (48 warps) and 4.03 ms as here.  The hot-key variant
+// keeps 256 threads and 8 rows per thread: there the warps' joined sums of a hot key meet on one table entry, and
+// 64 warps per SM made the power-law head of scripts/skew_check.py (2e8 rows) take 3.5 ms instead of 2.4 ms.
+template <bool HOT> struct RegionCfg {
+  static constexpr int THREADS = HOT ? 256 : 1024;
+  static constexpr int IPT = HOT ? 8 : 2;        // rows per thread and batch
+  static constexpr int CTAS = HOT ? 3 : 2;       // per SM, with a 64 KB table each
+};
 
 // The lanes with `join` add their partials to tab[] once per distinct key among them: per key, one butterfly over the
 // warp (the other lanes give zero) and one shared-memory add by the key's lowest lane.  Every lane calls it.
@@ -1480,17 +1491,18 @@ __device__ __forceinline__ void warp_key_sums(const Partial<CAT>& part, u32 key,
 }
 
 template <typename T, int CAT, typename KW, bool HOT>
-__global__ void __launch_bounds__(REGION_THREADS, 3)
+__global__ void __launch_bounds__(RegionCfg<HOT>::THREADS, RegionCfg<HOT>::CTAS)
 region_sum_kernel(const KW* __restrict__ lkey, const typename RawKey<T>::load_t* __restrict__ v,
                   const u32* __restrict__ bases, int rbits, int lbits, int64_t n, int64_t per,
                   const uint8_t* __restrict__ hot, u64* acc0)
 {
   typedef typename RawKey<T>::load_t L;
+  constexpr int REGION_THREADS = RegionCfg<HOT>::THREADS, REGION_IPT = RegionCfg<HOT>::IPT;
   extern __shared__ u64 tab[];                                // 2^lbits accumulators of the current region
   __shared__ u32 rb[256];
   const int tid = threadIdx.x, lane = tid & 31;
   const int nl = 1 << lbits;
-  rb[tid] = bases[tid];
+  if (tid < 256) rb[tid] = bases[tid];
   const int64_t s_end = ((int64_t)blockIdx.x + 1) * per < n ? ((int64_t)blockIdx.x + 1) * per : n;
   for (int i = tid; i < nl; i += REGION_THREADS) tab[i] = 0;
   __syncthreads();
@@ -1498,14 +1510,22 @@ region_sum_kernel(const KW* __restrict__ lkey, const typename RawKey<T>::load_t*
     const u32 d = slot_owner(rb, 0, 255, (u32)s0);
     const int64_t rend = d < 255 ? (int64_t)rb[d + 1] : n;
     const int64_t e = rend < s_end ? rend : s_end;
+    // the next batch is loaded before the current one is folded: a warp's loads stay in flight while it adds
+    KW kn[REGION_IPT]; L wn[REGION_IPT];
+    auto fetch = [&](int64_t b) {
+#pragma unroll
+      for (int j = 0; j < REGION_IPT; j++) {
+        const int64_t i = b + j * REGION_THREADS + tid;
+        kn[j] = i < e ? lkey[i] : (KW)0;
+        wn[j] = i < e ? v[i] : (L)0;
+      }
+    };
+    fetch(s0);
     for (int64_t i0 = s0; i0 < e; i0 += REGION_THREADS * REGION_IPT) {
       KW k[REGION_IPT]; L w[REGION_IPT];
 #pragma unroll
-      for (int j = 0; j < REGION_IPT; j++) {
-        const int64_t i = i0 + j * REGION_THREADS + tid;
-        k[j] = i < e ? lkey[i] : (KW)0;
-        w[j] = i < e ? v[i] : (L)0;
-      }
+      for (int j = 0; j < REGION_IPT; j++) { k[j] = kn[j]; w[j] = wn[j]; }
+      if (i0 + REGION_THREADS * REGION_IPT < e) fetch(i0 + REGION_THREADS * REGION_IPT);
       // lanes that repeat their left neighbour's key (runs) or hold a hot key join the warp's per-key sums; one vote
       // per batch tells whether any lane of the warp joins at all (spread-out keys: none)
       Partial<CAT> part[REGION_IPT];
@@ -1549,9 +1569,9 @@ static void run_region_sum(const void* lkey, int rbits, int lbits, const uint32_
   const int smem = (int)sizeof(u64) << lbits;
   err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
   if (err != cudaSuccess) return;
-  const int grid = grid_for((n + 65535) / 65536, 3);
+  const int grid = grid_for((n + 65535) / 65536, RegionCfg<HOT>::CTAS);
   const int64_t per = (n + grid - 1) / grid;
-  kern<<<grid, REGION_THREADS, smem, s>>>((const KW*)lkey, (const L*)vperm, bases, rbits, lbits, n, per, hot, acc0);
+  kern<<<grid, RegionCfg<HOT>::THREADS, smem, s>>>((const KW*)lkey, (const L*)vperm, bases, rbits, lbits, n, per, hot, acc0);
   err = cudaGetLastError();
 }
 
