@@ -183,6 +183,35 @@ __device__ __forceinline__ u32 slot_owner(const u32* b, u32 lo, u32 hi, u32 s) {
   return lo;
 }
 
+// The group that holds sorted position p: the last g in [0, ng) with offsets[g] <= p (offsets[0] <= p).
+__device__ __forceinline__ int64_t group_of(const int32_t* offsets, int64_t ng, int64_t p) {
+  int64_t lo = 0, hi = ng;
+  while (hi - lo > 1) { const int64_t mid = (lo + hi) >> 1; if ((int64_t)offsets[mid] <= p) lo = mid; else hi = mid; }
+  return lo;
+}
+
+// out[g] = a result of stype out_stype (bits: its bit pattern, a float32's in the low word), or that stype's NA
+// (stype.h:186-197)
+__device__ __forceinline__ void store_result(void* out, int out_stype, int64_t g, bool valid, u64 bits) {
+  switch (out_stype) {
+    case DTB_STYPE_BOOL: case DTB_STYPE_INT8:
+      ((int8_t*)out)[g] = valid ? (int8_t)bits : INT8_MIN; break;
+    case DTB_STYPE_INT16: ((int16_t*)out)[g] = valid ? (int16_t)bits : INT16_MIN; break;
+    case DTB_STYPE_INT32: case DTB_STYPE_DATE32:
+      ((int32_t*)out)[g] = valid ? (int32_t)bits : INT32_MIN; break;
+    case DTB_STYPE_INT64: case DTB_STYPE_TIME64:
+      ((int64_t*)out)[g] = valid ? (int64_t)bits : INT64_MIN; break;
+    case DTB_STYPE_FLOAT32: ((u32*)out)[g] = valid ? (u32)bits : raw_na<float>(); break;
+    case DTB_STYPE_FLOAT64: ((u64*)out)[g] = valid ? bits : raw_na<double>(); break;
+  }
+}
+
+// out[g] = r rounded to out_stype (float32 or float64), or NA
+__device__ __forceinline__ void store_float(void* out, int out_stype, int64_t g, bool valid, double r) {
+  store_result(out, out_stype, g, valid,
+               out_stype == DTB_STYPE_FLOAT32 ? (u64)__float_as_uint((float)r) : (u64)__double_as_longlong(r));
+}
+
 __device__ __forceinline__ unsigned lanemask_lt() {
   unsigned m; asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m)); return m;
 }

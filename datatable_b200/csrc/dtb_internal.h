@@ -198,19 +198,19 @@ size_t zero_fix_bytes(int64_t ngroups);
 // The reducer is a float min / max: the sign of a zero result needs the lookup above.
 bool minmax_zero_sign(int op, int stype);
 
-// pos[g] = min(pos[g], first position p in group g whose row order[p] (order NULL = identity) holds a valid value,
-// and with zero_only a float zero).  Row-parallel: one read of the positions and the values, one atomic per thread
-// and group.  gate != NULL: nothing happens unless *gate != 0.  pos: the caller sets the groups it wants to ~0.
-int launch_first_valid_pos(const void* v, int stype, int64_t nv, const void* order, int order_is64, const int32_t* offsets,
-                           int64_t ngroups, int64_t n, int zero_only, const unsigned long long* gate,
-                           unsigned long long* pos, cudaStream_t s);
+// pos[g] = min(pos[g], first position p in group g whose row order[p] (order NULL = identity) holds a zero of the
+// float32 / float64 column v).  Row-parallel: one read of the positions and the values, one atomic per thread and
+// group.  gate != NULL: nothing happens unless *gate != 0.  pos: the caller sets the groups it wants to ~0.
+int launch_first_zero_pos(const void* v, int stype, int64_t nv, const void* order, int order_is64, const int32_t* offsets,
+                          int64_t ngroups, int64_t n, const unsigned long long* gate, unsigned long long* pos,
+                          cudaStream_t s);
 
 // acc0/acc1: device scratch, ngroups uint64 each.  n = offsets[ngroups] (rows under the groups).
 int launch_reduce_impl(int op, const void* value, int stype, int64_t nrows_value,
                        const void* order, int order_is64, const int32_t* offsets, int64_t ngroups,
                        int64_t n, unsigned long long* acc0, unsigned long long* acc1,
                        void* out, cudaStream_t s, void* extra = nullptr);
-// device scratch `extra` that launch_reduce_impl needs for `op` (sd: m2[ng] and pivots[ng]; nunique: one flag byte per
+// device scratch `extra` that launch_reduce_impl needs for `op` (sd: sq[ng] and pivot[ng]; nunique: one flag byte per
 // row; float min / max: the zero lookup's marks, see GroupRows)
 size_t reduce_extra_bytes(int op, int stype, int64_t ng, int64_t n);
 int reduce_out_stype_host(int op, int stype);
@@ -302,9 +302,16 @@ int launch_mask_emit(const int8_t* mask, int64_t n, const unsigned long long* ti
                      cudaStream_t s);
 // an int8 / int16 / int64 selector as an int32 RowIndex, NA -> INT32_MIN (dtb_int_rows)
 int launch_narrow_rows(const void* sel, int stype, int64_t n, int32_t* out, cudaStream_t s);
-// sum/cnt: u64[ng] each, m2: double[2 * ng] (m2, then the groups' pivots), all zeroed
-int launch_sd(const void* v, int stype, int64_t nv, const int32_t* order, const int32_t* offsets, int64_t ng, int64_t n,
-              unsigned long long* sum, unsigned long long* cnt, double* m2, void* out, cudaStream_t s);
+// sd, cov and corr per group: two passes over the values shifted by a pivot, the value at the group's first valid
+// row.  The words of every group (device, ng each; the kernels set them): sum[k] = Σ (x_k - pivot_k) and cnt (the first
+// pass), sq[k] = Σ dx_k² and sxy = Σ dx_0 dx_1 (the second), pivot[k].  sd uses sum[0], cnt, sq[0] and pivot[0]; cov
+// sum, cnt, sxy and pivot; corr every word.
+struct MomentWords { double* sum[2]; unsigned long long* cnt; double* sq[2]; double* sxy; double* pivot[2]; };
+// op = DTB_OP_SD: sd of column x (y unused) through an int32 RowIndex; DTB_OP_COV / DTB_OP_CORR: over the pairs (x, y)
+// where both are valid, through int32 or int64 row ids.  out: out_stype, float32 or float64.
+int launch_moments(int op, const void* x, int sx, const void* y, int sy, int64_t nv, const void* order, int order_is64,
+                   const int32_t* offsets, int64_t ng, int64_t n, const MomentWords& w, int out_stype, void* out,
+                   cudaStream_t s);
 // cov / corr over the pairs (x, y) seen through `order` (int32 or int64 row ids), segmented by offsets.  scratch:
 // reduce2_scratch_bytes(ng) of device memory.  out: float32 when out_f32, else float64 (reduce2_out_stype_host).
 int reduce2_out_stype_host(int op, int stype_x, int stype_y);

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Times the per-group product and cov / corr next to the per-group sum on the same groups, on one GPU.
+"""Times the per-group product, sd and cov / corr next to the per-group sum on the same groups, on one GPU.
 
     python scripts/bench_binary_reducers.py [--rows 1e8,1e9] [--out DIR]
 
@@ -11,8 +11,9 @@ is timed with CUDA events on the current stream: 2 warm-up calls, the median of 
                    group key (dtb_groupby_reduce)
     sum_rowindex   the same sum gathered through the RowIndex (dtb_reduce on the handle's RowIndex)
     prod           the handle's PROD: it always gathers through the RowIndex, so sum_rowindex is its yardstick
-    cov, corr      dtb_groupby_reduce2(v1, v2): a pivot pass and two passes, each reading the RowIndex and two
-                   random value sectors per row
+    sd             the handle's SD(v1): a pivot pass and two passes, each reading the RowIndex and one random value
+                   sector per row
+    cov, corr      dtb_groupby_reduce2(v1, v2): the same moment kernels over two random value sectors per row
 
 A second case puts every row in one group under a random RowIndex (2e7 rows and the largest size asked for): every
 tile's boundary slots then belong to the same group.  The card's name and power limit are read in the same run and
@@ -81,6 +82,7 @@ def main():
         rec["sum_ms"], _ = timed(lambda: gb.reduce(_lib.OP_SUM, v))
         rec["sum_rowindex_ms"], _ = timed(lambda: gb.reduce_ordered(_lib.OP_SUM, v, order))
         rec["prod_ms"], _ = timed(lambda: gb.reduce(_lib.OP_PROD, v))
+        rec["sd_ms"], _ = timed(lambda: gb.reduce(_lib.OP_SD, v))
         rec["cov_ms"], _ = timed(lambda: gb.reduce2(_lib.OP_COV, v, v2))
         rec["corr_ms"], _ = timed(lambda: gb.reduce2(_lib.OP_CORR, v, v2))
         print(json.dumps(rec), flush=True)
@@ -94,6 +96,8 @@ def main():
             rec = {"shape": "one group", "rows": m, "groups": 1}
             rec["sum_rowindex_ms"], _ = timed(lambda: engine.reduce(_lib.OP_SUM, w, order, offsets))
             rec["prod_ms"], _ = timed(lambda: engine.reduce(_lib.OP_PROD, w, order, offsets))
+            rec["sd_ms"], _ = timed(lambda: engine.reduce(_lib.OP_SD, w, order, offsets))
+            rec["cov_ms"], _ = timed(lambda: engine.reduce2(_lib.OP_COV, w, w2, order, offsets))
             rec["corr_ms"], _ = timed(lambda: engine.reduce2(_lib.OP_CORR, w, w2, order, offsets))
             print(json.dumps(rec), flush=True)
             res["cases"].append(rec)
