@@ -31,7 +31,7 @@ EXPORTS = [
     "dtb_gather", "dtb_memcpy", "dtb_set_option", "dtb_get_option", "dtb_last_call_stats",
     "dtb_profile_count", "dtb_profile_get", "dtb_profile_reset",
     "dtb_dense_scatter", "dtb_dense_compact",
-    "dtb_sort_grouped", "dtb_qcut", "dtb_cumulative_out_stype", "dtb_cumulative", "dtb_shift", "dtb_fillna", "dtb_group_index",
+    "dtb_sort_grouped", "dtb_qcut", "dtb_cut", "dtb_cumulative_out_stype", "dtb_cumulative", "dtb_shift", "dtb_fillna", "dtb_group_index",
     "dtb_set_select", "dtb_largest_group", "dtb_join", "dtb_join_gather", "dtb_mask_rows", "dtb_int_rows", "dtb_cache_begin", "dtb_cache_end", "dtb_lower_bound",
 ]
 
@@ -125,6 +125,8 @@ def _load():
                                       c.POINTER(c.c_int64), c.c_void_p]
     lib.dtb_sort_grouped.argtypes = [dtb_col, c.c_int64, c.c_void_p, c.c_void_p, c.c_int64, c.c_void_p, c.c_void_p]
     lib.dtb_qcut.argtypes = [dtb_col, c.c_int64, c.c_void_p, c.c_void_p, c.c_int64, c.c_int, c.c_void_p, c.c_void_p]
+    lib.dtb_cut.argtypes = [dtb_col, c.c_int64, c.c_void_p, c.c_int, c.c_int64, c.c_int, c.c_void_p, c.c_int64, c.c_int,
+                            c.c_void_p, c.c_void_p]
     lib.dtb_cumulative_out_stype.argtypes = [c.c_int, c.c_int]
     lib.dtb_cumulative.argtypes = [c.c_int, c.c_int, dtb_col, c.c_int64, c.c_void_p, c.c_int, c.c_void_p, c.c_int64,
                                    c.c_void_p, c.c_void_p]

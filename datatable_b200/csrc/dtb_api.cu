@@ -1852,6 +1852,67 @@ int dtb_qcut(dtb_col value, int64_t nrows_value, const void* order, const void* 
   return c.finish(true);
 }
 
+int dtb_cut(dtb_col value, int64_t nrows_value, const void* order, int order_is64, int64_t n, int nbins,
+            const double* edges, int64_t nedges, int right_closed, dtb_stream stream, void* out)
+{
+  cudaStream_t s = (cudaStream_t)stream;
+  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
+  if (!edges) {
+    if (nbins <= 0) { set_error("Number of bins must be positive, instead got: " + std::to_string(nbins)); return DTB_EINVAL; }
+  } else {
+    if (nedges < 2) { set_error("To bin data at least two edges are required"); return DTB_EINVAL; }
+    if (edges[0] != edges[0]) { set_error("Bin edges must be numeric values only: edge 0 is NaN"); return DTB_EINVAL; }
+    for (int64_t i = 1; i < nedges; i++)
+      if (!(edges[i] > edges[i - 1])) {            // NaN fails the comparison too
+        set_error("Bin edges must be strictly increasing: edges " + std::to_string(i - 1) + " and " + std::to_string(i));
+        return DTB_EINVAL;
+      }
+  }
+  DTB_TRY(fixed_width(value.stype, "cut()"));
+  if (value.stype == DTB_STYPE_DATE32 || value.stype == DTB_STYPE_TIME64) {
+    set_error("cut() can only be applied to numeric columns, instead got stype " + std::to_string(value.stype));
+    return DTB_EINVAL;
+  }
+  if (n < 0 || nrows_value < 0) { set_error("negative size"); return DTB_EINVAL; }
+  if (!value.data && nrows_value > 0) { set_error("value column data is NULL"); return DTB_EINVAL; }
+  if (!order && n > 0 && n != nrows_value) { set_error("without an order, n must equal nrows_value"); return DTB_EINVAL; }
+  if (!out && n > 0) { set_error("out is NULL"); return DTB_EINVAL; }
+  DTB_TRY(ensure_context());
+  if (n == 0) return DTB_OK;
+  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
+  DevIn d_val, d_ord;
+  DTB_TRY(d_val.bind(value.data, (size_t)nrows_value * stype_bytes(value.stype), s));
+  DTB_TRY(d_ord.bind(order, (size_t)n * (order_is64 ? 8 : 4), s));
+  DevOut d_out; DTB_TRY(d_out.bind(out, (size_t)n * 4, s));
+  if (!edges) {
+    DevBuf st; DTB_TRY(st.alloc(sizeof(ColStats) + sizeof(CutCoef), s));
+    ColStats* d_stats = st.as<ColStats>();
+    CutCoef* d_coef = (CutCoef*)(d_stats + 1);
+    {
+      ProfScope ps("cut_stats", s);
+      if (d_ord.dptr) DTB_TRY(launch_col_stats_gather(d_val.dptr, value.stype, nrows_value, d_ord.dptr, order_is64, n,
+                                                      d_stats, s));
+      else            DTB_TRY(launch_col_stats(d_val.dptr, value.stype, n, d_stats, s));
+      DTB_TRY(launch_cut_coef(d_stats, value.stype, nbins, right_closed ? 1 : 0, d_coef, s));
+    }
+    {
+      ProfScope ps("cut_emit", s);
+      DTB_TRY(launch_cut_emit(d_val.dptr, value.stype, nrows_value, d_ord.dptr, order_is64, n, d_coef,
+                              (int32_t*)d_out.dptr, s));
+    }
+  } else {
+    DevIn d_edges; DTB_TRY(d_edges.bind(edges, sizeof(double) * (size_t)nedges, s));
+    ProfScope ps("cut_bins", s);
+    DTB_TRY(launch_cut_bins(d_val.dptr, value.stype, nrows_value, d_ord.dptr, order_is64, n,
+                            (const double*)d_edges.dptr, nedges, right_closed ? 1 : 0, (int32_t*)d_out.dptr, s));
+  }
+  if (d_out.staged()) {
+    DTB_TRY(d_out.finish((size_t)n * 4, s));
+    DTB_CUDA_CHECK(cudaStreamSynchronize(s));
+  }
+  return DTB_OK;
+}
+
 int dtb_set_select(int mode, const void* order, const void* offsets, int64_t ngroups, const int64_t* cum_sizes,
                    int ninputs, dtb_stream stream, void* rows_out, int64_t* nout)
 {

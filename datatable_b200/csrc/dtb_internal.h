@@ -61,6 +61,10 @@ size_t stats_hist_bytes(int64_t n);          // bytes of tile_hist (tile_na foll
 size_t stats_na_bytes(int64_t n);
 int launch_col_stats_hist(const void* data, int stype, int64_t n, ColStats* d_stats, unsigned short* tile_hist,
                           unsigned short* tile_na, cudaStream_t s);
+// The same statistics (bits_or / bits_and included) over the n positions of a RowIndex: position p reads
+// data[order[p]] (int32 or int64 row ids), and an index outside [0, nrows) counts as an NA row.
+int launch_col_stats_gather(const void* data, int stype, int64_t nrows, const void* order, int order_is64, int64_t n,
+                            ColStats* d_stats, cudaStream_t s);
 
 // ---------------------------------------------------------------------------
 // Key normalisation parameters for one key column (restates _initB/_initI/_initF,
@@ -329,6 +333,16 @@ int launch_distinct_flags(const void* v, int stype, int64_t nv, const int32_t* o
 size_t qcut_scratch_bytes(int64_t nc, int64_t ng);
 int launch_qcut(const void* vg, int stype, const int32_t* cord, const int32_t* coff, int64_t nc, const int32_t* gid,
                 int64_t ng, int64_t n, int q, void* scratch, int32_t* out, cudaStream_t s);
+// cut over the n positions of a RowIndex (dtb_cut, dtb_cut.cu); order NULL = identity.  out: int32[n].
+//   nbins mode: launch_cut_coef turns the statistics of the column seen through the RowIndex into the coefficients
+//               (device, one CutCoef), then launch_cut_emit writes the bins;
+//   edges mode: launch_cut_bins searches d_edges (device float64[nedges], strictly increasing, nedges >= 2).
+struct CutCoef { double a, b; int32_t shift, na; };
+int launch_cut_coef(const ColStats* d_stats, int stype, int nbins, int right_closed, CutCoef* coef, cudaStream_t s);
+int launch_cut_emit(const void* v, int stype, int64_t nv, const void* order, int order_is64, int64_t n,
+                    const CutCoef* coef, int32_t* out, cudaStream_t s);
+int launch_cut_bins(const void* v, int stype, int64_t nv, const void* order, int order_is64, int64_t n,
+                    const double* d_edges, int64_t nedges, int right_closed, int32_t* out, cudaStream_t s);
 // cumsum / cumprod / cummin / cummax inside every group (dtb_cumulative, dtb_reduce.cu): op DTB_OP_SUM / PROD / MIN /
 // MAX; out[p]: n elements of cumulative_out_stype(op, stype) (0: the op refuses the stype) for RowIndex position p.
 // scratch: cumulative_scratch_bytes(n) of device memory.

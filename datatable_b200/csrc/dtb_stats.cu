@@ -200,14 +200,68 @@ col_stats_hist_kernel(const typename RawKey<T>::load_t* __restrict__ data, int64
   stats_commit<T, IS_FLOAT>(acc, out);
 }
 
-template <typename T, bool IS_FLOAT>
-static int run_stats(const void* data, int64_t n, ColStats* d_stats, cudaStream_t s,
-                     unsigned short* tile_hist, unsigned short* tile_na) {
+// ---- statistics of the column seen through a RowIndex (cut over selected rows) -------------------------------
+// Position p reads data[order[p]]; an index outside [0, nrows) is an NA row.  Each thread issues GATHER_IPT index
+// loads, then GATHER_IPT value loads, before it folds any of them.
+constexpr int GATHER_IPT = 8;
+
+template <typename T, bool IS_FLOAT, typename OrdT>
+__global__ void __launch_bounds__(512)
+col_stats_gather_kernel(const typename RawKey<T>::load_t* __restrict__ data, int64_t nrows,
+                        const OrdT* __restrict__ order, int64_t n, ColStats* out)
+{
+  typedef typename RawKey<T>::load_t L;
+  StatAcc<T, IS_FLOAT> acc; acc.init();
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x * GATHER_IPT;
+  for (int64_t p0 = (int64_t)blockIdx.x * blockDim.x * GATHER_IPT + threadIdx.x; p0 < n; p0 += stride) {
+    int64_t j[GATHER_IPT];
+#pragma unroll
+    for (int k = 0; k < GATHER_IPT; k++) {
+      const int64_t p = p0 + (int64_t)k * blockDim.x;
+      j[k] = p < n ? (int64_t)order[p] : -1;
+    }
+    L raw[GATHER_IPT];
+#pragma unroll
+    for (int k = 0; k < GATHER_IPT; k++) raw[k] = (j[k] >= 0 && j[k] < nrows) ? data[j[k]] : raw_na<T>();
+#pragma unroll
+    for (int k = 0; k < GATHER_IPT; k++) if (p0 + (int64_t)k * blockDim.x < n) acc.add(raw[k]);   // every position, NA rows included
+  }
+  stats_commit<T, IS_FLOAT>(acc, out);
+}
+
+template <bool IS_FLOAT>
+static int stats_init(ColStats* d_stats, cudaStream_t s) {
   ColStats init;
   if (IS_FLOAT) { init.lo = ~0ull; init.hi = 0ull; }
   else { init.lo = (u64)INT64_MAX; init.hi = (u64)INT64_MIN; }
   init.bits_or = 0; init.bits_and = ~0ull; init.nacount = 0; init.nvalid = 0;
   DTB_CUDA_CHECK(cudaMemcpyAsync(d_stats, &init, sizeof(init), cudaMemcpyHostToDevice, s));
+  return DTB_OK;
+}
+
+int launch_col_stats_gather(const void* data, int stype, int64_t nrows, const void* order, int order_is64, int64_t n,
+                            ColStats* d_stats, cudaStream_t s) {
+  return with_stype(stype, "Unable to compute statistics of a Column of stype ", [&](auto t) {
+    typedef typename decltype(t)::type T;
+    constexpr bool F = std::is_floating_point<T>::value;
+    DTB_TRY(stats_init<F>(d_stats, s));
+    if (n == 0) return DTB_OK;
+    const int threads = 512;
+    with_order(order, order_is64, [&](auto o) {
+      col_stats_gather_kernel<T, F><<<grid_for((n + threads * GATHER_IPT - 1) / (threads * GATHER_IPT), 4), threads, 0,
+                                      s>>>(reinterpret_cast<const typename RawKey<T>::load_t*>(data), nrows, o, n,
+                                           d_stats);
+    });
+    count_launch();
+    DTB_CUDA_CHECK(cudaGetLastError());
+    return DTB_OK;
+  });
+}
+
+template <typename T, bool IS_FLOAT>
+static int run_stats(const void* data, int64_t n, ColStats* d_stats, cudaStream_t s,
+                     unsigned short* tile_hist, unsigned short* tile_na) {
+  DTB_TRY(stats_init<IS_FLOAT>(d_stats, s));
   if (n > 0 && tile_hist) {
     const int64_t nchunks = (n + CHUNK_ROWS - 1) / CHUNK_ROWS;
     col_stats_hist_kernel<T, IS_FLOAT><<<(unsigned)nchunks, PASS_THREADS, 0, s>>>(

@@ -426,6 +426,28 @@ def qcut(value, order, offsets, nquantiles=10, stype=None):
     return out
 
 
+def cut(value, order, nbins=10, edges=None, right_closed=True, stype=None):
+    """CutNbins_ColumnImpl / CutBins_ColumnImpl (column/cut.h:91-281) over the column seen through the RowIndex
+    `order` (None = identity; int32 or int64, an index < 0 is an NA row), as dt.cut without by() (dtb_cut): equal-width
+    bins between the min and max of those rows, or the bins of `edges` (float64, strictly increasing, at least 2; nbins
+    is then ignored).  Returns the int32 bins, one per position of `order`, NA as INT32_MIN; in HBM when the inputs
+    are."""
+    v = Col(value, stype)
+    o = None if order is None else Col(order)
+    if o is not None and o.stype not in (INT32, INT64):
+        raise _lib.DtbValueError("order must be int32 or int64")
+    if not -2**31 <= int(nbins) < 2**31:
+        raise _lib.DtbValueError(f"nbins does not fit in an int32: {nbins}")
+    e = None if edges is None else np.ascontiguousarray(edges, dtype=np.float64)
+    n = v.nrows if o is None else o.nrows
+    device = v.on_device and (o is None or o.on_device)
+    out, optr = _alloc(n, INT32, device)
+    check(lib.dtb_cut(v.c(), v.nrows, None if o is None else ctypes.c_void_p(o.ptr), 1 if o is not None and o.stype == INT64
+                      else 0, n, int(nbins), None if e is None else ctypes.c_void_p(e.ctypes.data),
+                      0 if e is None else e.shape[0], 1 if right_closed else 0, _stream(), ctypes.c_void_p(optr)))
+    return out
+
+
 def cumulative_out_stype(op, stype):
     return lib.dtb_cumulative_out_stype(op, stype)
 

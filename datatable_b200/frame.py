@@ -135,9 +135,9 @@ def count(x=None):
 
 class RowFn:
     """A function that returns one value per row and runs inside every group, the result in the grouped order (GtoALL):
-    qcut, cumsum, cumprod, cummin, cummax, shift, fillna, cumcount, ngroup.  `cols` as given (a column, a list or tuple
-    of columns, or f[:]; None for a function of no column); when the query runs they are resolved and columns() makes
-    one RowFnCol per column, with the function's checks of its other arguments (evaluate_n of the reference's FExpr)."""
+    qcut, cut, cumsum, cumprod, cummin, cummax, shift, fillna, cumcount, ngroup.  `cols` as given (a column, a list or
+    tuple of columns, or f[:]; None for a function of no column; a Frame for cut); when the query runs they are
+    resolved and columns() makes one RowFnCol per column, with the function's checks of its other arguments (evaluate_n of the reference's FExpr)."""
     def __init__(self, cols):
         self.cols = cols
 
@@ -145,9 +145,9 @@ class RowFn:
 class RowFnCol:
     """One output column of a RowFn over column `name`: run(c, order, offsets) -> (values, stype), one value per
     position of the RowIndex `order`, computed inside every group of `offsets`.  name None: the function reads no
-    column (c is None) and its output is unnamed (C0, C1, ...)."""
-    def __init__(self, name, run):
-        self.name, self.run = name, run
+    column of the query's frame (c is None) and its output is named `label`, or unnamed (C0, C1, ...) without one."""
+    def __init__(self, name, run, label=None):
+        self.name, self.run, self.label = name, run, label
 
 
 class Qcut(RowFn):
@@ -182,6 +182,138 @@ class Qcut(RowFn):
 
 def qcut(cols, nquantiles=None):
     return Qcut(cols, nquantiles)
+
+
+_NUMERIC = (BOOL, INT8, INT16, INT32, INT64, FLOAT32, FLOAT64)
+
+
+class Cut(RowFn):
+    """dt.cut(cols, nbins=None, bins=None, right_closed=True) (expr/fexpr_cut.cc:88-170): nbins (a list, one per
+    column, or one value for all) or the float64 bin edges of every column, checked by cut(); the column count and
+    the stypes are checked when the query runs.  Refused under by(), as the reference refuses it.  cols may be a
+    Frame with the query's row count: its columns are binned as they are, in the Frame's own row order."""
+    def __init__(self, cols, nbins, edges, right_closed):
+        super().__init__(cols)
+        self.nbins, self.edges, self.right_closed = nbins, edges, right_closed
+
+    def columns(self, DT, refs):
+        framearg = isinstance(self.cols, Frame)
+        src = self.cols if framearg else DT
+        ncols = len(refs)
+        if self.edges is not None:
+            if len(self.edges) != ncols:
+                raise ValueError(f"Number of elements in bins must be equal to the number of columns in the "
+                                 f"frame/expression, i.e. {ncols}, instead got: {len(self.edges)}")
+        elif len(self.nbins) != ncols and len(self.nbins) != 1:
+            raise ValueError(f"When nbins has more than one element, its length must be the same as the number of "
+                             f"columns in the frame/expression, i.e. {ncols}, instead got: {len(self.nbins)}")
+        out = []
+        for i, r in enumerate(refs):
+            st = src._stypes[r.name]
+            if st not in _NUMERIC:
+                sep = "" if self.edges is not None else " "       # the reference's two texts differ by this space
+                raise TypeError(f"cut() can only be applied to numeric{sep}columns, instead column {i} has an stype: "
+                                f"{_STYPE_NAMES.get(st, st)}")
+            kw = (dict(nbins=10, edges=self.edges[i]) if self.edges is not None else
+                  dict(nbins=self.nbins[i % len(self.nbins)]))
+            if not framearg:
+                out.append(RowFnCol(r.name, lambda c, order, offsets, kw=kw:
+                                    (engine.cut(c, order, right_closed=self.right_closed, **kw), INT32)))
+            else:
+                out.append(RowFnCol(None, lambda c, order, offsets, nm=r.name, kw=kw:
+                                    (self._frame_cut(DT, nm, order, kw), INT32), label=r.name))
+        return out
+
+    def _frame_cut(self, DT, name, order, kw):
+        """FExpr_Frame::evaluate_n (expr/fexpr_frame.cc:77-95): the Frame must have the query's row count."""
+        F = self.cols
+        n = DT.nrows if order is None else len(order)
+        if F.nrows != n:
+            if F.nrows == 1:
+                raise NotImplementedError("a 1-row Frame broadcast to the rows of a query is outside the GPU hot path")
+            raise ValueError(f"Frame has {F.nrows} rows, and cannot be used in an expression where {n} are expected")
+        return engine.cut(engine.Col(_dev(F._col(name)), F._stypes[name]), None, right_closed=self.right_closed, **kw)
+
+
+def cut(*args, cols=None, nbins=None, bins=None, right_closed=True):
+    """pyfn_cut (expr/fexpr_cut.cc:217-302): equal-width bins over the min / max of every column (nbins, default
+    10), or bins between explicit edges (bins: a list or tuple of 1-column Frames of at least 2 strictly increasing
+    numeric values), as int32 with NA as INT32_MIN.  The arguments are checked here, with the reference's texts."""
+    if len(args) > 1:
+        raise TypeError(f"Function datatable.cut() takes only one positional argument, but {len(args)} were given")
+    if args:
+        cols = args[0]
+    elif cols is None:
+        raise TypeError("Function datatable.cut() requires exactly 1 positional argument, but none were given")
+    if right_closed is None:
+        right_closed = True
+    if not isinstance(right_closed, bool):
+        raise TypeError(f"Argument right_closed in function datatable.cut() should be a boolean, instead got "
+                        f"{type(right_closed)}")
+    if bins is not None and nbins is not None:
+        raise ValueError("bins and nbins cannot be both set at the same time")
+    edges, nb = None, None
+    if bins is not None:
+        if not isinstance(bins, (list, tuple)):
+            raise TypeError(f"bins parameter must be a list or a tuple, instead got {type(bins)}")
+        edges = [_bin_edges(F, i) for i, F in enumerate(bins)]
+    elif isinstance(nbins, (list, tuple)):
+        nb = []
+        for i, x in enumerate(nbins):
+            x = _cut_int32(x)
+            if x <= 0:
+                raise ValueError(f"All elements in nbins must be positive, got nbins[{i}]: {x}")
+            nb.append(x)
+    else:
+        x = 10 if nbins is None else _cut_int32(nbins)
+        if x <= 0:
+            raise ValueError(f"Number of bins must be positive, instead got: {x}")
+        nb = [x]
+    if not isinstance(cols, Frame):
+        _column_args_only("cut", cols)
+    return Cut(cols, nb, edges, right_closed)
+
+
+def _cut_int32(x):
+    """to_int32_strict as pyfn_cut raises it: the reference's text says "too large" on both sides of the range."""
+    if isinstance(x, int) and not isinstance(x, bool) and x < -2**31:
+        raise ValueError(f"Value is too large to fit in an int32: {x}")
+    return _to_int32_strict(x)
+
+
+def _bin_edges(F, i):
+    """The edges of bins Frame number i as float64, read to the host once (FExpr_Cut::bins_to_vector,
+    fexpr_cut.cc:172-210)."""
+    if not isinstance(F, Frame):
+        raise TypeError(f"Expected a Frame, instead got {type(F)}")
+    if F.ncols != 1:
+        raise ValueError(f"To bin a column cut() needs exactly one column with the bin edges, instead for the frame "
+                         f"{i} got: {F.ncols}")
+    if F.nrows < 2:
+        raise ValueError(f"To bin data at least two edges are required, instead for the frame {i} got: {F.nrows}")
+    st = F.stypes[0]
+    if st not in _NUMERIC:
+        raise TypeError(f"Bin edges must be provided as the numeric columns only, instead for the frame {i} the column "
+                        f"stype is {_STYPE_NAMES.get(st, st)}")
+    a = F.to_numpy(F.names[0])
+    na = np.isnan(a) if st in (FLOAT32, FLOAT64) else a == _NA_VALUE[st]
+    e = a.astype(np.float64)                       # int64 rounds to nearest, as cast_inplace(FLOAT64) does
+    for k in range(len(e)):
+        if na[k]:
+            raise ValueError(f"Bin edges must be numeric values only, instead for the frame {i} got None at row {k}")
+        if k and not e[k] > e[k - 1]:
+            raise ValueError(f"Bin edges must be strictly increasing, instead for the frame {i} at rows {k - 1} and {k} "
+                             f"the values are {e[k - 1]:g} and {e[k]:g}")
+    return e
+
+
+def _has_cut(j):
+    """Whether j holds a cut() (in a list, tuple or dict)."""
+    if isinstance(j, Cut):
+        return True
+    if isinstance(j, (list, tuple)):
+        return builtins.any(_has_cut(x) for x in j)
+    return isinstance(j, dict) and builtins.any(_has_cut(x) for x in j.values())
 
 
 _STYPE_NAMES = {BOOL: "bool8", INT8: "int8", INT16: "int16", INT32: "int32", INT64: "int64", FLOAT32: "float32",
@@ -336,6 +468,8 @@ def _rowfn_cols(DT, e, bynames):
     leaves out the by() columns."""
     if e.cols is None:
         return e.columns(DT, [])
+    if isinstance(e, Cut) and isinstance(e.cols, Frame):    # FExpr_Frame::evaluate_n: the Frame's own columns
+        return e.columns(DT, [ColRef(nm) for nm in e.cols.names])
     refs = []
     for c in _flatten([e.cols]):
         if isinstance(c, ColRef) and isinstance(c.name, slice):
@@ -684,6 +818,8 @@ def _resolve(DT, j, by_, sort_, isel=None):
     if by_ is not None and sort_ is not None and sort_.na_position == "remove":
         # the rows dropped from the front of the RowIndex would still be counted by the groups
         raise ValueError("na_position = \"remove\" in sort() is not supported together with by()")
+    if by_ is not None and _has_cut(j):                # FExpr_Cut::evaluate_n checks ctx.has_groupby() first
+        raise NotImplementedError("cut() cannot be used in a groupby context")
     if by_ is not None:
         by_ = copy.copy(by_)
         by_.cols = [_bind(DT, r) for r in by_.cols]
@@ -1224,7 +1360,7 @@ def _resolve_j(DT, j, bynames=()):
             for x in vs:
                 if isinstance(x, RowFn):                        # several columns: k.x, k.y, ...
                     qc = _rowfn_cols(DT, x, bynames)
-                    names += [k] if len(qc) == 1 else [f"{k}.{c.name}" for c in qc]
+                    names += [k] if len(qc) == 1 else [f"{k}.{c.label or c.name}" for c in qc]
                     es += qc
                 else:
                     names.append(k)
@@ -1238,13 +1374,13 @@ def _resolve_j(DT, j, bynames=()):
     names = []
     nbin = 0
     for e in es:
-        if isinstance(e, Reducer2) or (isinstance(e, RowFnCol) and e.name is None):
+        if isinstance(e, Reducer2) or (isinstance(e, RowFnCol) and e.name is None and e.label is None):
             names.append(f"C{nbin}")                                  # unnamed columns (cov, corr, cumcount, ngroup): C0, C1, ...
             nbin += 1
         elif isinstance(e, Reducer):
             names.append("count" if e.arg is None else e.arg.name)     # reducers keep the column's name
         else:
-            names.append(e.name)
+            names.append(e.label if isinstance(e, RowFnCol) and e.label is not None else e.name)
     return names, es
 
 

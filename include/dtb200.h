@@ -460,6 +460,34 @@ DTB_API int dtb_qcut(dtb_col value, int64_t nrows_value, const void* order, cons
                      int nquantiles, dtb_stream stream, void* out);
 
 /*
+ * dtb_cut -- replaces CutNbins_ColumnImpl and CutBins_ColumnImpl (column/cut.h:91-281) as FExpr_Cut::evaluate_n runs
+ * them over a whole column (expr/fexpr_cut.cc:88-170; the reference refuses cut() under by()).  The value column
+ * (nrows_value rows) is seen through `order`: n positions, int32 row ids or int64 when order_is64; an index outside
+ * [0, nrows_value) is an NA row, as in dtb_gather.  order NULL = the identity, and then n must be 0 or nrows_value.
+ * Values are compared and scaled as float64: int64 rounded to nearest, NaN and the integer sentinels are NA.
+ *   edges NULL (nbins mode): min and max of the valid values at the n positions, as float64.  No valid value, or an
+ *     infinite min or max: every row is NA.  Else, rc = right_closed != 0:
+ *       min == max:  a = 0, b = (nbins - rc) / 2 (integer division), shift = 0
+ *       else:        a = (1 - FLT_EPSILON) * nbins / (max - min), b = -a * min, shift = 0 (rc), or
+ *                    b = -a * max, shift = nbins - 1 (not rc); max - min may overflow to inf, giving a = 0
+ *     and every valid v gets int32(a * v + b) + shift.  a * v + b is a multiply and an add, each rounded to nearest
+ *     (no fused multiply-add), as the reference computes it.  int32(r) truncates, and is INT32_MIN for a NaN or an r
+ *     outside the int32 range (x86-64's conversion, which the reference's static_cast compiles to); the add of shift
+ *     wraps.  The coefficients are computed on the device: the call does not wait for the statistics.
+ *   edges != NULL: a host float64[nedges] array, nedges >= 2, strictly increasing; nbins is ignored.  With
+ *     c = #{k : edges[k] < v} (right_closed) or #{k : edges[k] <= v} (not), v gets c - 1 when 1 <= c <= nedges - 1,
+ *     i.e. v in (edges[0], edges[nedges-1]] (right_closed) or [edges[0], edges[nedges-1]); else NA.  That is the
+ *     reference's bisection with v > e or v >= e.
+ * out: int32[n], out[p] = the bin of the row at position p, NA as INT32_MIN.  Host or device pointers (edges: host).
+ * Bit-exact.  Asynchronous unless out is host memory.  Arguments are checked in this order, on the host before any
+ * CUDA call: nbins <= 0 (nbins mode), or nedges < 2, a NaN edge, edges not strictly increasing: DTB_EINVAL; an stype
+ * without a fixed width: DTB_ENOTIMPL; date32 / time64: DTB_EINVAL; n < 0 or nrows_value < 0, value data NULL while
+ * nrows_value > 0, order NULL while 0 < n != nrows_value, out NULL while n > 0: DTB_EINVAL.  n == 0 then returns at once.
+ */
+DTB_API int dtb_cut(dtb_col value, int64_t nrows_value, const void* order, int order_is64, int64_t n, int nbins,
+                    const double* edges, int64_t nedges, int right_closed, dtb_stream stream, void* out);
+
+/*
  * dtb_set_select -- the group-selection step of union / intersect / setdiff / symdiff
  * (set_funcs.cc:126-456).  The caller concatenated K single-column inputs (input k holds the rows
  * cum_sizes[k-1] .. cum_sizes[k]-1), grouped the result with dtb_group and passes its (order, offsets).
