@@ -1353,7 +1353,8 @@ static int bind_groupby(const void* offsets, int64_t ngroups, bool check_offsets
                         int64_t& n)
 {
   DTB_TRY(d_off.bind(offsets, sizeof(int32_t) * (size_t)(ngroups + 1), s));
-  // caller-supplied offsets must be a Groupby: offsets[0] = 0, strictly increasing (groupby.h:41-47)
+  // caller-supplied offsets must be a Groupby: offsets[0] = 0, strictly increasing (groupby.h:41-47), or the one
+  // empty group [0, 0] of zero rows (Groupby::single_group(0), groupby.cc:60-68)
   int32_t n32 = 0;
   int bad = 0;
   if (is_device_ptr(offsets)) {
@@ -1367,7 +1368,9 @@ static int bind_groupby(const void* offsets, int64_t ngroups, bool check_offsets
     const int32_t* ho = (const int32_t*)offsets;
     n32 = ho[ngroups];
     if (ho[0] != 0) bad = 1;
-    for (int64_t g = 0; g < ngroups && !bad; g++) if (ho[g] >= ho[g + 1]) bad = (int)(g < INT32_MAX ? g + 1 : INT32_MAX);
+    const bool single_empty = ngroups == 1 && n32 == 0;
+    for (int64_t g = 0; g < ngroups && !bad; g++)
+      if (ho[g] >= ho[g + 1] && !single_empty) bad = (int)(g < INT32_MAX ? g + 1 : INT32_MAX);
   }
   if (bad) {
     set_error("offsets is not a Groupby: offsets[0] must be 0 and offsets strictly increasing (group " +
@@ -1419,7 +1422,12 @@ struct Grouped {
     if (nrows_value < 0) { set_error("nrows_value must be non-negative"); return DTB_EINVAL; }
     for (int i = 0; i < nvalues; i++)
       if (!value[i].data && nrows_value > 0) { set_error("value column data is NULL"); return DTB_EINVAL; }
-    if (!out && ngroups > 0) { set_error("out is NULL"); return DTB_EINVAL; }
+    // one output per position: the one empty group [0, 0] has none, so out may be NULL there (a 0-element tensor's
+    // data pointer); device offsets are read in bind()
+    if (!out && ngroups > 0 &&
+        !(per_position && ngroups == 1 && (is_device_ptr(offsets) || ((const int32_t*)offsets)[1] == 0))) {
+      set_error("out is NULL"); return DTB_EINVAL;
+    }
     DTB_TRY(ensure_context());
     if (ngroups == 0) return DTB_OK;
     scope.emplace(s);
@@ -1429,6 +1437,7 @@ struct Grouped {
   // out_esz: bytes per output element.
   int bind(int out_esz) {
     DTB_TRY(bind_groupby(offsets, ngroups, !handle, s, off, n));
+    if (!out && n > 0) { set_error("out is NULL"); return DTB_EINVAL; }
     if (within_column && !order && n > nrows_value) {
       set_error("offsets cover more rows than the value column has"); return DTB_EINVAL;
     }
@@ -1438,6 +1447,8 @@ struct Grouped {
     return dout.bind(out, (size_t)(per_position ? n : ngroups) * out_esz, s);
   }
 
+  // Afterwards n == 0 (no group, or the one empty group [0, 0]) leaves a per-position function nothing to write: it
+  // returns without a launch.  A reducer still writes the empty group's one result.
   int open(int out_esz) {
     DTB_TRY(enter());
     return ngroups ? bind(out_esz) : DTB_OK;
@@ -1563,7 +1574,7 @@ int dtb_cumulative(int op, int reverse, dtb_col value, int64_t nrows_value, cons
   }
   c.within_column = c.per_position = true;
   DTB_TRY(c.open(stype_bytes(out_st)));
-  if (c.ngroups == 0) return DTB_OK;
+  if (c.n == 0) return DTB_OK;
   DevBuf scr; DTB_TRY(scr.alloc(cumulative_scratch_bytes(c.n), c.s));
   {
     ProfScope ps("cumulative", c.s);
@@ -1580,7 +1591,7 @@ int dtb_shift(dtb_col value, int64_t nrows_value, const void* order, int order_i
   DTB_TRY(fixed_width(value.stype, "shift"));
   c.within_column = c.per_position = true;
   DTB_TRY(c.open(stype_bytes(value.stype)));
-  if (c.ngroups == 0) return DTB_OK;
+  if (c.n == 0) return DTB_OK;
   {
     ProfScope ps("shift", c.s);
     DTB_TRY(launch_shift(c.val[0].dptr, value.stype, nrows_value, c.ord.dptr, order_is64, c.offs(), ngroups, c.n, n,
@@ -1596,7 +1607,7 @@ int dtb_fillna(int reverse, dtb_col value, int64_t nrows_value, const void* orde
   DTB_TRY(fixed_width(value.stype, "fillna"));
   c.within_column = c.per_position = true;
   DTB_TRY(c.open(stype_bytes(value.stype)));
-  if (c.ngroups == 0) return DTB_OK;
+  if (c.n == 0) return DTB_OK;
   DevBuf scr; DTB_TRY(scr.alloc(cumulative_scratch_bytes(c.n), c.s));
   {
     ProfScope ps("fillna", c.s);
@@ -1614,7 +1625,7 @@ int dtb_group_index(int kind, int reverse, const void* offsets, int64_t ngroups,
   }
   c.per_position = true;
   DTB_TRY(c.open(sizeof(int64_t)));
-  if (c.ngroups == 0) return DTB_OK;
+  if (c.n == 0) return DTB_OK;
   {
     ProfScope ps("group_index", c.s);
     DTB_TRY(launch_group_index(kind, reverse, c.offs(), ngroups, c.n, (int64_t*)c.dout.dptr, c.s));
@@ -1822,7 +1833,7 @@ int dtb_sort_grouped(dtb_col value, int64_t nrows_value, const void* order, cons
   if (!stype_supported(value.stype)) { set_error("Unable to sort Column of stype " + std::to_string(value.stype)); return DTB_ENOTIMPL; }
   c.per_position = true;
   DTB_TRY(c.open(sizeof(int32_t)));
-  if (c.ngroups == 0) return DTB_OK;
+  if (c.n == 0) return DTB_OK;
   GroupedByValue gv;
   DTB_TRY(group_by_value(dtb_col{c.val[0].dptr, value.stype, 0}, nrows_value, c.ord.dptr, c.offs(), ngroups, c.n,
                          DTB_FLAG_SORT_ONLY, c.s, gv));
@@ -1841,7 +1852,7 @@ int dtb_qcut(dtb_col value, int64_t nrows_value, const void* order, const void* 
   DTB_TRY(fixed_width(value.stype, "qcut()"));
   c.within_column = c.per_position = true;
   DTB_TRY(c.open(sizeof(int32_t)));
-  if (c.ngroups == 0) return DTB_OK;
+  if (c.n == 0) return DTB_OK;
   GroupedByValue gv;
   DTB_TRY(group_by_value(dtb_col{c.val[0].dptr, value.stype, 0}, nrows_value, c.ord.dptr, c.offs(), ngroups, c.n, 0,
                          c.s, gv));

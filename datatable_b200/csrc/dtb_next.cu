@@ -50,7 +50,8 @@ __device__ __forceinline__ bool load_f64(const void* v, int st, int64_t j, doubl
 }
 
 // ===========================================================================
-// first / last: out[g] = v[order[offsets[g]]] or v[order[offsets[g+1]-1]] (NA stays NA)
+// first / last: out[g] = v[order[offsets[g]]] or v[order[offsets[g+1]-1]] (NA stays NA); the empty group of zero
+// rows, offsets [0, 0], is NA and reads no position
 // ===========================================================================
 template <typename E>
 __global__ void firstlast_kernel(const E* __restrict__ v, int64_t nv, const int32_t* __restrict__ order,
@@ -58,7 +59,9 @@ __global__ void firstlast_kernel(const E* __restrict__ v, int64_t nv, const int3
 {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += stride) {
-    const int64_t p = last ? (int64_t)offsets[g + 1] - 1 : (int64_t)offsets[g];
+    const int64_t a = offsets[g], b = offsets[g + 1];
+    if (a >= b) { out[g] = na; continue; }
+    const int64_t p = last ? b - 1 : a;
     const int64_t j = order ? (int64_t)order[p] : p;
     out[g] = (j >= 0 && j < nv) ? v[j] : na;
   }

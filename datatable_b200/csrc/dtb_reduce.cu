@@ -503,10 +503,12 @@ __global__ void prod_finalize_kernel(const int32_t* __restrict__ offsets, int64_
     if (g < ng) {
       p = prod_word<CAT>(acc0, acc1, g);
       const int64_t a = offsets[g], b = offsets[g + 1];
-      const int64_t ta = a / RTILE, tend = (ta + 1) * RTILE < n ? (ta + 1) * RTILE : n;
-      if (a == ta * RTILE) p_merge(p, prod_word<CAT>(c0, c1, 2 * ta), 0);
-      else if (b >= tend)  p_merge(p, prod_word<CAT>(c0, c1, 2 * ta + 1), 0);
-      t1 = ta + 1; t2 = (b - 1) / RTILE;
+      if (a < b) {                                             // the empty group of zero rows has no tile
+        const int64_t ta = a / RTILE, tend = (ta + 1) * RTILE < n ? (ta + 1) * RTILE : n;
+        if (a == ta * RTILE) p_merge(p, prod_word<CAT>(c0, c1, 2 * ta), 0);
+        else if (b >= tend)  p_merge(p, prod_word<CAT>(c0, c1, 2 * ta + 1), 0);
+        t1 = ta + 1; t2 = (b - 1) / RTILE;
+      }
     }
     const bool wide = t2 - t1 >= 32;
     if (!wide) for (int64_t t = t1; t <= t2; t++) p_merge(p, prod_word<CAT>(c0, c1, 2 * t), 0);
@@ -617,11 +619,15 @@ int reduce_out_stype_host(int op, int st) { return reduce_out_stype(op, st); }
 
 // Groupby invariants (groupby.h:41-47): offsets[0] = 0 and strictly increasing.  reduce_kernel marks
 // group starts in a one-bit-per-row bitmap, so an empty group would silently shift every later group of
-// the tile: caller-supplied offsets are checked first.  *bad receives the index of a violating group + 1.
+// the tile: caller-supplied offsets are checked first.  The one exception is the single group of zero rows,
+// offsets [0, 0] (Groupby::single_group(0), groupby.cc:60-68), which no row-parallel kernel sees.  *bad
+// receives the index of a violating group + 1.
 __global__ void offsets_check_kernel(const int32_t* __restrict__ offsets, int64_t ng, int* bad) {
+  const bool single_empty = ng == 1 && offsets[1] == 0;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < ng; g += stride) {
-    if (offsets[g] >= offsets[g + 1] || (g == 0 && offsets[0] != 0)) atomicMax(bad, (int)(g < INT32_MAX ? g + 1 : INT32_MAX));
+    if ((offsets[g] >= offsets[g + 1] && !single_empty) || (g == 0 && offsets[0] != 0))
+      atomicMax(bad, (int)(g < INT32_MAX ? g + 1 : INT32_MAX));
   }
 }
 

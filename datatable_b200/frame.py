@@ -1302,9 +1302,18 @@ def _reducer_cols(up, names, exprs, keys, order, groups, late):
     if late:
         late_results = iter([_late_reduce(up, gb, e) for e in _fused(exprs)])
     ifused = 0
+    npos = gb.norder if gb is not None else (up.frame.nrows if order is None else len(order))
     for name, e in zip(names, exprs):
         if not isinstance(e, Reducer):
             raise NotImplementedError("mixing reducers and plain columns under by() is outside the hot path")
+        if e.op == _lib.OP_MEDIAN and npos == 0 and _red_stype(up.col, e):
+            # over zero rows the reference's median is an NA column of its argument's own stype, not of the median's
+            # (compute_median, head_reduce_unary.cc:493-496)
+            st = up.col(e.arg.name).stype
+            ng = gb.ngroups if gb is not None else int(groups.shape[0]) - 1
+            yield name, torch.full((ng,), float("nan") if st in (FLOAT32, FLOAT64) else _NA_VALUE[st],
+                                   dtype=engine._torch_dtype(st), device="cuda"), st
+            continue
         if gb is None:
             data = _reduce(up.col, e, order, groups, bynames)
         elif isinstance(e, Reducer2):

@@ -213,10 +213,13 @@ DTB_API int         dtb_groupby_destroy(dtb_groupby* g, dtb_stream stream);
  *   1. the function's own argument (op, kind, nquantiles): DTB_EINVAL;
  *   2. the stype: one without a fixed width gives DTB_ENOTIMPL, one the op refuses DTB_EINVAL;
  *   3. ngroups < 0;  4. offsets NULL;  5. nrows_value < 0;  6. value data NULL while nrows_value > 0;
- *   7. out NULL while ngroups > 0: DTB_EINVAL.
+ *   7. out NULL while ngroups > 0 (for one output per position: unless the only group is [0, 0]): DTB_EINVAL.
  * ngroups == 0 then returns at once.  Caller offsets must be a Groupby (groupby.h:41-47): offsets[0] = 0 and
  * strictly increasing, so no group is empty; otherwise DTB_EINVAL (device offsets are checked on the device; a
- * handle's own offsets are not checked).  Positions beyond the value column: without an order, n > nrows_value is
+ * handle's own offsets are not checked).  The one exception is ngroups == 1 with offsets [0, 0], the single group
+ * of zero rows a query without by() reduces over (Groupby::single_group(0), groupby.cc:60-68): the reducers write
+ * its one result -- SUM 0, PROD 1, COUNT / COUNTNA / NROWS / NUNIQUE 0, every other reducer NA -- and the functions
+ * with one output per position write nothing.  No kernel reads a row or a RowIndex position for it.  Positions beyond the value column: without an order, n > nrows_value is
  * DTB_EINVAL for the row functions (dtb_cumulative, dtb_shift, dtb_fillna, dtb_qcut); the reducers and
  * dtb_sort_grouped read those positions as NA (nrows_value bounds the gather).
  */

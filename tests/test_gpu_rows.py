@@ -140,9 +140,8 @@ def _same(got, want, rtol):
 
 
 @pytest.mark.parametrize("device", [False, True], ids=["host", "device"])
-# DT[True, :] keeps its NotImplementedError.  Reducers over zero selected rows take the path of an empty slice, whose
-# one empty group the reducers refuse today, for every form of `i`.
-@pytest.mark.parametrize("case", [c for c in CASES if c["name"] not in ("err.bool_literal", "mask.norows_sum")],
+# DT[True, :] keeps its NotImplementedError.
+@pytest.mark.parametrize("case", [c for c in CASES if c["name"] not in ("err.bool_literal",)],
                          ids=lambda c: c["name"])
 def test_frame_against_golden(torch, case, device):
     env = _env(case, device)
