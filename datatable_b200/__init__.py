@@ -11,5 +11,6 @@ from . import engine
 from .frame import (Frame, f, g, by, sort, join, sum, prod, cov, corr, mean, min, max, count, countna, first, last, sd, median,   # noqa: A004
                     qcut, cut, cumsum, cumprod, cummin, cummax, shift, fillna, cumcount, ngroup, unique, nunique, union, intersect, setdiff, symdiff)
 from .jay import open_jay, save_jay
+from . import time
 
-__all__ = ["engine", "Frame", "f", "g", "by", "sort", "sum", "prod", "cov", "corr", "mean", "min", "max", "count", "countna", "first", "last", "sd", "median", "qcut", "cut", "cumsum", "cumprod", "cummin", "cummax", "shift", "fillna", "cumcount", "ngroup", "join", "unique", "nunique", "union", "intersect", "setdiff", "symdiff", "open_jay", "save_jay", "DtbError", "DtbValueError", "DtbNotImplError", "DtbCudaError", "DtbMemoryError"]
+__all__ = ["engine", "Frame", "f", "g", "by", "sort", "sum", "prod", "cov", "corr", "mean", "min", "max", "count", "countna", "first", "last", "sd", "median", "qcut", "cut", "cumsum", "cumprod", "cummin", "cummax", "shift", "fillna", "cumcount", "ngroup", "join", "time", "unique", "nunique", "union", "intersect", "setdiff", "symdiff", "open_jay", "save_jay", "DtbError", "DtbValueError", "DtbNotImplError", "DtbCudaError", "DtbMemoryError"]

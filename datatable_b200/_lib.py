@@ -19,6 +19,7 @@ OP_SUM, OP_MEAN, OP_MIN, OP_MAX, OP_COUNT, OP_COUNTNA, OP_NROWS = 1, 2, 3, 4, 5,
 OP_FIRST, OP_LAST, OP_SD, OP_MEDIAN, OP_NUNIQUE = 8, 9, 10, 11, 12
 OP_PROD, OP_COV, OP_CORR = 13, 14, 15
 GROUP_CUMCOUNT, GROUP_NGROUP = 1, 2
+TIME_YEAR, TIME_MONTH, TIME_DAY, TIME_DAY_OF_WEEK, TIME_HOUR, TIME_MINUTE, TIME_SECOND, TIME_NANOSECOND = range(1, 9)
 SET_UNION, SET_INTERSECT, SET_SETDIFF, SET_SYMDIFF = 0, 1, 2, 3
 OK, EINVAL, ENOTIMPL, ECUDA, ENOMEM, ENOSPACE = 0, -1, -2, -3, -4, -5
 
@@ -31,7 +32,7 @@ EXPORTS = [
     "dtb_gather", "dtb_memcpy", "dtb_set_option", "dtb_get_option", "dtb_last_call_stats",
     "dtb_profile_count", "dtb_profile_get", "dtb_profile_reset",
     "dtb_dense_scatter", "dtb_dense_compact",
-    "dtb_sort_grouped", "dtb_qcut", "dtb_cut", "dtb_cumulative_out_stype", "dtb_cumulative", "dtb_shift", "dtb_fillna", "dtb_group_index",
+    "dtb_sort_grouped", "dtb_qcut", "dtb_cut", "dtb_time_part", "dtb_cumulative_out_stype", "dtb_cumulative", "dtb_shift", "dtb_fillna", "dtb_group_index",
     "dtb_set_select", "dtb_largest_group", "dtb_join", "dtb_join_gather", "dtb_mask_rows", "dtb_int_rows", "dtb_cache_begin", "dtb_cache_end", "dtb_lower_bound",
 ]
 
@@ -127,6 +128,7 @@ def _load():
     lib.dtb_qcut.argtypes = [dtb_col, c.c_int64, c.c_void_p, c.c_void_p, c.c_int64, c.c_int, c.c_void_p, c.c_void_p]
     lib.dtb_cut.argtypes = [dtb_col, c.c_int64, c.c_void_p, c.c_int, c.c_int64, c.c_int, c.c_void_p, c.c_int64, c.c_int,
                             c.c_void_p, c.c_void_p]
+    lib.dtb_time_part.argtypes = [c.c_int, dtb_col, c.c_int64, c.c_void_p, c.c_int, c.c_int64, c.c_void_p, c.c_void_p]
     lib.dtb_cumulative_out_stype.argtypes = [c.c_int, c.c_int]
     lib.dtb_cumulative.argtypes = [c.c_int, c.c_int, dtb_col, c.c_int64, c.c_void_p, c.c_int, c.c_void_p, c.c_int64,
                                    c.c_void_p, c.c_void_p]

@@ -1924,6 +1924,46 @@ int dtb_cut(dtb_col value, int64_t nrows_value, const void* order, int order_is6
   return DTB_OK;
 }
 
+int dtb_time_part(int part, dtb_col value, int64_t nrows_value, const void* order, int order_is64, int64_t n,
+                  dtb_stream stream, void* out)
+{
+  cudaStream_t s = (cudaStream_t)stream;
+  t_stats = dtb_call_stats{0, 0, 0, 0, 0};
+  if (part < DTB_TIME_YEAR || part > DTB_TIME_NANOSECOND) {
+    set_error("unknown time part " + std::to_string(part)); return DTB_EINVAL;
+  }
+  DTB_TRY(fixed_width(value.stype, "time functions"));
+  if (value.stype != DTB_STYPE_DATE32 && value.stype != DTB_STYPE_TIME64) {
+    set_error("time functions need a date32 or time64 column, instead got stype " + std::to_string(value.stype));
+    return DTB_EINVAL;
+  }
+  if (value.stype == DTB_STYPE_DATE32 && part >= DTB_TIME_HOUR) {
+    set_error("hour, minute, second and nanosecond need a time64 column, instead got a date32 column");
+    return DTB_EINVAL;
+  }
+  if (n < 0 || nrows_value < 0) { set_error("negative size"); return DTB_EINVAL; }
+  if (!value.data && nrows_value > 0) { set_error("value column data is NULL"); return DTB_EINVAL; }
+  if (!order && n > 0 && n != nrows_value) { set_error("without an order, n must equal nrows_value"); return DTB_EINVAL; }
+  if (!out && n > 0) { set_error("out is NULL"); return DTB_EINVAL; }
+  DTB_TRY(ensure_context());
+  if (n == 0) return DTB_OK;
+  ArenaScope scope(s); if (scope.rc != DTB_OK) return scope.rc;
+  DevIn d_val, d_ord;
+  DTB_TRY(d_val.bind(value.data, (size_t)nrows_value * stype_bytes(value.stype), s));
+  DTB_TRY(d_ord.bind(order, (size_t)n * (order_is64 ? 8 : 4), s));
+  DevOut d_out; DTB_TRY(d_out.bind(out, (size_t)n * 4, s));
+  {
+    ProfScope ps("time_part", s);
+    DTB_TRY(launch_time_part(part, d_val.dptr, value.stype, nrows_value, d_ord.dptr, order_is64, n,
+                             (int32_t*)d_out.dptr, s));
+  }
+  if (d_out.staged()) {
+    DTB_TRY(d_out.finish((size_t)n * 4, s));
+    DTB_CUDA_CHECK(cudaStreamSynchronize(s));
+  }
+  return DTB_OK;
+}
+
 int dtb_set_select(int mode, const void* order, const void* offsets, int64_t ngroups, const int64_t* cum_sizes,
                    int ninputs, dtb_stream stream, void* rows_out, int64_t* nout)
 {

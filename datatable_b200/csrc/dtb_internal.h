@@ -343,6 +343,10 @@ int launch_cut_emit(const void* v, int stype, int64_t nv, const void* order, int
                     const CutCoef* coef, int32_t* out, cudaStream_t s);
 int launch_cut_bins(const void* v, int stype, int64_t nv, const void* order, int order_is64, int64_t n,
                     const double* d_edges, int64_t nedges, int right_closed, int32_t* out, cudaStream_t s);
+// part DTB_TIME_* of a date32 / time64 column over the n positions of a RowIndex (dtb_time_part, dtb_time.cu); order
+// NULL = identity.  out: int32[n].
+int launch_time_part(int part, const void* v, int stype, int64_t nv, const void* order, int order_is64, int64_t n,
+                     int32_t* out, cudaStream_t s);
 // cumsum / cumprod / cummin / cummax inside every group (dtb_cumulative, dtb_reduce.cu): op DTB_OP_SUM / PROD / MIN /
 // MAX; out[p]: n elements of cumulative_out_stype(op, stype) (0: the op refuses the stype) for RowIndex position p.
 // scratch: cumulative_scratch_bytes(n) of device memory.

@@ -448,6 +448,21 @@ def cut(value, order, nbins=10, edges=None, right_closed=True, stype=None):
     return out
 
 
+def time_part(part, value, order, stype=None):
+    """Part TIME_YEAR .. TIME_NANOSECOND of a date32 or time64 column seen through the RowIndex `order` (None =
+    identity; int32 or int64, an index < 0 is an NA row), as dt.time.year() .. nanosecond() compute it (dtb_time_part).
+    Returns int32, one value per position of `order`, NA as INT32_MIN; in HBM when the inputs are."""
+    v = Col(value, stype)
+    o = None if order is None else Col(order)
+    if o is not None and o.stype not in (INT32, INT64):
+        raise _lib.DtbValueError("order must be int32 or int64")
+    n = v.nrows if o is None else o.nrows
+    out, optr = _alloc(n, INT32, v.on_device and (o is None or o.on_device))
+    check(lib.dtb_time_part(int(part), v.c(), v.nrows, None if o is None else ctypes.c_void_p(o.ptr),
+                            1 if o is not None and o.stype == INT64 else 0, n, _stream(), ctypes.c_void_p(optr)))
+    return out
+
+
 def cumulative_out_stype(op, stype):
     return lib.dtb_cumulative_out_stype(op, stype)
 

@@ -135,8 +135,8 @@ def count(x=None):
 
 class RowFn:
     """A function that returns one value per row and runs inside every group, the result in the grouped order (GtoALL):
-    qcut, cut, cumsum, cumprod, cummin, cummax, shift, fillna, cumcount, ngroup.  `cols` as given (a column, a list or
-    tuple of columns, or f[:]; None for a function of no column; a Frame for cut); when the query runs they are
+    qcut, cut, cumsum, cumprod, cummin, cummax, shift, fillna, cumcount, ngroup, the time parts.  `cols` as given (a
+    column, a list or tuple of columns, or f[:]; None for a function of no column; a Frame for cut); when the query runs they are
     resolved and columns() makes one RowFnCol per column, with the function's checks of its other arguments (evaluate_n of the reference's FExpr)."""
     def __init__(self, cols):
         self.cols = cols
@@ -444,6 +444,74 @@ def cumcount(reverse=False): return GroupIndex(_lib.GROUP_CUMCOUNT, "cumcount", 
 def ngroup(reverse=False): return GroupIndex(_lib.GROUP_NGROUP, "ngroup", reverse)
 
 
+class TimePart(RowFn):
+    """dt.time.year / month / day / day_of_week / hour / minute / second / nanosecond(cols) (expr/time/): one int32
+    part of every date32 or time64 column, row by row, so the same under by() as without.  The columns' stypes are
+    checked when the query runs.  As a by() / sort() key (_as_ref) the part is a derived key column (_TKey); a minus
+    in front of it is the key's DESCENDING flag, as it is for a column (unnegate_column, fexpr_list.cc:346-358)."""
+    def __init__(self, part, fname, cols, negated=False):
+        _column_args_only(f"time.{fname}", cols)
+        for c in _flatten([cols]):
+            if isinstance(c, ColRef) and c.negated:
+                raise NotImplementedError(f"time.{fname}() of an expression ({c!r}) is outside the GPU hot path")
+        super().__init__(cols)
+        self.part, self.fname, self.negated = part, fname, negated
+
+    def __neg__(self):
+        return TimePart(self.part, self.fname, self.cols, not self.negated)
+
+    def __repr__(self):
+        return f"{'-' if self.negated else ''}time.{self.fname}({_cols_repr(self.cols)})"
+
+    def key_ref(self):
+        """The ColRef of this part as a by() / sort() key: one column, named by a _TKey of its (unbound) source."""
+        cols = _flatten([self.cols])
+        if len(cols) != 1 or (isinstance(cols[0], ColRef) and isinstance(cols[0].name, slice)):
+            raise NotImplementedError(f"{self!r} of several columns as a by() / sort() key is outside the GPU hot path")
+        src = _as_ref(cols[0])
+        return ColRef(_TKey(src, self.part, self.fname), self.negated)
+
+    def columns(self, DT, refs):
+        if self.negated:
+            raise NotImplementedError(f"{self!r} (arithmetic negation) is outside the GPU hot path")
+        out = []
+        for r in refs:
+            _time_stype_check(self.part, self.fname, DT._stypes[r.name])
+            out.append(RowFnCol(r.name, lambda c, order, offsets: (engine.time_part(self.part, c, order), INT32)))
+        return out
+
+
+def _time_stype_check(part, fname, st):
+    """FExpr_YearMonthDay / FExpr_DayOfWeek / FExpr_HourMinSec::evaluate1: date32 or time64 for the calendar parts,
+    time64 for the clock parts."""
+    calendar = part <= _lib.TIME_DAY_OF_WEEK
+    if st == TIME64 or (calendar and st == DATE32):
+        return
+    raise TypeError(f"Function time.{fname}() requires a {'date32 or time64' if calendar else 'time64'} column, "
+                    f"instead received column of type {_STYPE_NAMES.get(st, st)}")
+
+
+class _TKey(str):
+    """The name under which a query's stages read a time part of a column as a by() / sort() key: its text is the
+    source column's name (the result's key column is named after it), but it equals only the same part of the same
+    column, so f.d and year(f.d) never collide.  src: the source's ColRef until _bind binds it, then the source's name
+    (an X column's name or a _JKey)."""
+
+    def __new__(cls, src, part, fname):
+        k = str.__new__(cls, str(src.name) if isinstance(src, ColRef) else str(src))
+        k.src, k.part, k.fname = src, part, fname
+        return k
+
+    def __eq__(self, other):
+        return isinstance(other, _TKey) and other.part == self.part and other.src == self.src
+
+    def __ne__(self, other):
+        return not self == other
+
+    def __hash__(self):
+        return hash(("time", self.part, self.src))
+
+
 def _cols_repr(cols):
     if isinstance(cols, (list, tuple)):
         return "[" + ", ".join(_cols_repr(c) for c in cols) + "]"
@@ -530,6 +598,8 @@ def _flatten(cols):
 def _as_ref(c):
     if isinstance(c, ColRef):
         return c
+    if isinstance(c, TimePart):
+        return c.key_ref()
     if isinstance(c, str):
         return ColRef(c)
     raise TypeError(f"Unsupported key expression {c!r}: only column references are on the GPU path")
@@ -1083,6 +1153,13 @@ def _bind(DT, ref):
         if ref.frame:
             raise NotImplementedError("column slices of the join frame are outside the GPU hot path")
         return ref
+    if isinstance(ref.name, _TKey):                      # a time part as a key: bind its source column
+        src = ref.name.src if isinstance(ref.name.src, ColRef) else ColRef(ref.name.src)
+        nm = _bind(DT, src).name
+        if nm not in DT._stypes:
+            raise KeyError(f"Column `{nm}` does not exist in the Frame")
+        _time_stype_check(ref.name.part, ref.name.fname, DT._stypes[nm])
+        return ColRef(_TKey(nm, ref.name.part, ref.name.fname), ref.negated)
     J = DT._joined
     if ref.frame:
         if J is None:
@@ -1099,6 +1176,11 @@ def _bind_expr(DT, e):
     """Expression e of j with its column references bound (_bind); row functions bind theirs in _rowfn_cols."""
     if isinstance(e, ColRef):
         return _bind(DT, e)
+    if isinstance(e, Reducer):
+        for x in (e.arg, getattr(e, "arg2", None)):
+            if isinstance(x, TimePart) or (isinstance(x, ColRef) and isinstance(x.name, _TKey)):
+                raise NotImplementedError(f"a time function as the argument of {e.opname}() is outside the GPU hot "
+                                          f"path")
     if isinstance(e, Reducer) and isinstance(e.arg, ColRef):
         e = copy.copy(e)
         e.arg = _bind(DT, e.arg)
@@ -1121,6 +1203,7 @@ class _Upload:
         self._cache = {}
         self._pending = {}        # name -> (Col in HBM, event of its upload)
         self._pieces = {}         # large value columns travel in pieces, each with its own event (see _late_reduce)
+        keynames = [nm.src if isinstance(nm, _TKey) else nm for nm in keynames]
         needed = list(keynames)
         for e in exprs:
             nm = e.arg.name if isinstance(e, Reducer) and e.arg is not None else getattr(e, "name", None)
@@ -1168,7 +1251,11 @@ class _Upload:
 
     def col(self, name):
         if name not in self._cache:
-            if name in self._pending:
+            if isinstance(name, _TKey):
+                # a derived key: the part of the whole source column in storage order, an int32 column in HBM that
+                # group() then reads like any stored key
+                c = engine.Col(engine.time_part(name.part, self.col(name.src), None), INT32)
+            elif name in self._pending:
                 c, ev = self._pending[name]
                 torch.cuda.current_stream().wait_event(ev)
                 c.data.record_stream(torch.cuda.current_stream())

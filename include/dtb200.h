@@ -490,6 +490,38 @@ DTB_API int dtb_qcut(dtb_col value, int64_t nrows_value, const void* order, cons
 DTB_API int dtb_cut(dtb_col value, int64_t nrows_value, const void* order, int order_is64, int64_t n, int nbins,
                     const double* edges, int64_t nedges, int right_closed, dtb_stream stream, void* out);
 
+/* the parts of dtb_time_part: YearMonthDay_ColumnImpl<1..3> (expr/time/fexpr_year_month_day.cc), DayOfWeek_ColumnImpl
+ * (fexpr_day_of_week.cc), HourMinSec_ColumnImpl<1..4> (fexpr_hour_min_sec.cc) */
+#define DTB_TIME_YEAR         1
+#define DTB_TIME_MONTH        2
+#define DTB_TIME_DAY          3
+#define DTB_TIME_DAY_OF_WEEK  4
+#define DTB_TIME_HOUR         5
+#define DTB_TIME_MINUTE       6
+#define DTB_TIME_SECOND       7
+#define DTB_TIME_NANOSECOND   8
+
+/*
+ * dtb_time_part -- one calendar or clock part of a date32 or time64 column, as dt.time.year() .. nanosecond() compute
+ * it.  The value column (nrows_value rows) is seen through `order`: n positions, int32 row ids or int64 when
+ * order_is64; an index outside [0, nrows_value) is an NA row, as in dtb_gather.  order NULL = the identity, and then n
+ * must be 0 or nrows_value.  NA (INT32_MIN / INT64_MIN) gives NA.
+ *   date32 v (days since 1970-01-01): YEAR / MONTH / DAY of the proleptic Gregorian calendar, DAY_OF_WEEK 1 (Monday)
+ *     .. 7 (Sunday).  Day numbers near the ends of the int32 range wrap in the conversion's int32 adds, as the
+ *     reference's do.
+ *   time64 v (nanoseconds since 1970-01-01T00:00): the four above of the day floor(v / DAY) (the time64 -> date32
+ *     cast; for v < 0 it computes v - (DAY - 1) with int64 wrap-around), and HOUR / MINUTE / SECOND / NANOSECOND
+ *     = ((v mod DAY) / SCALE) % MODULO with the floor modulo, DAY = 86400e9 ns.
+ * out: int32[n], out[p] = the part of the row at position p, NA as INT32_MIN.  Host or device pointers.  Bit-exact.
+ * Asynchronous unless out is host memory.  Arguments are checked in this order, on the host before any CUDA call:
+ * part outside DTB_TIME_YEAR .. DTB_TIME_NANOSECOND: DTB_EINVAL; an stype without a fixed width: DTB_ENOTIMPL; an stype
+ * other than date32 / time64, or a clock part (HOUR .. NANOSECOND) of date32: DTB_EINVAL; n < 0 or nrows_value < 0,
+ * value data NULL while nrows_value > 0, order NULL while 0 < n != nrows_value, out NULL while n > 0: DTB_EINVAL.
+ * n == 0 then returns at once.
+ */
+DTB_API int dtb_time_part(int part, dtb_col value, int64_t nrows_value, const void* order, int order_is64, int64_t n,
+                          dtb_stream stream, void* out);
+
 /*
  * dtb_set_select -- the group-selection step of union / intersect / setdiff / symdiff
  * (set_funcs.cc:126-456).  The caller concatenated K single-column inputs (input k holds the rows
